@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the FlowMap optimisation hot path on B200 (contract: DESIGN.md section 6).
+"""Benchmark of the FlowMap optimisation hot path on H100 (contract: DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--mode scenes|pairs]
 
@@ -321,27 +321,6 @@ def cpu_baseline(sample_frames, steps, warmup, full=True):
             **parts}
 
 
-# ------------------------------------------------------------------------------ ncu evidence
-NCU_SUMMARY = ROOT / "profiles" / "r2_path_ncu_summary.txt"  # tools/ncu_summary.py output, committed
-
-
-def ncu_traffic_from_profiles(path=NCU_SUMMARY):
-    """{op: dram bytes per launch} for the three pixel kernels from the committed ncu summary."""
-    names = {"k_moments_dense": "procrustes_fwd(k_moments)", "k_flow_lean": "flow_loss_fwd_bwd(k_flow_lean)",
-             "k_distribute_dense": "procrustes_bwd(k_distribute)"}
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    out, cur = {}, None
-    if not Path(path).exists():
-        return {}, None
-    for line in Path(path).read_text().splitlines():
-        if line.startswith("====="):
-            cur = next((v for k, v in names.items() if f"::{k}<" in line or f"::{k}(" in line), None)
-        elif cur and ("dram__bytes_read.sum " in line or "dram__bytes_write.sum " in line):
-            parts = line.split()
-            out[cur] = out.get(cur, 0.0) + float(parts[1]) * unit.get(parts[2], 1.0)
-    return out, str(Path(path).relative_to(ROOT))
-
-
 # ------------------------------------------------------------------------------ pair sharding
 def device_shard_inputs(f, h, w, pair_lo, pair_hi, dev):
     """The frames [pair_lo, pair_hi] / pairs [pair_lo, pair_hi) of one synthetic video, generated on
@@ -478,6 +457,27 @@ def sharded_record(f, h, w, full, rank, world, dev, steps, barrier, max_over_ran
                         + (" + pose gather, tracking-sum all-reduce (F x 10 doubles), focal broadcast" if full else "")}
 
 
+DUMP_SAMPLE = 1 << 20  # entries kept of each per-pixel output, at fixed seeded positions
+
+
+def dump_outputs(out_dir, o, last):
+    """Write what the timed path returned in its last step (total loss, relative poses) and the
+    state that step left (intrinsics used, depth and weight logits after Adam) as float32 .npy files
+    under out_dir.  The per-pixel parameters are sampled at DUMP_SAMPLE positions drawn from a fixed
+    seed, so every run and every build writes the same entries (about 8 MB in all)."""
+    import numpy as np
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {"loss": last[0].reshape(1), "relative_poses": last[1], "intrinsics_k4": o.intrinsics_k4()}
+    g = torch.Generator().manual_seed(0)
+    for name, p in (("depth", o.model.backbone.depth), ("weight_logits", o.model.backbone.weights)):
+        flat = p.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(DUMP_SAMPLE, flat.numel()),), generator=g).sort().values
+        arrays[f"{name}_sample"] = flat[idx.to(flat.device)]
+    for name, t in arrays.items():
+        np.save(out / f"{name}.npy", t.detach().float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------ GPU arm
 def run_gpu(args):
     from flowmap_b200 import ops, parallel
@@ -497,6 +497,7 @@ def run_gpu(args):
         dist.init_process_group("nccl", device_id=dev)
     pairs_mode = args.mode in ("pairs", "pairs-full")
     pairs_full = args.mode == "pairs-full"
+    torch.manual_seed(rank)  # the step clock's seed (softmin point subsets) comes from torch's generator
 
     inputs = synthetic_inputs(F_, H_, W_, seed=rank)
     batch = Batch(torch.zeros(1, 1, 1, 1, 1, device=dev).expand(1, F_, 3, H_, W_),
@@ -585,6 +586,8 @@ def run_gpu(args):
     l0 = lib().fm_launch_count()
     ms, last = time_steps(o.training_step, args.steps)
     launches = lib().fm_launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, o, last)
     graph_replay = bool(getattr(o, "_graphs", None))
     if graph_replay:  # replayed graph nodes are not host launches: count the kernels they contain
         launches = launches_per_step * args.steps
@@ -745,7 +748,7 @@ def run_gpu(args):
     if peaks_path.exists():
         peak, peak_src = json.loads(peaks_path.read_text())["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3), not measured"
     n, p_ = H_ * W_, F_ - 1
     ops_bytes = {  # algorithmic bytes per launch: inputs read once, outputs written once
         "procrustes_fwd(k_moments)": n * (4 * F_ + (8 + 4) * p_),
@@ -758,26 +761,19 @@ def run_gpu(args):
     path_ms = t_fwd + t_flow + t_bwd
     path_gbs = algorithmic_bytes(F_, H_, W_) / (path_ms * 1e-3) / 1e9
     dom_gbs = ops_bytes[dom] / (times[dom] * 1e-3) / 1e9
-    # DRAM bytes per launch: parsed from the committed `ncu --set full` summary of these kernels at
-    # this shape (dram__bytes_read.sum + dram__bytes_write.sum); None if the file is missing
-    ncu_traffic, traffic_file = ncu_traffic_from_profiles()
     roofline = {"bound": "hbm", "kernel": dom, "achieved": round(dom_gbs, 1), "peak": peak,
-                "unit": "GB/s", "frac": round(dom_gbs / peak, 4), "traffic": ncu_traffic.get(dom),
+                "unit": "GB/s", "frac": round(dom_gbs / peak, 4),
                 "algorithmic_bytes": ops_bytes[dom],
-                "traffic_source": f"ncu --set full capture of this kernel at this shape ({traffic_file})",
-                "path_traffic": (sum(ncu_traffic.values()) if len(ncu_traffic) == 3 else None),
                 "peak_source": peak_src,
                 "path": {"what": "unproject->Procrustes->reproject->loss+grad (3 ops, summed)",
                          "algorithmic_bytes": algorithmic_bytes(F_, H_, W_),
                          "ms": round(path_ms, 4), "achieved": round(path_gbs, 1),
                          "frac": round(path_gbs / peak, 4)},
                 "ops_ms": {k: round(v, 4) for k, v in times.items()},
-                "note": "k_distribute is bound by L2 RED (atomic add) throughput, k_flow_lean by exposed "
-                        "load latency at 2 CTAs/SM (128 registers), k_moments by L1 gather wavefronts "
-                        "(profiles/README.md); HBM is the denominator the task names"}
+                "note": "algorithmic bytes over CUDA-event kernel time; HBM bandwidth is the denominator"}
 
     # ---- informative: the unmodified reference in its own execution mode, CUDA eager on this same
-    # B200 (flowmap/overfit.py:50,96 hard-code cuda:0) -- what a FlowMap user runs today
+    # GPU (flowmap/overfit.py:50,96 hard-code cuda:0) -- what a FlowMap user runs today
     ref_cuda = None
     if world == 1 and not pairs_mode and reference_available() and os.environ.get("FM_BENCH_SKIP_CPU") != "1":
         try:
@@ -827,7 +823,7 @@ def run_gpu(args):
                                    % (world, F_ - 1, o.reducer.bytes_per_step())) +
                                   (" + pose gather, tracking-sum all-reduce (F x 10 doubles), focal broadcast"
                                    if pairs_full else ""),
-                   "l2": "inputs (1.1 GB) exceed the 126 MB L2, no flush needed",
+                   "l2": "inputs (1.1 GB) exceed the 50 MB L2, no flush needed",
                    "mask_sum": "loop-invariant flow-loss denominator hoisted out of the loop "
                                "(recomputed every step in the e2e leg, where the masks are re-uploaded)"},
         "e2e": {"value": round(world * 1000.0 / e2e_ms, 3), "unit": "it/s",
@@ -861,7 +857,7 @@ def run_gpu(args):
 def run_reference(args):
     """The reference's own CPU implementation of the path: the UNMODIFIED reference modules staged
     under baseline/_ref (baseline/install_ref.py) on the full C3 workload; if they are missing
-    (a checkout that never ran build() next to /root/reference) the oracle port on a bounded
+    (baseline/install_ref.py was not run) the oracle port on a bounded
     sample, labelled as such."""
     if int(os.environ.get("RANK", 0)) != 0:
         return
@@ -900,6 +896,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--mode", default="scenes", choices=["scenes", "pairs", "pairs-full"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

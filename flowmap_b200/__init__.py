@@ -1,4 +1,4 @@
-"""flowmap_b200: B200-native (sm_100a) implementation of FlowMap's per-iteration
+"""flowmap_b200: H100-native (sm_90a) implementation of FlowMap's per-iteration
 optimisation hot path behind the reference's Python surface.  See DESIGN.md."""
 from .types import Batch, Flows, Tracks, BackboneOutput, ModelOutput, ModelExports  # noqa: F401
 

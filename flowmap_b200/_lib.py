@@ -2,7 +2,7 @@
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the
 caller gets an exception.  The library is built in-tree by ``flowmap_b200.build.build()``
-(``nvcc -gencode arch=compute_100a,code=sm_100a``), see ``__graft_entry__.build``.
+(``nvcc -gencode arch=compute_90a,code=sm_90a``), see ``__graft_entry__.build``.
 """
 from __future__ import annotations
 
@@ -131,7 +131,7 @@ def lib() -> ctypes.CDLL:
         if not SO_PATH.exists():
             raise FlowmapLibraryError(
                 f"{SO_PATH} not found: build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a).  flowmap_b200 has no CPU or PyTorch fallback.")
+                "g.build()'` (nvcc, sm_90a).  flowmap_b200 has no CPU or PyTorch fallback.")
         _lib = load_library(SO_PATH)
     return _lib
 

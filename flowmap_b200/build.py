@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library for sm_100a (no torch extension machinery: the
+"""In-tree build of the CUDA library for sm_90a (no torch extension machinery: the
 library is a plain C-ABI .so, see include/flowmap_b200.h)."""
 from __future__ import annotations
 
@@ -9,7 +9,7 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent / "csrc"
 SOURCES = ["fm_kernels.cu", "fm_io.cu"]
 HEADERS = ["fm_math.cuh", "fm_procrustes.cuh", "fm_pixel.cuh", "fm_tiled.cuh", "fm_host.h"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 

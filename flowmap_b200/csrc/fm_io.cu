@@ -1,4 +1,4 @@
-// sm_100a kernels + C ABI for the stages either side of the optimisation hot path (SURVEY 8(f)
+// sm_90a kernels + C ABI for the stages either side of the optimisation hot path (SURVEY 8(f)
 // rank 4): the flow-side preprocessing that builds `Flows` (consistency masks, rescaling) and the
 // point-cloud part of the COLMAP export.  One-off, HBM-bound elementwise work: one thread per
 // output pixel, coalesced stores, gathers through the read-only path.

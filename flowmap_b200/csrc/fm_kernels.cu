@@ -1,4 +1,4 @@
-// sm_100a kernels + C ABI of the FlowMap optimisation hot path (see include/flowmap_b200.h).
+// sm_90a kernels + C ABI of the FlowMap optimisation hot path (see include/flowmap_b200.h).
 //
 // Roofline: everything here is pointwise + reduction work over (frame, H, W) tensors --
 // HBM-bound, no tensor cores.  Per frame pair the algorithmic traffic is 32 B per
@@ -168,8 +168,8 @@ __device__ __forceinline__ void red_add4(float* addr, float a, float b, float c,
 
 // Adds v0 / v1 at columns x0 / x0 + 1 of a row.  With 16-byte aligned rows (ALIGNED) the pair
 // goes out as ONE vector RED on the aligned group of four floats that contains x0 unless it
-// straddles two groups; measured on B200 (tools/red_bench.cu) the padded vector form is
-// 1.5x faster than four scalar REDs for scattered taps.
+// straddles two groups: one RED instruction instead of two for scattered taps (tools/red_bench.cu
+// times the two forms).
 template <bool ALIGNED>
 __device__ __forceinline__ void red_pair(float* row, int x0, int W, float v0, float v1) {
   const int k = x0 & 3;
@@ -250,8 +250,8 @@ __device__ __forceinline__ ItemRange block_item_range(long long total) {
 // The same decomposition applied to each of `rounds` consecutive slices of the item list (all blocks
 // share slice 0, then slice 1, ...).  The gathers / REDs of the Procrustes kernels touch a band of rows
 // around a block's position; with one round the resident blocks sit in as many different places as there
-// are blocks, and at 720p those bands (grid x band x row bytes x 2 arrays) no longer fit the 126 MB L2
-// (k_distribute 2.4 -> 4.5 ms at 150 x 720 x 1280).  With more rounds the blocks advance together through
+// are blocks, and at 720p those bands (grid x band x row bytes x 2 arrays) no longer fit in L2.
+// With more rounds the blocks advance together through
 // a few frame pairs and share their bands.  Blocks are rotated between rounds so that the odd chunk of
 // an uneven split does not always land on the same block.
 __device__ __forceinline__ ItemRange block_item_range(long long total, int rounds, int round) {
@@ -553,11 +553,10 @@ k_flow(const float* __restrict__ depth, const float* __restrict__ k4, const floa
   block_accumulate<kFlowVals>(acc, flowacc + (size_t)frame * kFlowAcc, smem);
 }
 
-// Chunks ahead whose streaming operands k_flow_lean requests into L2 (measured on B200: 0.274 ms
-// without, 0.255 / 0.253 / 0.261 / 0.307 ms at distance 1 / 2 / 4 / 8).
+// Chunks ahead whose streaming operands k_flow_lean requests into L2.
 constexpr int kFlowPrefetchChunks = 2;
 // Lean phase C (constant intrinsics or one shared focal length): see fm_pixel.cuh.  The vector
-// instantiation processes its 4 pixels as two packed float32x2 pairs (FFMA2 / FMUL2 / FADD2).
+// instantiation processes its 4 pixels as two pairs (F2, fm_math.cuh).
 template <int VEC, bool HASF, bool HASB, bool FOCAL>
 __device__ __forceinline__ void flow_frame_body_lean(const FlowFrameLean& f, const float* __restrict__ D,
                                                      const float* __restrict__ ff, const float* __restrict__ mf,
@@ -1302,8 +1301,8 @@ __device__ __forceinline__ SegInfo load_seg(const int* seg, int s) {
 
 // Per-frame record: R (9, row-major, camera-to-world), t (3), c = -R^T t (3), fx fy cx cy ifx ify,
 // 3 pad -- every value stored TWICE in a row (2 * kTrackRec floats per frame), so that an 8-byte
-// shared-memory load yields the (v, v) register pair a packed float32x2 instruction takes as its
-// broadcast operand (rec2), no register moves.  rec1 reads one copy.
+// shared-memory load yields the (v, v) pair the two-wide F2 arithmetic takes as its broadcast
+// operand (rec2), no register moves.  rec1 reads one copy.
 __device__ __forceinline__ void load_segment_frames(float* sm, const float* ext, const float* k4,
                                                     const SegInfo& si) {
   for (int row = threadIdx.x; row < si.rows; row += blockDim.x) {
@@ -1424,8 +1423,8 @@ __device__ __forceinline__ float warp_sum_n(float* v, int lane) {
 
 // One sweep over the (source row, target row, point) triples.  A block of kTrackThreads threads owns
 // (segment, source row, kTrackPoints = 2 * kTrackThreads points): every thread keeps TWO usable source
-// points in registers and evaluates their terms against one target row as ONE packed float32x2
-// computation (FFMA2 / FMUL2 / FADD2: the two points share every target-frame constant; lean_term2 of
+// points in registers and evaluates their terms against one target row as ONE two-wide F2
+// computation (fm_math.cuh: the two points share every target-frame constant; lean_term2 of
 // fm_pixel.cuh is the two-pixel form of the flow kernel's term).  The source-side sums stay in
 // registers; the target-side sums (pose twist and K of the TARGET frame) of one loop iteration belong
 // to one frame for the whole block, so the two points' contributions are added and each warp reduces
@@ -1785,10 +1784,14 @@ k_sweep(const float* __restrict__ depth, const float* __restrict__ k4, const flo
     float rx, ry;
     ray_of(x, y, kb, rx, ry);
     const float p0 = D * rx, p1 = D * ry, p2 = D;
-    const float X0 = T.r[0] * p0 + T.r[1] * p1 + T.r[2] * p2 + T.t[0];
-    const float X1 = T.r[3] * p0 + T.r[4] * p1 + T.r[5] * p2 + T.t[1];
-    const float X2 = T.r[6] * p0 + T.r[7] * p1 + T.r[8] * p2 + T.t[2];
-    const Proj pr = project_point(X0, X1, X2, ka);
+    // The softmin over the candidates' errors amplifies their rounding: the transform and the
+    // projection are rounded per operation, as the reference's float32 ops are (no FMA contraction).
+    const float X0 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T.r[0], p0), __fmul_rn(T.r[1], p1)), __fmul_rn(T.r[2], p2)), T.t[0]);
+    const float X1 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T.r[3], p0), __fmul_rn(T.r[4], p1)), __fmul_rn(T.r[5], p2)), T.t[1]);
+    const float X2 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T.r[6], p0), __fmul_rn(T.r[7], p1)), __fmul_rn(T.r[8], p2)), T.t[2]);
+    Proj pr = project_point(X0, X1, X2, ka);
+    pr.uvx = __fadd_rn(__fmul_rn(ka.fx, pr.u[0]), __fmul_rn(ka.cx, pr.u[2]));
+    pr.uvy = __fadd_rn(__fmul_rn(ka.fy, pr.u[1]), __fmul_rn(ka.cy, pr.u[2]));
     const float ex = (pr.uvx - x) - __ldg(fl + 2 * j), ey = (pr.uvy - y) - __ldg(fl + 2 * j + 1);
     const float w = wt ? weight_of(__ldg(wt + j), wsens) : 1.f;
     const float a = ex * w, b = ey * w;
@@ -2056,9 +2059,8 @@ int blocks_for(int n_items_per_row, int vec) {
   return nb < 1 ? 1 : nb;
 }
 
-// Lanes per row of the warp patch of the dense Procrustes kernels (PatchSite).  Measured on B200 at
-// 150 x 360 x 640, iid flows, fwd / bwd op in ms: strips 0.231 / 0.592, 4 lanes x 8 rows 0.222 / 0.611,
-// 8 x 4 0.227 / 0.564, 16 x 2 0.224 / 0.590 (profiles/README.md).
+// Lanes per row of the warp patch of the dense Procrustes kernels (PatchSite); tools/ab_libs.py
+// compares builds with other values.
 #ifndef FM_PATCH_LANES  // build-time knob for tools/ab_libs.py (0 = strips only)
 #define FM_PATCH_LANES 8
 #endif
@@ -2074,7 +2076,7 @@ int sm_count_cached() {
   static const int n = [] {
     int dev = 0, v = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1)
-      v = 148;
+      v = 132;
     return v;
   }();
   return n;
@@ -2085,18 +2087,16 @@ int persistent_grid(int ctas_per_sm, long long items) {
 }
 
 // Rounds of the dense Procrustes kernels (block_item_range): runs of about kRunChunks chunks per block
-// and round.  Measured on B200 (tools/ab_libs.py): k_distribute_dense (REDs + the fused Adam streams)
-// gains at every shape -- 150 x 720 x 1280: 4.32 ms in one round, 2.47 / 2.44 / 2.69 / 3.73 ms with runs
-// of 4 / 8 / 16 / 32 chunks; 150 x 360 x 640: 0.565 -> 0.553 ms.  k_moments_dense (read-only gathers)
-// gains only once the resident blocks' row bands (sized for flows of a few percent of the image) stop
-// fitting in L2: 1.04 -> 0.95 ms at 720p, but 0.223 -> 0.239 ms at 360 x 640, so it keeps one round there.
+// and round.  k_distribute_dense (REDs + the fused Adam streams) uses rounds at every shape;
+// k_moments_dense (read-only gathers) only once the resident blocks' row bands (sized for flows of a few
+// percent of the image) stop fitting in a third of L2, and keeps one round below that.
 constexpr int kRunChunks = 8;
 int procrustes_rounds(int H, int W, long long items, int grid, bool gathers_only) {
   if (gathers_only) {
     static const double l2_bytes = [] {
       int dev = 0, v = 0;
       if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, dev) != cudaSuccess || v < 1)
-        v = 126 << 20;
+        v = 50 << 20;
       return (double)v;
     }();
     const double band_rows = 0.07 * H + 6.0;
@@ -2191,7 +2191,7 @@ int sm_count() {
   static const int n = [] {
     int dev = 0, v = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1)
-      v = 148;
+      v = 132;
     return v;
   }();
   return n;
@@ -2396,7 +2396,7 @@ static int procrustes_bwd_impl(const float* depth, const float* k4, const float*
   float* weights_rw = const_cast<float*>(weights);
   if (include_flow_loss && flow_scale && !depth_prescaled) {
     // the direct depth gradient already sitting in g_depth was computed for scale 1
-    k_scale_inplace<<<148 * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)BF * H * W);
+    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)BF * H * W);
     FM_CHECK_LAUNCH("fm_procrustes_bwd: k_scale_inplace");
   }
   if (plan) {
@@ -2527,7 +2527,7 @@ int fm_mask_sum(const float* forward_mask, const float* backward_mask, double* o
   if (count == 0) return 0;
   size_t nb = (count / 4 + kThreads * 8 - 1) / (kThreads * 8);
   if (nb < 1) nb = 1;
-  if (nb > 148 * 8) nb = 148 * 8;
+  if (nb > (size_t)sm_count_cached() * 8) nb = (size_t)sm_count_cached() * 8;
   k_mask_sum<<<(unsigned)nb, kThreads, 0, s>>>(forward_mask, backward_mask, out, count);
   FM_CHECK_LAUNCH("fm_mask_sum");
   return 0;
@@ -2588,7 +2588,7 @@ int fm_adam_step_clock(float* param, const float* grad, float* exp_avg, float* e
   if (count == 0) return 0;
   size_t nb = (count / 4 + kThreads * 2 - 1) / (kThreads * 2);
   if (nb < 1) nb = 1;
-  if (nb > 148 * 16) nb = 148 * 16;
+  if (nb > (size_t)sm_count_cached() * 16) nb = (size_t)sm_count_cached() * 16;
   const StepClock* c = (const StepClock*)clock;
   k_adam<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(
       param, grad, exp_avg, exp_avg_sq, count, (float)beta1_d, (float)beta2_d, (float)(1.0 - beta1_d),
@@ -2615,7 +2615,7 @@ int fm_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg
   const float bc2_sqrt = (float)sqrt(bc2);
   size_t nb = (count / 4 + kThreads * 2 - 1) / (kThreads * 2);
   if (nb < 1) nb = 1;
-  if (nb > 148 * 16) nb = 148 * 16;
+  if (nb > (size_t)sm_count_cached() * 16) nb = (size_t)sm_count_cached() * 16;
   k_adam<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(param, grad, exp_avg, exp_avg_sq, count, beta1, beta2, (float)(1.0 - (double)beta1_d), (float)(1.0 - (double)beta2_d), eps, step_size, bc2_sqrt);
   FM_CHECK_LAUNCH("fm_adam_step");
   return 0;
@@ -2987,8 +2987,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
     // two branches of the step (the tracking sweep is issue-bound, the flow kernel waits on memory:
-    // where blocks of both share an SM they fill each other's idle slots; measured 1.889 -> 1.846 ms per
-    // full step on B200, limiting the flow kernel to one block per SM to force the sharing 1.922).
+    // where blocks of both share an SM they fill each other's idle slots).
     SideLane* fwd_lane = a->tracks ? side_lane() : nullptr;
     if (fwd_lane) {
       if ((e = cudaEventRecord(fwd_lane->fork, s)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
@@ -3026,7 +3025,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   const float* tscale = a->phase == FM_STEP_BACKWARD ? a->track_grad_scale : nullptr;
   if (fscale) {  // the direct flow-loss gradient in g_depth was computed for scale 1; scale it before
     // the tracking loss adds its own (differently scaled) part
-    k_scale_inplace<<<148 * 4, kThreads, 0, s>>>(a->g_depth, fscale, (size_t)F * N);
+    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, (size_t)F * N);
     FM_CHECK_LAUNCH("fm_overfit_step: k_scale_inplace");
   }
   const float* g_rt = a->phase == FM_STEP_BACKWARD ? a->g_rt : nullptr;           // the caller's

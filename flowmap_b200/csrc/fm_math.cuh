@@ -2,9 +2,9 @@
 //
 // The CUDA kernels in fm_kernels.cu call these from device code; tests/host_emulation
 // compiles the very same header with g++ to check the analytic gradients against the
-// oracle in a container without a GPU (test infrastructure -- the shipped library has
-// no CPU path).  All semantics follow SURVEY.md Appendix A; citations are to
-// /root/reference/flowmap/...
+// oracle on a machine without a GPU (test infrastructure -- the shipped library has
+// no CPU path).  All semantics follow SURVEY.md Appendix A; citations are to the
+// reference's flowmap/...
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -61,9 +61,10 @@ FM_HD float fm_fma(float a, float b, float c) {
 #endif
 }
 
-// Packed pairs of float32.  sm_100 issues add / mul / fma on two packed float32 per instruction
-// (FADD2 / FMUL2 / FFMA2, `fma.rn.f32x2`): the lean flow kernel processes two neighbouring pixels
-// per lane-pair with these.  On the host (tests/host_emulation) the same code runs component-wise.
+// Pairs of float32: the lean flow kernel processes two neighbouring pixels per lane-pair with
+// these.  sm_90 has no packed float32 instructions, so each operation is two scalar IEEE-rounded
+// ones; the explicit _rn forms keep the compiler from contracting a mul and an add into one FMA,
+// so every component is rounded exactly as the host form (tests/host_emulation) rounds it.
 struct F2 {
   float x, y;
 };
@@ -71,24 +72,21 @@ FM_HD F2 f2(float a, float b) { F2 r; r.x = a; r.y = b; return r; }
 FM_HD F2 f2s(float a) { F2 r; r.x = a; r.y = a; return r; }
 FM_HD F2 f2_fma(F2 a, F2 b, F2 c) {
 #if defined(__CUDA_ARCH__)
-  const float2 r = __ffma2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y), make_float2(c.x, c.y));
-  return f2(r.x, r.y);
+  return f2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 #else
   return f2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 #endif
 }
 FM_HD F2 f2_mul(F2 a, F2 b) {
 #if defined(__CUDA_ARCH__)
-  const float2 r = __fmul2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  return f2(r.x, r.y);
+  return f2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 #else
   return f2(a.x * b.x, a.y * b.y);
 #endif
 }
 FM_HD F2 f2_add(F2 a, F2 b) {
 #if defined(__CUDA_ARCH__)
-  const float2 r = __fadd2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  return f2(r.x, r.y);
+  return f2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #else
   return f2(a.x + b.x, a.y + b.y);
 #endif

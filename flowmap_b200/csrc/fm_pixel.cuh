@@ -287,7 +287,7 @@ FM_HD float flow_pixel_lean(const FlowFrameLean& f, float x, float y, float D, f
 }
 
 // ---------------------------------------------------------------------------------
-// Two-pixel (packed float32x2) form of lean_term / flow_pixel_lean: the two pixels are
+// Two-pixel (F2, fm_math.cuh) form of lean_term / flow_pixel_lean: the two pixels are
 // neighbours in a row, so they share y, the per-frame constants and every control decision
 // except the per-pixel selects (finite test, Huber branch).
 // ---------------------------------------------------------------------------------

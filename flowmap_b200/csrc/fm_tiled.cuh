@@ -1,10 +1,10 @@
-// Tiled, atomic-free form of the Procrustes passes (phase A and phase D), sm_100a.
+// Tiled, atomic-free form of the Procrustes passes (phase A and phase D), sm_90a.
 //
 // Included by fm_kernels.cu (inside its anonymous namespace, after the shared helpers).
 //
 // Why: the backward of align_surfaces (projection.py:235-242) scatters every later-frame
 // pixel's adjoint into four bilinear taps of the earlier frame.  As global REDs that scatter
-// sits on the L2 atomic path (profiles/README.md).  The backward flow -- and with it the whole
+// sits on the L2 atomic path.  The backward flow -- and with it the whole
 // tap pattern -- is LOOP-INVARIANT during an overfit run (flow/__init__.py:23,
 // model_wrapper_overfit.py:44-49), so the scatter matrix B^T (4 entries per source pixel) is
 // transposed ONCE per set of flows into a static "splat plan": for every earlier-frame cell the

@@ -3,7 +3,7 @@ into the ``Flows`` the losses consume (flowmap/flow/flow_predictor.py:40-101).
 
 The predictor networks themselves (RAFT, GMFlow) stay with the reference; any callable
 ``videos (b f 3 h w) -> flow (b f-1 h w 2)`` can be plugged in.  The consistency masks and the
-rescaling run on the sm_100a kernels of csrc/fm_io.cu (no CPU path).
+rescaling run on the sm_90a kernels of csrc/fm_io.cu (no CPU path).
 """
 from __future__ import annotations
 

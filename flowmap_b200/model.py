@@ -2,7 +2,7 @@
 
 Mirrors flowmap/model/model.py:41-110 and the registries of flowmap/model/{backbone,
 intrinsics,extrinsics}/__init__.py with the same class names, cfg dataclasses and
-forward signatures; the bodies call the sm_100a kernels through flowmap_b200.ops.
+forward signatures; the bodies call the sm_90a kernels through flowmap_b200.ops.
 """
 from __future__ import annotations
 

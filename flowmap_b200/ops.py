@@ -1,7 +1,7 @@
 """torch.autograd.Functions over the C ABI (include/flowmap_b200.h).
 
 PyTorch is used for device memory, streams and autograd bookkeeping only; every number
-is produced by the sm_100a kernels in csrc/.  Inputs must be CUDA float32 tensors in the
+is produced by the sm_90a kernels in csrc/.  Inputs must be CUDA float32 tensors in the
 reference's layouts; anything else raises (there is no CPU or eager fallback).
 """
 from __future__ import annotations

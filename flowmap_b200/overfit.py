@@ -142,8 +142,8 @@ class FusedOverfitter(Overfitter):
     use_splat_plan=True selects the DETERMINISTIC backward (ops.SplatPlan, csrc/fm_tiled.cuh): the
     bilinear scatter of the Procrustes adjoint is transposed once per Flows into a static plan and
     evaluated as a gather with TMA-staged windows -- no atomics, bit-reproducible gradients.  It is
-    parity-green but measured ~10 % slower per backward than the default global-RED kernel on
-    B200 (profiles/README.md), hence opt-in."""
+    parity-green but has been slower per backward than the default global-RED kernel
+    (tools/ab_tiled.py compares the two), hence opt-in."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):

@@ -4,7 +4,7 @@ The flow loss is pair-local (SURVEY A.6): pair i needs depth frames i and i+1, i
 weights/flows/masks and the shared focal length.  Rank g therefore owns a contiguous pair
 range [a_g, b_g) and the frames [a_g, b_g]; flows, masks and weights are sharded and
 never move.  Per optimisation step there is one exchange (NCCL over NVLink/NVSwitch on the
-B200 box, gloo in the CPU tests): an all-reduce of [loss, d(focal)] and, grouped with it, a
+GPUs, gloo in the CPU tests): an all-reduce of [loss, d(focal)] and, grouped with it, a
 send/recv of ONE boundary depth-gradient frame with each neighbour (its size does not grow
 with the number of ranks).
 

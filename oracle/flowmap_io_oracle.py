@@ -9,7 +9,7 @@ Parity status: PINNED against outputs of the unmodified reference
 (``tests/golden/make_golden_io.py`` -> ``tests/golden/io_*.npz``, checked by
 ``tests/test_oracle_golden.py``).  Everything is spelled out with index arithmetic instead of
 ``F.grid_sample`` / ``F.interpolate`` so that the sampling rules the CUDA kernels implement
-are explicit.  Citations are relative to /root/reference.
+are explicit.  Citations are relative to the reference checkout.
 """
 
 from __future__ import annotations

@@ -8,7 +8,7 @@ What it is: a plain-PyTorch (CPU, autograd) restatement of the algorithm the ref
 runs every optimisation step (SURVEY.md section 8(a), rows a1-a17).  The reference is pure
 Python on top of ATen, so the restatement is Python on top of ATen as well; it is
 dtype-generic (the reference hard-codes float32, SURVEY A.8 item 13) so the same code
-also serves as the float64 arbiter.  All citations are relative to /root/reference.
+also serves as the float64 arbiter.  All citations are relative to the reference checkout.
 
 Parity status: PINNED.  The reference ships no tests or golden vectors for this path
 (SURVEY section 4), so the pin is against outputs of the reference itself: the script

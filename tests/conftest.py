@@ -1,7 +1,7 @@
 """pytest configuration: the `gpu` marker and shared helpers.
 
 `-m "not gpu"` runs in the build container (no GPU): oracle vs golden vectors, host logic,
-C-ABI symbol checks, world_size-2 gloo tests.  `-m gpu` runs on a B200 and checks the CUDA
+C-ABI symbol checks, world_size-2 gloo tests.  `-m gpu` runs on an H100 and checks the CUDA
 path (called through the C ABI) against the oracle and the golden vectors.
 """
 import sys
@@ -18,7 +18,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100)")
 
 
 def pytest_collection_modifyitems(config, items):

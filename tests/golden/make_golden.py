@@ -1,13 +1,13 @@
 """Generate golden input/output vectors from the UNMODIFIED reference.
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where a checkout of the reference is available (FLOWMAP_REFERENCE names its root):
 
     python tests/golden/make_golden.py            # float32 run of the reference
     python tests/golden/make_golden.py --f64      # float64 run of the same modules
 
 The reference ships no tests or golden vectors for this path (SURVEY.md section 4), so
 these files are the pin for ``oracle/flowmap_oracle.py`` and, through it, for the CUDA
-kernels.  The reference modules are imported from /root/reference as they lie (nothing
+kernels.  The reference modules are imported from that checkout as they lie (nothing
 is copied); only the Lightning shell is restated here (model_wrapper_overfit.py:51-73,
 104-105) because lightning/hydra are not installed.
 
@@ -29,7 +29,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("FLOWMAP_REFERENCE", "reference")
 OUT = Path(__file__).resolve().parent
 
 

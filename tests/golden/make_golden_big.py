@@ -1,6 +1,6 @@
 """Golden vectors at the BENCHMARKED shapes, generated from the UNMODIFIED reference.
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where a checkout of the reference is available (FLOWMAP_REFERENCE names its root):
 
     python tests/golden/make_golden_big.py c3        # 150 x 360 x 640, full loop (~17 GB RSS)
     python tests/golden/make_golden_big.py c2        # 30 x 360 x 480, flow + tracks
@@ -27,7 +27,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("FLOWMAP_REFERENCE", "reference")
 OUT = Path(__file__).resolve().parent
 ROOT = OUT.parent.parent
 sys.path.insert(0, str(ROOT))

@@ -1,5 +1,5 @@
 """Golden vectors for the stages either side of the hot path (flow preprocessing, export),
-generated from the UNMODIFIED reference in the build container:
+generated from the UNMODIFIED reference (FLOWMAP_REFERENCE names the root of its checkout):
 
     python tests/golden/make_golden_io.py
 
@@ -21,7 +21,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("FLOWMAP_REFERENCE", "reference")
 OUT = Path(__file__).resolve().parent
 
 

@@ -135,8 +135,10 @@ def test_emulated_step_matches_reference(emu, name, mapping, focal, npts, lean):
 
 
 @pytest.mark.parametrize("total,rounds,grid", [
-    (33525, 1, 444), (33525, 9, 444), (134100, 37, 444),   # 149 pairs of 360x640 / 720x1280, B200 grid
+    (33525, 1, 444), (33525, 9, 444), (134100, 37, 444),   # 149 pairs of 360x640 / 720x1280, 444 blocks
     (16762, 4, 444),                                        # one rank of an 8-way split at 720p
+    (33525, 1, 396), (33525, 10, 396), (134100, 42, 396),  # the same on the H100 grid (132 SMs x 3)
+    (16762, 5, 396),
     (7, 3, 5), (5, 8, 444), (1000, 1, 1), (4096, 16, 3), (0, 2, 4),
 ])
 def test_item_decomposition_covers_every_item_once_and_is_balanced(emu, total, rounds, grid):

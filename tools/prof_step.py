@@ -1,5 +1,5 @@
 """Profiling driver: the three pixel-parallel ops of one optimisation step at the BASELINE
-shape, called through the C ABI a few times (for ncu; see profiles/README.md)."""
+shape, called through the C ABI a few times (for a profiler run of its own)."""
 import sys
 from pathlib import Path
 

@@ -1,5 +1,5 @@
-// Micro-benchmark: throughput of fire-and-forget float adds (RED) on B200 for the access
-// patterns of the Procrustes-adjoint scatter (tools only; results in profiles/).
+// Micro-benchmark: throughput of fire-and-forget float adds (RED) on the GPU for the access
+// patterns of the Procrustes-adjoint scatter (tools only).
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <vector>
@@ -154,7 +154,7 @@ int main() {
   const char* n2[] = {"2D patch: 4 scalar reds", "2D patch: v4 padded", "2D patch: smem window + v4 flush"};
   float m2[3] = {run2d<0>(buf, H, W, J, frames), run2d<1>(buf, H, W, J, frames), run2d<2>(buf, H, W, J, frames)};
   for (int i = 0; i < 3; ++i) printf("%-32s %8.3f ms  %7.2f Gpx/s\n", n2[i], m2[i], px / m2[i] / 1e6);
-  const int sweep[] = {148, 111, 74, 56, 37, 18};
+  const int sweep[] = {132, 99, 66, 50, 33, 16};
   for (int sms : sweep)
     printf("SMs %3d: scalar jittered %8.3f ms   v4 padded %8.3f ms   aligned v4 %8.3f ms\n", sms,
            run_sms<0>(buf, H, W, J, frames, sms), run_sms<2>(buf, H, W, J, frames, sms), run_sms<4>(buf, H, W, J, frames, sms));
