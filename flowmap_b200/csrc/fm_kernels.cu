@@ -16,7 +16,11 @@
 //                                                  (loss_flow.py:31-70, projection.py:116-184)
 //   k_adjoint      phase D1 pose gradient -> per-pair adjoint constants (SURVEY A.7)
 //   k_distribute   phase D2 per-point adjoints: aligned add into the later frame,
-//                           bilinear scatter into the earlier frame, weight gradient
+//                           bilinear scatter into the earlier frame, weight gradient.  All
+//                           pixels, W % 4 == 0: k_distribute_window, 2-D tiles whose scatter
+//                           is accumulated in a shared-memory window of the earlier frame and
+//                           flushed with coalesced 16-byte REDs; other widths:
+//                           k_distribute_dense, one RED per tap row
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
@@ -777,7 +781,7 @@ __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* _
 
 // ================================================================== phase D2: distribute
 // Optional Adam update of the weight logits inside phase D2 (dense path): their gradient is
-// final there and the kernel is bound by L2 REDs, not HBM, so the 28 B/parameter of a separate
+// final there and the kernel is bound by its scatter, not HBM, so the 28 B/parameter of a separate
 // Adam pass over the weights disappear into it.
 struct AdamFuse {
   float* m; float* v;
@@ -820,7 +824,7 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4,
 #pragma unroll
   for (int k = 0; k < 8; ++k) kacc[k] = 0.f;
 
-  {  // index mode only; all pixels: k_distribute_dense
+  {  // index mode only; all pixels: k_distribute_window / k_distribute_dense
     for (int t = blockIdx.x * kThreads + threadIdx.x; t < num_indices; t += gridDim.x * kThreads) {
       const int j = (int)indices[t];
       const int r = j / W, c = j - r * W;
@@ -838,9 +842,74 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4,
   block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
 }
 
-// Dense (all-pixel) phase D2 on the item decomposition of block_item_range: same per-pixel work as
-// k_distribute's dense branch, per-pair constants re-staged when a block moves on to its next pair.
-template <int VEC, int LX>
+// Per-pixel work of the dense phase D2 for the VEC consecutive pixels of row r from column c0
+// (linear index base in the frame, wi = base + the pair's offset in the weight-shaped arrays): the
+// earlier frame's taps go to `scatter`, the later frame's depth gradient is one aligned RED, then the
+// weight gradient and (fuse_adam) the Adam update of the logits.  The weight-shaped arrays are passed
+// without the pair's offset.
+template <int VEC, typename Scatter>
+__device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairAdjoint& ad, const float* da,
+                                                  const float* db, const float* fl, float* weights, float* gdb,
+                                                  float* g_weights, float wsens, const AdamFuse& adam,
+                                                  bool fuse_adam, long long wi, int base, int r, int c0,
+                                                  Scatter scatter, float* kacc) {
+  auto load_a = [da](int o) { return __ldg(da + o); };
+  float dv[VEC], wv[VEC], wraw[VEC], fv[2 * VEC], gwv[VEC], gdv[VEC];
+  load_vec<VEC>(db + base, dv);
+  load_vec2<VEC>(fl + 2 * base, fv);
+  float* wt = weights ? weights + wi : nullptr;
+  if (wt) {
+    if (VEC == 4) {  // plain (coherent) load: the logits may be updated in place below
+      const float4 w4 = *reinterpret_cast<const float4*>(wt);
+      wraw[0] = w4.x; wraw[1] = w4.y; wraw[2] = w4.z; wraw[3] = w4.w;
+    } else {
+      wraw[0] = *wt;
+    }
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) wv[v] = weight_of(wraw[v], wsens);
+  } else {
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) wv[v] = 1.f;
+  }
+  const float y = pix_coord(r, g.grid.Hf, g.grid.invH);
+#pragma unroll
+  for (int v = 0; v < VEC; ++v)
+    distribute_point(g, ad, pix_coord(c0 + v, g.grid.Wf, g.grid.invW), y, dv[v], wv[v],
+                     fv[2 * v], fv[2 * v + 1], load_a, scatter, gdv[v], gwv[v], kacc);
+  if (VEC == 4) red_add4(gdb + base, gdv[0], gdv[1], gdv[2], gdv[3]);
+  else red_add(gdb + base, gdv[0]);
+  if (wt) {
+    if (wsens != 0.f) {  // chain rule of the sigmoid: d/d logit = sens * w (1 - w) * d/dw
+#pragma unroll
+      for (int v = 0; v < VEC; ++v) gwv[v] *= wsens * wv[v] * (1.0f - wv[v]);
+    }
+    if (g_weights) {
+      if (VEC == 4) *reinterpret_cast<float4*>(g_weights + wi) = make_float4(gwv[0], gwv[1], gwv[2], gwv[3]);
+      else g_weights[wi] = gwv[0];
+    }
+    if (VEC == 4 && fuse_adam) {  // torch.optim.Adam on the logits (k_adam's order)
+      // the step clock's constants are re-read here (L1 hits) rather than held across the pixel loop
+      const float step_size = adam.consts ? __ldg(adam.consts) : adam.step_size;
+      const float bc2_sqrt = adam.consts ? __ldg(adam.consts + 1) : adam.bc2_sqrt;
+      float4 mm = *reinterpret_cast<float4*>(adam.m + wi);
+      float4 vv = *reinterpret_cast<float4*>(adam.v + wi);
+      float* mp = &mm.x; float* vp = &vv.x;
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        mp[v] = mp[v] + adam.omb1 * (gwv[v] - mp[v]);
+        vp[v] = vp[v] * adam.beta2 + adam.omb2 * gwv[v] * gwv[v];
+        wraw[v] = wraw[v] - step_size * (mp[v] / (sqrtf(vp[v]) / bc2_sqrt + adam.eps));
+      }
+      *reinterpret_cast<float4*>(adam.m + wi) = mm;
+      *reinterpret_cast<float4*>(adam.v + wi) = vv;
+      *reinterpret_cast<float4*>(wt) = make_float4(wraw[0], wraw[1], wraw[2], wraw[3]);
+    }
+  }
+}
+
+// Dense (all-pixel) phase D2 for widths that are not a multiple of 4: one pixel per thread on the
+// item decomposition of block_item_range (chunks of kThreads pixels), taps as REDs, per-pair constants
+// re-staged when a block moves on to its next pair.  The weight Adam runs as a separate pass.
 __global__ void __launch_bounds__(kThreads, 3)
 k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4,
                    const float* __restrict__ bflow, float* weights, const PairAdjoint* __restrict__ adj,
@@ -849,11 +918,8 @@ k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   const int N = H * W;
-  constexpr int kChunk = kThreads * VEC;
-  const int chunks = (N + kChunk - 1) / kChunk;
-  const int dr = kChunk / W, dc = kChunk - dr * W;
-  const int tiles_x = LX > 0 ? W / (4 * LX) : 1, tiles = N / 128;
-  if (adam.on && adam.consts) { adam.step_size = __ldg(adam.consts); adam.bc2_sqrt = __ldg(adam.consts + 1); }
+  const int chunks = (N + kThreads - 1) / kThreads;
+  const int dr = kThreads / W, dc = kThreads - dr * W;
 #pragma unroll 1
   for (int round = 0; round < rounds; ++round) {
   const ItemRange range = block_item_range((long long)BP * chunks, rounds, round);
@@ -868,84 +934,154 @@ k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4
     const PairAdjoint ad = s_adj;
     const PairAddr pa = pair_addr(lay, pair, N);
     const PairGeom g = pair_geom(depth, k4, pa, H, W);
-    const int a = pa.k4_frame_a;
     const float* da = opaque_ptr(depth + pa.depth_a);
-    const float* db = da + N;
-    const float* fl = bflow + pa.flow;
-    float* wt = weights ? weights + pa.weight : nullptr;
     float* gda = g_depth + pa.depth_a;
-    auto load_a = [da](int o) { return __ldg(da + o); };
-    auto scatter = [gda, W](int y0, int x0, float v0, float v1) { red_pair<VEC == 4>(gda + y0 * W, x0, W, v0, v1); };
-    float* gdb = gda + N;
-    float* gw = g_weights ? g_weights + pa.weight : nullptr;
-    const bool fuse_adam = VEC == 4 && adam.on && pair >= adam.first_pair;
+    auto scatter = [gda, W](int y0, int x0, float v0, float v1) { red_pair<false>(gda + y0 * W, x0, W, v0, v1); };
     float kacc[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) kacc[k] = 0.f;
-    int base = (cb * kThreads + (int)threadIdx.x) * VEC;
+    int base = cb * kThreads + (int)threadIdx.x;
     int r = base / W, c0 = base - r * W;
 #pragma unroll 1
-    for (int c = cb; c < ce; ++c, base += kChunk) {
-      bool inside = base < N;
-      if constexpr (LX > 0) {
-        const PatchSite<LX> ps = patch_site<LX>(c, W, tiles_x, tiles);
-        base = ps.base; r = ps.r; c0 = ps.c0; inside = ps.inside;
-      }
-      if (inside) {
-        float dv[VEC], wv[VEC], wraw[VEC], fv[2 * VEC], gwv[VEC], gdv[VEC];
-        load_vec<VEC>(db + base, dv);
-        load_vec2<VEC>(fl + 2 * base, fv);
-        if (wt) {
-          if (VEC == 4) {  // plain (coherent) load: the logits may be updated in place below
-            const float4 w4 = *reinterpret_cast<const float4*>(wt + base);
-            wraw[0] = w4.x; wraw[1] = w4.y; wraw[2] = w4.z; wraw[3] = w4.w;
-          } else {
-            wraw[0] = wt[base];
-          }
-#pragma unroll
-          for (int v = 0; v < VEC; ++v) wv[v] = weight_of(wraw[v], wsens);
-        } else {
-#pragma unroll
-          for (int v = 0; v < VEC; ++v) wv[v] = 1.f;
-        }
-        const float y = pix_coord(r, g.grid.Hf, g.grid.invH);
-#pragma unroll
-        for (int v = 0; v < VEC; ++v)
-          distribute_point(g, ad, pix_coord(c0 + v, g.grid.Wf, g.grid.invW), y, dv[v], wv[v],
-                           fv[2 * v], fv[2 * v + 1], load_a, scatter, gdv[v], gwv[v], kacc);
-        if (VEC == 4) red_add4(gdb + base, gdv[0], gdv[1], gdv[2], gdv[3]);
-        else red_add(gdb + base, gdv[0]);
-        if (wt) {
-          if (wsens != 0.f) {  // chain rule of the sigmoid: d/d logit = sens * w (1 - w) * d/dw
-#pragma unroll
-            for (int v = 0; v < VEC; ++v) gwv[v] *= wsens * wv[v] * (1.0f - wv[v]);
-          }
-          if (gw) {
-            if (VEC == 4) *reinterpret_cast<float4*>(gw + base) = make_float4(gwv[0], gwv[1], gwv[2], gwv[3]);
-            else gw[base] = gwv[0];
-          }
-          if (fuse_adam) {  // torch.optim.Adam on the logits (k_adam's order)
-            float4 mm = *reinterpret_cast<float4*>(adam.m + pa.weight + base);
-            float4 vv = *reinterpret_cast<float4*>(adam.v + pa.weight + base);
-            float* mp = &mm.x; float* vp = &vv.x;
-#pragma unroll
-            for (int v = 0; v < 4; ++v) {
-              mp[v] = mp[v] + adam.omb1 * (gwv[v] - mp[v]);
-              vp[v] = vp[v] * adam.beta2 + adam.omb2 * gwv[v] * gwv[v];
-              wraw[v] = wraw[v] - adam.step_size * (mp[v] / (sqrtf(vp[v]) / adam.bc2_sqrt + adam.eps));
-            }
-            *reinterpret_cast<float4*>(adam.m + pa.weight + base) = mm;
-            *reinterpret_cast<float4*>(adam.v + pa.weight + base) = vv;
-            *reinterpret_cast<float4*>(wt + base) = make_float4(wraw[0], wraw[1], wraw[2], wraw[3]);
-          }
-        }
-      }
+    for (int c = cb; c < ce; ++c, base += kThreads) {
+      if (base < N)
+        distribute_pixels<1>(g, ad, da, da + N, bflow + pa.flow, weights, gda + N, g_weights, wsens, adam, false,
+                             pa.weight + base, base, r, c0, scatter, kacc);
       r += dr; c0 += dc;
       if (c0 >= W) { c0 -= W; ++r; }
     }
     // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
-    block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
+    block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
     i += ce - cb;
+  }
+  }
+}
+
+// Tile and halo of k_distribute_window (build-time knobs for tools/ab_libs.py).  With the defaults
+// 0.04 % of the tap rows of N(0, 0.01^2) flows (6.4 x 3.6 px at 640 x 360) miss the window
+// (tools/window_fallback.py).
+#ifndef FM_WIN_TW
+#define FM_WIN_TW 64
+#endif
+#ifndef FM_WIN_TH
+#define FM_WIN_TH 32
+#endif
+#ifndef FM_WIN_HX
+#define FM_WIN_HX 16
+#endif
+#ifndef FM_WIN_HY
+#define FM_WIN_HY 12
+#endif
+#ifndef FM_WIN_CTAS  // resident blocks per SM (register cap: 80 at 3, 128 at 2)
+#define FM_WIN_CTAS 3
+#endif
+constexpr int kWinTW = FM_WIN_TW, kWinTH = FM_WIN_TH;      // tile of the later frame
+constexpr int kWinW = kWinTW + 2 * FM_WIN_HX, kWinH = kWinTH + 2 * FM_WIN_HY;  // window of the earlier frame
+// A tap pair (x0, x0 + 1) goes to the window when x0 is inside it, so x0 + 1 may be one column past
+// it: each row has one more aligned group, flushed like the others where it lies inside the image.
+constexpr int kWinPitch = kWinW + 4;
+constexpr int kWinRowThreads = kWinTW / 4, kWinRowsPerPass = kThreads / kWinRowThreads;
+static_assert(kWinTW % 4 == 0 && FM_WIN_HX % 2 == 0 && kThreads % kWinRowThreads == 0 &&
+              kWinTH % kWinRowsPerPass == 0 && kWinTW % 16 == 0 && kWinTH % 8 == 0, "window geometry");
+static_assert(kWinH * kWinPitch * 4 + 8 * (kThreads / 32) * 8 + (int)sizeof(PairAdjoint) <= 48 * 1024,
+              "static shared memory");
+
+// Dense phase D2 for W % 4 == 0.  Work unit: a kWinTW x kWinTH tile of the later frame (a thread owns
+// 4 consecutive pixels of a row), walked with the rounds of block_item_range.  The taps into the earlier
+// frame's depth gradient are added with shared-memory float atomics into a window of that frame: the
+// tile plus a halo, shifted by the mean backward flow of the tile and clamped onto the image, with a
+// 16-byte aligned x origin.  Taps outside the window are REDs as in k_distribute_dense.  After the
+// tile the window is flushed with aligned vector REDs (not stores: neighbouring windows overlap, and
+// k_track_apply adds into the same gradient concurrently in fm_overfit_step) and zeroed.  This replaces
+// ~2.6 scattered 32-byte RED requests per pixel (bound by the L2 atomic units) with ~0.7 coalesced ones.
+__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
+k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k4,
+                    const float* __restrict__ bflow, float* weights, const PairAdjoint* __restrict__ adj,
+                    float* __restrict__ g_depth, float* __restrict__ g_weights, double* __restrict__ k4acc,
+                    float wsens, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
+  __shared__ double smem[8 * (kThreads / 32)];
+  __shared__ PairAdjoint s_adj;
+  __shared__ PairGeom s_geom;
+  __shared__ __align__(16) float win[kWinH * kWinPitch];
+  const int N = H * W;
+  const int tiles_x = (W + kWinTW - 1) / kWinTW, tiles = tiles_x * ((H + kWinTH - 1) / kWinTH);
+  const int lane = threadIdx.x & 31;
+  for (int k = threadIdx.x; k < kWinH * kWinPitch / 4; k += kThreads)
+    reinterpret_cast<float4*>(win)[k] = make_float4(0.f, 0.f, 0.f, 0.f);  // barrier: the s_adj staging
+#pragma unroll 1
+  for (int round = 0; round < rounds; ++round) {
+  const ItemRange range = block_item_range((long long)BP * tiles, rounds, round);
+#pragma unroll 1
+  for (int i = range.i0; i < range.i1;) {
+    const int pair = i / tiles, tb = i - pair * tiles;
+    const int te = (tb + (range.i1 - i) < tiles) ? tb + (range.i1 - i) : tiles;
+    __syncthreads();  // the previous pair's s_adj is no longer read
+    const PairAddr pa = pair_addr(lay, pair, N);
+    if (threadIdx.x < sizeof(PairAdjoint) / 4)
+      reinterpret_cast<float*>(&s_adj)[threadIdx.x] = reinterpret_cast<const float*>(adj + pair)[threadIdx.x];
+    if (threadIdx.x == 32) s_geom = pair_geom(depth, k4, pa, H, W);
+    __syncthreads();
+    // the pair's constants are read from shared memory: as register copies they more than double the
+    // spills of the pixel loop at the 80 registers of 3 blocks per SM
+    const PairAdjoint& ad = s_adj;
+    const PairGeom& g = s_geom;
+    const float* da = opaque_ptr(depth + pa.depth_a);
+    const float* fl = bflow + pa.flow;
+    float* gda = g_depth + pa.depth_a;
+    const bool fuse_adam = adam.on && pair >= adam.first_pair;
+    float kacc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) kacc[k] = 0.f;
+#pragma unroll 1
+    for (int t = tb; t < te; ++t) {
+      const int ty = t / tiles_x, X0 = (t - ty * tiles_x) * kWinTW, Y0 = ty * kWinTH;
+      // Window shift: the mean backward flow of 8 x 4 samples spread over the tile (every warp sums the
+      // same samples in the same order, so all warps place the window identically).  A single sample
+      // would move the window by the flow's own noise.
+      float sx, sy;
+      {
+        const int sr = min(Y0 + (lane >> 3) * (kWinTH / 4) + kWinTH / 8, H - 1);
+        const int sc = min(X0 + (lane & 7) * (kWinTW / 8) + kWinTW / 16, W - 1);
+        const float2 f = __ldg(reinterpret_cast<const float2*>(fl) + sr * W + sc);
+        sx = warp_sum_f(f.x);
+        sy = warp_sum_f(f.y);
+      }
+      // the taps of column c lie around c + W flx - .5 (bilinear_taps); clamped first so that a
+      // non-finite flow cannot overflow the integer
+      const int shx = __float2int_rn(fminf(fmaxf(sx * (g.grid.Wf / 32.f) - 0.5f, -g.grid.Wf), g.grid.Wf));
+      const int shy = __float2int_rn(fminf(fmaxf(sy * (g.grid.Hf / 32.f) - 0.5f, -g.grid.Hf), g.grid.Hf));
+      const int wx0 = max(0, min((X0 - FM_WIN_HX + shx + 2) & ~3, W - kWinW));
+      const int wy0 = max(0, min(Y0 - FM_WIN_HY + shy, H - kWinH));
+      auto scatter = [=](int y0, int x0, float v0, float v1) {
+        const unsigned ly = (unsigned)(y0 - wy0), lx = (unsigned)(x0 - wx0);
+        if (ly < (unsigned)kWinH && lx < (unsigned)kWinW) {
+          float* s = win + ly * kWinPitch + lx;
+          atomicAdd(s, v0);
+          atomicAdd(s + 1, v1);
+        } else {
+          red_pair<true>(gda + y0 * W, x0, W, v0, v1);
+        }
+      };
+      const int c0 = X0 + 4 * ((int)threadIdx.x % kWinRowThreads);
+#pragma unroll 1
+      for (int r = Y0 + (int)threadIdx.x / kWinRowThreads; r < Y0 + kWinTH; r += kWinRowsPerPass)
+        if (r < H && c0 < W)
+          distribute_pixels<4>(g, ad, da, da + N, fl, weights, gda + N, g_weights, wsens, adam, fuse_adam,
+                               pa.weight + r * W + c0, r * W + c0, r, c0, scatter, kacc);
+      __syncthreads();
+      for (int k = threadIdx.x; k < kWinH * (kWinPitch / 4); k += kThreads) {
+        const int ly = k / (kWinPitch / 4), lx = (k - ly * (kWinPitch / 4)) * 4;
+        float4* s = reinterpret_cast<float4*>(win) + k;
+        const float4 v = *s;
+        *s = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (wy0 + ly < H && wx0 + lx < W && (v.x != 0.f || v.y != 0.f || v.z != 0.f || v.w != 0.f))
+          red_add4(gda + (wy0 + ly) * W + wx0 + lx, v.x, v.y, v.z, v.w);
+      }
+      __syncthreads();  // the window is zero again before the next tile's taps
+    }
+    // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
+    block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
+    i += te - tb;
   }
   }
 }
@@ -2087,7 +2223,7 @@ int persistent_grid(int ctas_per_sm, long long items) {
 }
 
 // Rounds of the dense Procrustes kernels (block_item_range): runs of about kRunChunks chunks per block
-// and round.  k_distribute_dense (REDs + the fused Adam streams) uses rounds at every shape;
+// and round.  The dense phase-D2 kernels (REDs + the fused Adam streams) use rounds at every shape;
 // k_moments_dense (read-only gathers) only once the resident blocks' row bands (sized for flows of a few
 // percent of the image) stop fitting in a third of L2, and keeps one round below that.
 constexpr int kRunChunks = 8;
@@ -2418,18 +2554,15 @@ static int procrustes_bwd_impl(const float* depth, const float* k4, const float*
   if (indices) {
     dim3 grid(blocks_for_points(num_indices), BP);
     k_distribute<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
-  } else if (patch_shape_ok(H, W)) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_distribute_dense<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items, pg, false));
   } else if (W % 4 == 0) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_distribute_dense<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items, pg, false));
+    const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
+    const int pg = persistent_grid(FM_WIN_CTAS, items);
+    const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);  // rounds are sized in 1024-pixel chunks
+    k_distribute_window<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
   } else {
     const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
     const int pg = persistent_grid(3, items);
-    k_distribute_dense<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
+    k_distribute_dense<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
   }
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
   k_k4_finalize<<<(BF + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, B, F);

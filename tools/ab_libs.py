@@ -3,7 +3,8 @@ files, e.g. with -D knobs, instead of living behind run-time switches in the pro
 
   python tools/ab_libs.py flowmap_b200/csrc/ab/base.so flowmap_b200/csrc/ab/x.so ... [--no-step]
 
-Building a variant (the knobs are `#ifndef` defaults in csrc/fm_kernels.cu, e.g. FM_PATCH_LANES):
+Building a variant (the knobs are `#ifndef` defaults in csrc/fm_kernels.cu, e.g. FM_PATCH_LANES or
+the FM_WIN_* tile / halo / blocks-per-SM of k_distribute_window):
 
   cd flowmap_b200/csrc && mkdir -p ab && nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 \
       --expt-extended-lambda -Xcompiler -fPIC -shared -DFM_PATCH_LANES=4 -o ab/lanes4.so fm_kernels.cu fm_io.cu
