@@ -983,17 +983,44 @@ constexpr int kWinPitch = kWinW + 4;
 constexpr int kWinRowThreads = kWinTW / 4, kWinRowsPerPass = kThreads / kWinRowThreads;
 static_assert(kWinTW % 4 == 0 && FM_WIN_HX % 2 == 0 && kThreads % kWinRowThreads == 0 &&
               kWinTH % kWinRowsPerPass == 0 && kWinTW % 16 == 0 && kWinTH % 8 == 0, "window geometry");
-static_assert(kWinH * kWinPitch * 4 + 8 * (kThreads / 32) * 8 + (int)sizeof(PairAdjoint) <= 48 * 1024,
+// The window holds fixed-point sums (fix_encode in fm_math.cuh) in two int32 planes, hi and lo.
+// They cannot overflow: a pixel adds to a given cell at most once (its four taps are distinct
+// cells; a bottom tap row clamped onto the top one carries weight 0, and zero values are not added), so a cell
+// receives at most kWinTW * kWinTH = 2048 nonzero adds per tile, each with |hi| <= 2^19 and
+// lo in [0, 2^16]: |sum hi| <= 2^30 and sum lo <= 2^27.
+static_assert(kWinTW * kWinTH <= 2048, "fixed-point window sums would overflow int32");
+static_assert(2 * kWinH * kWinPitch * 4 + 8 * (kThreads / 32) * 8 + (int)sizeof(PairAdjoint) +
+                  (int)sizeof(PairGeom) + 8 <= 48 * 1024,
               "static shared memory");
+
+#ifdef FM_WIN_COUNT  // counting build: tap rows {in the window, out of fixed-point range, outside the window}
+__device__ unsigned long long fm_win_counts[3];
+#define FM_WIN_TALLY(i) atomicAdd(&fm_win_counts[i], 1ull)
+}  // namespace
+// copies the counts to out[3] and resets them (tools/window_counts.py); exported, so outside the
+// anonymous namespace
+extern "C" int fm_window_counts(unsigned long long* out) {
+  static const unsigned long long zero[3] = {0, 0, 0};
+  if (cudaMemcpyFromSymbol(out, fm_win_counts, sizeof(zero)) != cudaSuccess) return 1;
+  return cudaMemcpyToSymbol(fm_win_counts, zero, sizeof(zero)) == cudaSuccess ? 0 : 1;
+}
+namespace {
+#else
+#define FM_WIN_TALLY(i)
+#endif
 
 // Dense phase D2 for W % 4 == 0.  Work unit: a kWinTW x kWinTH tile of the later frame (a thread owns
 // 4 consecutive pixels of a row), walked with the rounds of block_item_range.  The taps into the earlier
-// frame's depth gradient are added with shared-memory float atomics into a window of that frame: the
-// tile plus a halo, shifted by the mean backward flow of the tile and clamped onto the image, with a
-// 16-byte aligned x origin.  Taps outside the window are REDs as in k_distribute_dense.  After the
-// tile the window is flushed with aligned vector REDs (not stores: neighbouring windows overlap, and
-// k_track_apply adds into the same gradient concurrently in fm_overfit_step) and zeroed.  This replaces
-// ~2.6 scattered 32-byte RED requests per pixel (bound by the L2 atomic units) with ~0.7 coalesced ones.
+// frame's depth gradient are added into a window of that frame in shared memory: the tile plus a halo,
+// shifted by the mean backward flow of the tile and clamped onto the image, with a 16-byte aligned x
+// origin.  The window sums in fixed point with native 32-bit integer shared-memory atomics (float
+// atomics on shared memory are compare-and-swap loops on sm_90a), at a power-of-two scale chosen per
+// pair from its constants (tap_magnitude).  Taps outside the window, and values outside the
+// fixed-point range (including non-finite ones), are float REDs as in k_distribute_dense.  After the
+// tile the window is converted back to float and flushed with aligned vector REDs (not stores:
+// neighbouring windows overlap, and k_track_apply adds into the same gradient concurrently in
+// fm_overfit_step) and zeroed.  This replaces ~2.6 scattered 32-byte RED requests per pixel (bound by
+// the L2 atomic units) with ~0.7 coalesced ones.
 __global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
 k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k4,
                     const float* __restrict__ bflow, float* weights, const PairAdjoint* __restrict__ adj,
@@ -1002,12 +1029,16 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   __shared__ PairGeom s_geom;
-  __shared__ __align__(16) float win[kWinH * kWinPitch];
+  __shared__ float s_fix[2];  // the pair's fixed-point scale 2^e and its inverse
+  __shared__ __align__(16) int win_hi[kWinH * kWinPitch];
+  __shared__ __align__(16) int win_lo[kWinH * kWinPitch];
   const int N = H * W;
   const int tiles_x = (W + kWinTW - 1) / kWinTW, tiles = tiles_x * ((H + kWinTH - 1) / kWinTH);
   const int lane = threadIdx.x & 31;
-  for (int k = threadIdx.x; k < kWinH * kWinPitch / 4; k += kThreads)
-    reinterpret_cast<float4*>(win)[k] = make_float4(0.f, 0.f, 0.f, 0.f);  // barrier: the s_adj staging
+  for (int k = threadIdx.x; k < kWinH * kWinPitch / 4; k += kThreads) {  // barrier: the s_adj staging
+    reinterpret_cast<int4*>(win_hi)[k] = make_int4(0, 0, 0, 0);
+    reinterpret_cast<int4*>(win_lo)[k] = make_int4(0, 0, 0, 0);
+  }
 #pragma unroll 1
   for (int round = 0; round < rounds; ++round) {
   const ItemRange range = block_item_range((long long)BP * tiles, rounds, round);
@@ -1019,7 +1050,13 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
     const PairAddr pa = pair_addr(lay, pair, N);
     if (threadIdx.x < sizeof(PairAdjoint) / 4)
       reinterpret_cast<float*>(&s_adj)[threadIdx.x] = reinterpret_cast<const float*>(adj + pair)[threadIdx.x];
-    if (threadIdx.x == 32) s_geom = pair_geom(depth, k4, pa, H, W);
+    if (threadIdx.x == 32) {
+      const PairGeom pg = pair_geom(depth, k4, pa, H, W);
+      s_geom = pg;
+      const int e = fix_exponent(tap_magnitude(adj[pair], pg));
+      s_fix[0] = fix_pow2(e);
+      s_fix[1] = fix_pow2(-e);
+    }
     __syncthreads();
     // the pair's constants are read from shared memory: as register copies they more than double the
     // spills of the pixel loop at the 80 registers of 3 blocks per SM
@@ -1054,11 +1091,18 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
       const int wy0 = max(0, min(Y0 - FM_WIN_HY + shy, H - kWinH));
       auto scatter = [=](int y0, int x0, float v0, float v1) {
         const unsigned ly = (unsigned)(y0 - wy0), lx = (unsigned)(x0 - wx0);
-        if (ly < (unsigned)kWinH && lx < (unsigned)kWinW) {
-          float* s = win + ly * kWinPitch + lx;
-          atomicAdd(s, v0);
-          atomicAdd(s + 1, v1);
+        const bool inside = (ly < (unsigned)kWinH) & (lx < (unsigned)kWinW);
+        int h0, l0, h1, l1;
+        const float fix_s = s_fix[0];  // an LDS per call: one register fewer across the pixel loop
+        if (inside & fix_encode(v0, fix_s, h0, l0) & fix_encode(v1, fix_s, h1, l1)) {
+          FM_WIN_TALLY(0);
+          const int o = ly * kWinPitch + lx;
+          if (h0 != 0) atomicAdd(win_hi + o, h0);
+          if (l0 != 0) atomicAdd(win_lo + o, l0);
+          if (h1 != 0) atomicAdd(win_hi + o + 1, h1);
+          if (l1 != 0) atomicAdd(win_lo + o + 1, l1);
         } else {
+          FM_WIN_TALLY(inside ? 1 : 2);
           red_pair<true>(gda + y0 * W, x0, W, v0, v1);
         }
       };
@@ -1069,13 +1113,17 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
           distribute_pixels<4>(g, ad, da, da + N, fl, weights, gda + N, g_weights, wsens, adam, fuse_adam,
                                pa.weight + r * W + c0, r * W + c0, r, c0, scatter, kacc);
       __syncthreads();
+      const float inv_s = s_fix[1];
       for (int k = threadIdx.x; k < kWinH * (kWinPitch / 4); k += kThreads) {
         const int ly = k / (kWinPitch / 4), lx = (k - ly * (kWinPitch / 4)) * 4;
-        float4* s = reinterpret_cast<float4*>(win) + k;
-        const float4 v = *s;
-        *s = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (wy0 + ly < H && wx0 + lx < W && (v.x != 0.f || v.y != 0.f || v.z != 0.f || v.w != 0.f))
-          red_add4(gda + (wy0 + ly) * W + wx0 + lx, v.x, v.y, v.z, v.w);
+        int4* sh = reinterpret_cast<int4*>(win_hi) + k;
+        int4* sl = reinterpret_cast<int4*>(win_lo) + k;
+        const int4 h = *sh, l = *sl;
+        *sh = make_int4(0, 0, 0, 0);
+        *sl = make_int4(0, 0, 0, 0);
+        if (wy0 + ly < H && wx0 + lx < W && ((h.x | h.y | h.z | h.w | l.x | l.y | l.z | l.w) != 0))
+          red_add4(gda + (wy0 + ly) * W + wx0 + lx, fix_decode(h.x, l.x, inv_s), fix_decode(h.y, l.y, inv_s),
+                   fix_decode(h.z, l.z, inv_s), fix_decode(h.w, l.w, inv_s));
       }
       __syncthreads();  // the window is zero again before the next tile's taps
     }

@@ -8,6 +8,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <string.h>
 
 #if defined(__CUDACC__)
 #define FM_HD __host__ __device__ __forceinline__
@@ -188,6 +189,62 @@ FM_HD int floor_pos(float v, float& frac, float& fl) {
 #else
   return (int)fl;
 #endif
+}
+
+// ---------------------------------------------------------------------------------
+// Fixed-point accumulation in two int32 channels (the shared-memory scatter window of
+// k_distribute_window: 32-bit integer adds are native shared-memory atomics on sm_90, float adds
+// are compare-and-swap loops).  A value v is represented by x = v * 2^e rounded to an integer
+// x = hi * 2^16 + lo, |hi| < 2^19, lo in [0, 2^16].  The exponent e is chosen per frame pair so
+// that an estimate T of the pair's largest value maps to [2^23, 2^24): values with |v| >= T are
+// then encoded exactly as float32 rounds them, smaller ones within half a float32 ulp at T (one
+// unit 2^-e; a negative x above -2^16 is rounded twice, which adds at most 2^-9 of a unit).  Sums
+// of the integers are exact and independent of the order of the adds.
+// ---------------------------------------------------------------------------------
+constexpr float kFixLimit = 34359738368.0f;  // 2^35: |x| below this encodes, anything else falls back
+
+// e with T * 2^e in [2^23, 2^24), clamped so that 2^e and 2^-e are normal floats.  T <= 0 or
+// non-finite gives e = 0 (then every value is 0 or takes the fall-back).
+FM_HD int fix_exponent(float T) {
+  if (!(T > 0.0f && T <= 3.0e38f)) return 0;
+  int ex;
+  frexpf(T, &ex);  // T = m 2^ex, m in [.5, 1)
+  const int e = 24 - ex;
+  return e < -120 ? -120 : (e > 120 ? 120 : e);
+}
+
+// 2^e as a float for |e| <= 126.
+FM_HD float fix_pow2(int e) {
+  const uint32_t bits = (uint32_t)(127 + e) << 23;
+  float f;
+  memcpy(&f, &bits, 4);
+  return f;
+}
+
+// Encodes v with scale s = 2^e.  Returns false (hi = lo = 0) when |v s| >= 2^35 or v is not
+// finite: the caller adds such a value as a float.  Branch-free, so that the kernel keeps hi / lo
+// in registers.  Both roundings run on the FP32 add pipe as in floor_pos: hi = floor(x / 2^16) (an
+// exact integer x / 2^16 may give hi one lower, with lo = 2^16), lo = rint(x - hi 2^16).
+FM_HD bool fix_encode(float v, float s, int& hi, int& lo) {
+  const bool ok = fabsf(v * s) < kFixLimit;
+  const float x = ok ? v * s : 0.0f;
+  const float magic = 12582912.0f;  // 1.5 * 2^23
+  const float mh = (x * (1.0f / 65536.0f) - 0.5f) + magic;  // |x / 2^16 - .5| < 2^22
+  const float fh = mh - magic;
+  const float ml = (x - fh * 65536.0f) + magic;
+#if defined(__CUDA_ARCH__)
+  hi = __float_as_int(mh) - 0x4B400000;
+  lo = __float_as_int(ml) - 0x4B400000;
+#else
+  hi = (int)fh;
+  lo = (int)(ml - magic);
+#endif
+  return ok;
+}
+
+// Sum of encoded values -> float with one rounding (the product with 2^-e is exact).
+FM_HD float fix_decode(int hi, int lo, float inv_s) {
+  return (float)((long long)hi * 65536 + lo) * inv_s;
 }
 
 FM_HD Taps bilinear_taps(float ex, float ey, const GridDims& g) {

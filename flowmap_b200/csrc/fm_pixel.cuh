@@ -501,6 +501,23 @@ FM_HD void distribute_point(const PairGeom& g, const PairAdjoint& ad, float x, f
   kacc[3] -= ea1 * qz_true;
 }
 
+// Order of magnitude of the largest tap value distribute_point scatters for a pair, from its
+// constants alone (an estimate, not a bound): a tap value is a bilinear weight times
+// qb . (rx, ry, 1) with qb = w (Cbar dp + ad.qb), w <= 1, |dp| of the order of the depth times a
+// ray (the centre depth z0 stands in for the depth), and no ray component larger than R, the
+// largest over the image of either frame.
+FM_HD float ray_bound(const Cam& k) {
+  return fmaxf(fmaxf(fabsf(k.cx), fabsf(1.0f - k.cx)) * fabsf(k.ifx),
+               fmaxf(fabsf(k.cy), fabsf(1.0f - k.cy)) * fabsf(k.ify));
+}
+FM_HD float tap_magnitude(const PairAdjoint& ad, const PairGeom& g) {
+  float c = 0.0f, q = 0.0f;
+  for (int i = 0; i < 9; ++i) c = fmaxf(c, fabsf(ad.cbar[i]));
+  for (int i = 0; i < 3; ++i) q = fmaxf(q, fabsf(ad.qb[i]));
+  const float R = fmaxf(1.0f, fmaxf(ray_bound(g.ka), ray_bound(g.kb)));
+  return R * (3.0f * c * fabsf(g.z0) * R + q);
+}
+
 }  // namespace fm
 
 // ---------------------------------------------------------------------------------
