@@ -1454,7 +1454,7 @@ k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m
 // The loss is sum / count with a count that depends on the PREDICTED positions, so the
 // gradient scale is only known after a full pass.  Everything is therefore accumulated
 // unscaled in ONE sweep over the (source, target, point) triples and scaled at the end:
-//   k_track_src     block = (segment, source row, point chunk): bilinear-sample xyz at the track
+//   k_track_src     work item = (segment, source row, half of its points): bilinear-sample xyz at the track
 //                   location, lift to world space, loop over the segment's target rows:
 //                   loss sum + valid count, the unscaled camera-space adjoint of the sampled
 //                   point (stored per sample), source-frame K / pose-twist sums in registers,
@@ -1484,14 +1484,13 @@ __device__ __forceinline__ SegInfo load_seg(const int* seg, int s) {
 }
 
 // Per-frame record: R (9, row-major, camera-to-world), t (3), c = -R^T t (3), fx fy cx cy ifx ify,
-// 3 pad -- every value stored TWICE in a row (2 * kTrackRec floats per frame), so that an 8-byte
-// shared-memory load yields the (v, v) pair the two-wide F2 arithmetic takes as its broadcast
-// operand (rec2), no register moves.  rec1 reads one copy.
+// 3 pad -- kTrackRec floats, 16-byte aligned, so that a warp reads a record with six broadcast
+// 16-byte shared-memory loads (TrackRec).
 __device__ __forceinline__ void load_segment_frames(float* sm, const float* ext, const float* k4,
                                                     const SegInfo& si) {
   for (int row = threadIdx.x; row < si.rows; row += blockDim.x) {
     const float* P = ext + (size_t)(si.start_frame + row) * 16;
-    float* o = sm + row * 2 * kTrackRec;
+    float* o = sm + row * kTrackRec;
     float v[kTrackRec];
     float* R = v;
     float* t = v + 9;
@@ -1507,41 +1506,25 @@ __device__ __forceinline__ void load_segment_frames(float* sm, const float* ext,
     v[15] = k.x; v[16] = k.y; v[17] = k.z; v[18] = k.w; v[19] = 1.0f / k.x; v[20] = 1.0f / k.y;
     v[21] = v[22] = v[23] = 0.f;
 #pragma unroll
-    for (int i = 0; i < kTrackRec; ++i) reinterpret_cast<float2*>(o)[i] = make_float2(v[i], v[i]);
+    for (int i = 0; i < kTrackRec / 4; ++i)
+      reinterpret_cast<float4*>(o)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
   }
   __syncthreads();
 }
-__device__ __forceinline__ float rec1(const float* rec, int i) { return rec[2 * i]; }
-__device__ __forceinline__ F2 rec2(const float* rec, int i) {
-  const float2 v = reinterpret_cast<const float2*>(rec)[i];
-  return f2(v.x, v.y);
-}
-__device__ __forceinline__ Cam sm_cam(const float* rec) {
-  Cam c;
-  c.fx = rec1(rec, 15); c.fy = rec1(rec, 16); c.cx = rec1(rec, 17); c.cy = rec1(rec, 18);
-  c.ifx = rec1(rec, 19); c.ify = rec1(rec, 20);
-  return c;
-}
-
-// Block-level stream compaction: every thread offers (valid, value); afterwards list[0..count)
-// holds the values of the valid threads in thread order.  Keeps whole warps idle instead of
-// 30 % of the lanes of every warp (track visibility is ~70 %).
-template <int NT = kThreads>
-__device__ __forceinline__ int block_compact(bool valid, int value, int* list, int* warp_base) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned m = __ballot_sync(0xffffffffu, valid);
-  if (lane == 0) warp_base[warp] = __popc(m);
-  __syncthreads();
-  int base = 0, total = 0;
-#pragma unroll
-  for (int w = 0; w < NT / 32; ++w) {
-    const int c = warp_base[w];
-    if (w < warp) base += c;
-    total += c;
-  }
-  if (valid) list[base + __popc(m & ((1u << lane) - 1u))] = value;
-  __syncthreads();
-  return total;
+static_assert(kTrackRec % 4 == 0, "frame records are read as float4");
+struct TrackRec {
+  float R[9], t[3], c[3];
+  Cam k;
+};
+__device__ __forceinline__ TrackRec load_rec(const float* rec) {
+  const float4* r4 = reinterpret_cast<const float4*>(rec);
+  const float4 a = r4[0], b = r4[1], c = r4[2], d = r4[3], e = r4[4], f = r4[5];
+  TrackRec r;
+  r.R[0] = a.x; r.R[1] = a.y; r.R[2] = a.z; r.R[3] = a.w; r.R[4] = b.x; r.R[5] = b.y; r.R[6] = b.z; r.R[7] = b.w;
+  r.R[8] = c.x; r.t[0] = c.y; r.t[1] = c.z; r.t[2] = c.w;
+  r.c[0] = d.x; r.c[1] = d.y; r.c[2] = d.z;
+  r.k.fx = d.w; r.k.fy = e.x; r.k.cx = e.y; r.k.cy = e.z; r.k.ifx = e.w; r.k.ify = f.x;
+  return r;
 }
 
 // Warp sum of N per-lane values by recursive halving (N = 10: 12 shuffles instead of 50; N = 6:
@@ -1605,189 +1588,268 @@ __device__ __forceinline__ float warp_sum_n(float* v, int lane) {
   return v[0];
 }
 
-// One sweep over the (source row, target row, point) triples.  A block of kTrackThreads threads owns
-// (segment, source row, kTrackPoints = 2 * kTrackThreads points): every thread keeps TWO usable source
-// points in registers and evaluates their terms against one target row as ONE two-wide F2
-// computation (fm_math.cuh: the two points share every target-frame constant; lean_term2 of
-// fm_pixel.cuh is the two-pixel form of the flow kernel's term).  The source-side sums stay in
-// registers; the target-side sums (pose twist and K of the TARGET frame) of one loop iteration belong
-// to one frame for the whole block, so the two points' contributions are added and each warp reduces
-// them with warp_sum_n into its own [target row][10] slice of shared memory -- one reduction per 64
-// terms -- folded into the per-frame accumulators at the end.
+// One sweep over the (source row, target row, point) triples.  Work item = one of kTrackParts
+// contiguous point ranges of a (segment, source row): a persistent grid of kTrackThreads-thread blocks
+// takes the items in order from a counter in the workspace, so the per-item costs -- staging the
+// segment's frame records, the source-side block sums and the float64 atomics of the target-side
+// sums -- are paid kTrackParts times per row.  Items cost about the same (rows x usable points); at the
+// benchmark shape whole rows are 1146 items for 660 resident blocks, and halves of rows measured
+// faster on H100 (a shorter last wave) than whole rows or thirds.
+//
+// Per item the range's usable source points (visible and inside [0,1)^2, recorded in `flag`) are compacted
+// in point order into a shared list, at most kTrackListCap points per round.  The list is cut into warp
+// passes of kTrackPass points, and warp w takes passes w, w + NW, ...: every warp of the block stays busy
+// until the last kTrackPass points.  In a pass every lane keeps kTrackPPT source points in registers and
+// evaluates their terms (lean_term of fm_pixel.cuh, the flow kernel's term) against each target row of
+// the segment.  The source-side sums stay in registers for the whole item; the target-side sums of one
+// target row (pose twist and K of the TARGET frame) belong to one frame for the whole warp, so the
+// lane's points are added and the warp reduces them with warp_sum_n into its own [target row][10]
+// slice of shared memory, which accumulates over the warp's passes and is folded into the per-frame
+// accumulators once per item.
 // SHARED_K: every frame has the same intrinsics (one focal length, or constants), so only the SUM
 // over frames of the intrinsics gradient matters: the target-frame terms are then added to the
 // thread's own (source-frame) accumulators and only the 6 pose values go through the reduction.
 constexpr int kTrackThreads = 128;
-constexpr int kTrackPoints = 2 * kTrackThreads;
+#ifndef FM_TRACK_PPT
+#define FM_TRACK_PPT 2  // source points per lane (1 or 2); 2 measured faster on H100
+#endif
+#ifndef FM_TRACK_BPS
+#define FM_TRACK_BPS 5  // blocks per SM the register budget is sized for
+#endif
+#ifndef FM_TRACK_PARTS
+#define FM_TRACK_PARTS 2  // work items per source row (halves of its points: a shorter last wave)
+#endif
+constexpr int kTrackParts = FM_TRACK_PARTS;
+constexpr int kTrackPPT = FM_TRACK_PPT;
+constexpr int kTrackPass = 32 * kTrackPPT;
+constexpr int kTrackListCap = 2048;
+static_assert(kTrackPPT == 1 || kTrackPPT == 2, "FM_TRACK_PPT must be 1 or 2");
+
+// Dynamic shared memory of k_track_src: frame records, the warps' target-side slices, the point list.
+__host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap) {
+  return ((size_t)max_rows * (kTrackRec + (kTrackThreads / 32) * kTrackAcc) + (size_t)list_cap) * sizeof(float);
+}
 
 template <bool SHARED_K>
-__global__ void __launch_bounds__(kTrackThreads, 5)  // 96 registers: 5 blocks per SM (122 unbounded: 4; 80: spills)
+__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS)
 k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,
             const int* __restrict__ seg, const float* __restrict__ txy,
             const unsigned char* __restrict__ tvis, int mapping, float delta, double* __restrict__ sums,
             unsigned char* __restrict__ flag, float* __restrict__ dq_out,
-            double* __restrict__ trackacc, int H, int W, TrackShard sh) {
-  extern __shared__ float sm[];
+            double* __restrict__ trackacc, int* __restrict__ next_item, int num_items, int max_rows,
+            int list_cap, int H, int W, TrackShard sh) {
+  extern __shared__ float4 sm4[];
+  float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
+  constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
+  constexpr int SLOT0 = kTrackAcc - NRED;  // twist values live in slots 4..9 either way
   __shared__ double red[kTrackAcc * NW];
-  const SegInfo si = load_seg(seg, blockIdx.z);
-  const int row = blockIdx.y;
-  if (row >= si.rows || !sh.owns(si.start_frame + row)) return;
-  load_segment_frames(sm, ext, k4, si);
-  float* s_tgt = sm + (size_t)gridDim.y * 2 * kTrackRec;  // [warp][target row][kTrackAcc]
-  __shared__ int s_list[kTrackPoints];
   __shared__ int s_wbase[NW];
+  __shared__ int s_item[2];
+  float* s_tgt = sm + (size_t)max_rows * kTrackRec;  // [warp][target row][kTrackAcc]
+  int* s_list = reinterpret_cast<int*>(s_tgt + (size_t)NW * max_rows * kTrackAcc);
   const GridDims grid = make_grid(H, W);
   const RobustCfg rc = make_robust(mapping, delta, H, W);
-  const int frame = si.start_frame + row;
-  const float* D = depth + (size_t)(frame - sh.depth_frame0) * H * W;
-  const float* rsrec = sm + row * 2 * kTrackRec;
-  float rs[12];  // source pose: R (9), t (3)
-#pragma unroll
-  for (int i = 0; i < 12; ++i) rs[i] = rec1(rsrec, i);
-  const Cam ks = sm_cam(rsrec);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  float acc[kTrackAcc], lc[2] = {0.f, 0.f};
-#pragma unroll
-  for (int i = 0; i < kTrackAcc; ++i) acc[i] = 0.f;
-  // which of this block's points are usable sources (visible and inside [0,1)^2)?  Two offers per
-  // thread, compacted one after the other into one list.
-  int count = 0;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int p_own = blockIdx.x * kTrackPoints + h * kTrackThreads + (int)threadIdx.x;
-    bool ok_own = false;
-    if (p_own < si.n) {
-      const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p_own;
-      const float2 sxy = __ldg(reinterpret_cast<const float2*>(txy) + sidx);
-      ok_own = tvis[sidx] && in_unit_square(sxy.x, sxy.y);
-      flag[sidx] = ok_own ? 1 : 0;
-    }
-    count += block_compact<kTrackThreads>(ok_own, p_own, s_list + count, s_wbase);
-  }
-  const int half = (count + 1) >> 1;  // thread t works on list[t] and list[t + half]
-  const bool live_a = (int)threadIdx.x < half, live_b = (int)threadIdx.x + half < count;
-  if (warp * 32 < half) {  // warp-uniform: the shuffles below need all 32 lanes
-    const int pa = live_a ? s_list[threadIdx.x] : 0, pb = live_b ? s_list[threadIdx.x + half] : 0;
-    const size_t row0 = (size_t)si.sample_start + (size_t)row * si.n;
-    float qa[3] = {0.f, 0.f, 0.f}, qb[3] = {0.f, 0.f, 0.f};
-    F2 Xw[3] = {f2s(0.f), f2s(0.f), f2s(0.f)};
-    auto lift = [&](int p, float* q, float* X) {
-      const float2 sxy = __ldg(reinterpret_cast<const float2*>(txy) + row0 + p);
-      const Taps t = bilinear_taps(sxy.x, sxy.y, grid);
-      sample_surface(t, grid, ks, [D](int o) { return __ldg(D + o); }, q[0], q[1], q[2]);
-#pragma unroll
-      for (int i = 0; i < 3; ++i)
-        X[i] = fm_fma(rs[i * 3 + 0], q[0], fm_fma(rs[i * 3 + 1], q[1], fm_fma(rs[i * 3 + 2], q[2], rs[9 + i])));
-    };
-    if (live_a) { float X[3]; lift(pa, qa, X); Xw[0].x = X[0]; Xw[1].x = X[1]; Xw[2].x = X[2]; }
-    if (live_b) { float X[3]; lift(pb, qb, X); Xw[0].y = X[0]; Xw[1].y = X[1]; Xw[2].y = X[2]; }
-    F2 G[3] = {f2s(0.f), f2s(0.f), f2s(0.f)}, lc2[2] = {f2s(0.f), f2s(0.f)};
-    F2 kt[4] = {f2s(0.f), f2s(0.f), f2s(0.f), f2s(0.f)};  // SHARED_K: intrinsics terms of the targets
-    constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
-    constexpr int SLOT0 = kTrackAcc - NRED;  // twist values live in slots 4..9 either way
-    const TrackSlot slot = track_slot<NRED>(lane);
+  const TrackSlot slot = track_slot<NRED>(lane);
+  const float2* xy2 = reinterpret_cast<const float2*>(txy);
+  for (int it = 0;; ++it) {
+    // s_item alternates, so the next item can be fetched while slow threads still read this one
+    if (threadIdx.x == 0) s_item[it & 1] = atomicAdd(next_item, 1);
+    __syncthreads();
+    const int item = s_item[it & 1];
+    if (item >= num_items) break;
+    const int part = item % kTrackParts, srow = item / kTrackParts;
+    const SegInfo si = load_seg(seg, srow / max_rows);
+    const int row = srow % max_rows;
+    if (row >= si.rows || !sh.owns(si.start_frame + row)) continue;
+    load_segment_frames(sm, ext, k4, si);
     float* tgt = s_tgt + (size_t)warp * si.rows * kTrackAcc;
-    // the next target row's visibility / position is fetched while the current one is processed
-    size_t ia = (size_t)si.sample_start + pa, ib = (size_t)si.sample_start + pb;
-    unsigned char va_n = live_a ? tvis[ia] : 0, vb_n = live_b ? tvis[ib] : 0;
-    float2 ga_n = live_a ? __ldg(reinterpret_cast<const float2*>(txy) + ia) : make_float2(0.f, 0.f);
-    float2 gb_n = live_b ? __ldg(reinterpret_cast<const float2*>(txy) + ib) : make_float2(0.f, 0.f);
-    for (int ft = 0; ft < si.rows; ++ft) {
-      const unsigned char vis_a = va_n, vis_b = vb_n;
-      const float2 ga = ga_n, gb = gb_n;
-      if (ft + 1 < si.rows) {
-        if (live_a) { ia += si.n; va_n = tvis[ia]; ga_n = __ldg(reinterpret_cast<const float2*>(txy) + ia); }
-        if (live_b) { ib += si.n; vb_n = tvis[ib]; gb_n = __ldg(reinterpret_cast<const float2*>(txy) + ib); }
+    for (int i = lane; i < si.rows * kTrackAcc; i += 32) tgt[i] = 0.f;
+    __syncwarp();
+    const int frame = si.start_frame + row;
+    const float* D = depth + (size_t)(frame - sh.depth_frame0) * H * W;
+    const float* rsrec = sm + row * kTrackRec;
+    const size_t row0 = (size_t)si.sample_start + (size_t)row * si.n;
+    const float2* seg_xy = xy2 + si.sample_start;
+    const unsigned char* seg_vis = tvis + si.sample_start;
+    float acc[kTrackAcc], lc[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < kTrackAcc; ++i) acc[i] = 0.f;
+    const int p_end = (int)((long long)si.n * (part + 1) / kTrackParts);
+    for (int base = (int)((long long)si.n * part / kTrackParts); base < p_end; base += list_cap) {
+      // compaction in point order: warp w scans [lo, hi), counts, then writes at its offset
+      const int len = min(list_cap, p_end - base);
+      const int per = (len + NW * 32 - 1) / (NW * 32) * 32;
+      const int lo = base + warp * per, hi = min(base + len, lo + per);
+      int cnt = 0;
+      for (int p0 = lo; p0 < hi; p0 += 32) {
+        const int p = p0 + lane;
+        bool ok = false;
+        if (p < hi) {
+          const size_t sidx = row0 + p;
+          const float2 sxy = __ldg(xy2 + sidx);
+          ok = tvis[sidx] && in_unit_square(sxy.x, sxy.y);
+          flag[sidx] = ok ? 1 : 0;
+        }
+        cnt += __popc(__ballot_sync(0xffffffffu, ok));
       }
-      float c[NRED];
+      if (lane == 0) s_wbase[warp] = cnt;
+      __syncthreads();
+      int wb = 0, total = 0;
 #pragma unroll
-      for (int i = 0; i < NRED; ++i) c[i] = 0.f;
-      bool ok = false;
-      if (vis_a | vis_b) {
-        const float* rec = sm + ft * 2 * kTrackRec;
-        F2 R[9];
+      for (int w = 0; w < NW; ++w) {
+        const int c = s_wbase[w];
+        if (w < warp) wb += c;
+        total += c;
+      }
+      for (int p0 = lo; p0 < hi; p0 += 32) {
+        const int p = p0 + lane;
+        const bool ok = p < hi && flag[row0 + p];  // this lane's own store above
+        const unsigned m = __ballot_sync(0xffffffffu, ok);
+        if (ok) s_list[wb + __popc(m & ((1u << lane) - 1u))] = p;
+        wb += __popc(m);
+      }
+      __syncthreads();
+      const int npass = (total + kTrackPass - 1) / kTrackPass;
+      for (int ps = warp; ps < npass; ps += NW) {  // warp-uniform: the shuffles below need all 32 lanes
+        const int pb = ps * kTrackPass + lane;
+        // lift the pass's source points to world space
+        float Xw[kTrackPPT][3];
+        int ix[kTrackPPT];  // sample offset within the segment: row ft of point p is p + ft * n
+        {
+          const TrackRec rs = load_rec(rsrec);
 #pragma unroll
-        for (int i = 0; i < 9; ++i) R[i] = rec2(rec, i);
-        // Y = R_t^T Xw + c_t for both points
-        const F2 dir0 = f2_fma(R[0], Xw[0], f2_fma(R[3], Xw[1], f2_mul(R[6], Xw[2])));
-        const F2 dir1 = f2_fma(R[1], Xw[0], f2_fma(R[4], Xw[1], f2_mul(R[7], Xw[2])));
-        const F2 dir2 = f2_fma(R[2], Xw[0], f2_fma(R[5], Xw[1], f2_mul(R[8], Xw[2])));
-        Cam2 kc;
-        kc.fx = rec2(rec, 15); kc.fy = rec2(rec, 16); kc.cx = rec2(rec, 17); kc.cy = rec2(rec, 18);
-        const LeanTerm2 lt = lean_term2(f2s(1.0f), dir0, dir1, dir2, rec2(rec, 12), rec2(rec, 13), rec2(rec, 14), kc,
-                                        f2(ga.x, gb.x), f2(ga.y, gb.y), f2s(0.f), f2s(0.f), f2s(1.0f), rc);
-        // projection.py:294-296: the PREDICTED target position decides
-        const bool oa = vis_a && in_unit_square(lt.uvx.x, lt.uvy.x);
-        const bool ob = vis_b && in_unit_square(lt.uvx.y, lt.uvy.y);
-        if (oa | ob) {
-          ok = true;
-          // an invalid point contributes nothing (selects, not products: its adjoint may hold inf / nan;
-          // the camera-space point P itself is always finite)
-          const F2 d0 = f2(oa ? lt.d0.x : 0.f, ob ? lt.d0.y : 0.f);
-          const F2 d1 = f2(oa ? lt.d1.x : 0.f, ob ? lt.d1.y : 0.f);
-          const F2 d2 = f2(oa ? lt.d2.x : 0.f, ob ? lt.d2.y : 0.f);
-          lc2[0] = f2_add(lc2[0], f2(oa ? lt.loss.x : 0.f, ob ? lt.loss.y : 0.f));
-          lc2[1] = f2_add(lc2[1], f2(oa ? 1.f : 0.f, ob ? 1.f : 0.f));
-          // world-space gradient g = R_t dY
-          const F2 g0 = f2_fma(R[0], d0, f2_fma(R[1], d1, f2_mul(R[2], d2)));
-          const F2 g1 = f2_fma(R[3], d0, f2_fma(R[4], d1, f2_mul(R[5], d2)));
-          const F2 g2 = f2_fma(R[6], d0, f2_fma(R[7], d1, f2_mul(R[8], d2)));
-          G[0] = f2_add(G[0], g0); G[1] = f2_add(G[1], g1); G[2] = f2_add(G[2], g2);
-          // target-frame K gradient: duv = d (P_z + eps) / f and uv - c = f P / (P_z + eps)
-          const F2 ex = f2_mul(d0, rec2(rec, 19)), ey = f2_mul(d1, rec2(rec, 20));
-          if (SHARED_K) {
-            kt[0] = f2_fma(ex, lt.P0, kt[0]); kt[1] = f2_fma(ey, lt.P1, kt[1]);
-            kt[2] = f2_fma(ex, lt.P2, kt[2]); kt[3] = f2_fma(ey, lt.P2, kt[3]);
-          } else {
-            const F2 k0 = f2_mul(ex, lt.P0), k1 = f2_mul(ey, lt.P1), k2 = f2_mul(ex, lt.P2), k3 = f2_mul(ey, lt.P2);
-            c[0] = k0.x + k0.y; c[1] = k1.x + k1.y; c[2] = k2.x + k2.y; c[3] = k3.x + k3.y;
+          for (int j = 0; j < kTrackPPT; ++j) {
+            Xw[j][0] = Xw[j][1] = Xw[j][2] = 0.f;
+            ix[j] = -1;
+            if (pb + 32 * j < total) {
+              const int p = s_list[pb + 32 * j];
+              ix[j] = p;
+              const float2 sxy = __ldg(xy2 + row0 + p);
+              const Taps t = bilinear_taps(sxy.x, sxy.y, grid);
+              float q[3];
+              sample_surface(t, grid, rs.k, [D](int o) { return __ldg(D + o); }, q[0], q[1], q[2]);
+#pragma unroll
+              for (int i = 0; i < 3; ++i)
+                Xw[j][i] = fm_fma(rs.R[i * 3 + 0], q[0], fm_fma(rs.R[i * 3 + 1], q[1], fm_fma(rs.R[i * 3 + 2], q[2], rs.t[i])));
+            }
           }
-          // twist of the target pose: (Xw - t) x g, -g (an invalid point has g = 0)
-          const F2 e0 = f2_sub(Xw[0], rec2(rec, 9)), e1 = f2_sub(Xw[1], rec2(rec, 10)), e2 = f2_sub(Xw[2], rec2(rec, 11));
-          const F2 t0 = f2_fma(e2, g1, f2_neg(f2_mul(e1, g2)));
-          const F2 t1 = f2_fma(e0, g2, f2_neg(f2_mul(e2, g0)));
-          const F2 t2 = f2_fma(e1, g0, f2_neg(f2_mul(e0, g1)));
-          float* tw = c + (SHARED_K ? 0 : 4);
-          tw[0] = t0.x + t0.y; tw[1] = t1.x + t1.y; tw[2] = t2.x + t2.y;
-          tw[3] = -(g0.x + g0.y); tw[4] = -(g1.x + g1.y); tw[5] = -(g2.x + g2.y);
+        }
+        float G[kTrackPPT][3];
+#pragma unroll
+        for (int j = 0; j < kTrackPPT; ++j) G[j][0] = G[j][1] = G[j][2] = 0.f;
+        // the next target row's visibility / position is fetched while the current one is processed
+        unsigned char vn[kTrackPPT];
+        float2 gn[kTrackPPT];
+#pragma unroll
+        for (int j = 0; j < kTrackPPT; ++j) {
+          vn[j] = ix[j] >= 0 ? seg_vis[ix[j]] : 0;
+          gn[j] = ix[j] >= 0 ? __ldg(seg_xy + ix[j]) : make_float2(0.f, 0.f);
+        }
+        for (int ft = 0; ft < si.rows; ++ft) {
+          unsigned char v[kTrackPPT];
+          float2 g[kTrackPPT];
+          bool any = false;
+#pragma unroll
+          for (int j = 0; j < kTrackPPT; ++j) {
+            v[j] = vn[j]; g[j] = gn[j];
+            any |= v[j] != 0;
+            if (ft + 1 < si.rows && ix[j] >= 0) {
+              ix[j] += si.n;
+              vn[j] = seg_vis[ix[j]];
+              gn[j] = __ldg(seg_xy + ix[j]);
+            }
+          }
+          float c[NRED];
+#pragma unroll
+          for (int i = 0; i < NRED; ++i) c[i] = 0.f;
+          bool ok = false;
+          if (any) {
+            const TrackRec r = load_rec(sm + ft * kTrackRec);
+#pragma unroll
+            for (int j = 0; j < kTrackPPT; ++j) {
+              // Y = R_t^T Xw + c_t
+              const float dir0 = fm_fma(r.R[0], Xw[j][0], fm_fma(r.R[3], Xw[j][1], __fmul_rn(r.R[6], Xw[j][2])));
+              const float dir1 = fm_fma(r.R[1], Xw[j][0], fm_fma(r.R[4], Xw[j][1], __fmul_rn(r.R[7], Xw[j][2])));
+              const float dir2 = fm_fma(r.R[2], Xw[j][0], fm_fma(r.R[5], Xw[j][1], __fmul_rn(r.R[8], Xw[j][2])));
+              const LeanTerm lt = lean_term(1.0f, dir0, dir1, dir2, r.c[0], r.c[1], r.c[2], r.k, g[j].x, g[j].y, 0.f,
+                                            0.f, 1.0f, rc);
+              // projection.py:294-296: the PREDICTED target position decides
+              const bool o = v[j] && in_unit_square(lt.uvx, lt.uvy);
+              ok |= o;
+              // an invalid point contributes nothing (selects, not products: its adjoint may hold inf / nan;
+              // the camera-space point P itself is always finite)
+              const float d0 = o ? lt.d0 : 0.f, d1 = o ? lt.d1 : 0.f, d2 = o ? lt.d2 : 0.f;
+              lc[0] = __fadd_rn(lc[0], o ? lt.loss : 0.f);
+              lc[1] = __fadd_rn(lc[1], o ? 1.f : 0.f);
+              // world-space gradient g = R_t dY
+              const float g0 = fm_fma(r.R[0], d0, fm_fma(r.R[1], d1, __fmul_rn(r.R[2], d2)));
+              const float g1 = fm_fma(r.R[3], d0, fm_fma(r.R[4], d1, __fmul_rn(r.R[5], d2)));
+              const float g2 = fm_fma(r.R[6], d0, fm_fma(r.R[7], d1, __fmul_rn(r.R[8], d2)));
+              G[j][0] = __fadd_rn(G[j][0], g0); G[j][1] = __fadd_rn(G[j][1], g1); G[j][2] = __fadd_rn(G[j][2], g2);
+              // target-frame K gradient: duv = d (P_z + eps) / f and uv - c = f P / (P_z + eps)
+              const float ex = __fmul_rn(d0, r.k.ifx), ey = __fmul_rn(d1, r.k.ify);
+              if (SHARED_K) {  // straight into the thread's own intrinsics sums
+                acc[0] = fm_fma(ex, lt.P0, acc[0]); acc[1] = fm_fma(ey, lt.P1, acc[1]);
+                acc[2] = fm_fma(ex, lt.P2, acc[2]); acc[3] = fm_fma(ey, lt.P2, acc[3]);
+              } else {
+                c[0] = __fadd_rn(c[0], __fmul_rn(ex, lt.P0)); c[1] = __fadd_rn(c[1], __fmul_rn(ey, lt.P1));
+                c[2] = __fadd_rn(c[2], __fmul_rn(ex, lt.P2)); c[3] = __fadd_rn(c[3], __fmul_rn(ey, lt.P2));
+              }
+              // twist of the target pose: (Xw - t) x g, -g (an invalid point has g = 0)
+              const float e0 = __fsub_rn(Xw[j][0], r.t[0]), e1 = __fsub_rn(Xw[j][1], r.t[1]);
+              const float e2 = __fsub_rn(Xw[j][2], r.t[2]);
+              float* tw = c + (SHARED_K ? 0 : 4);
+              tw[0] = __fadd_rn(tw[0], fm_fma(e2, g1, -__fmul_rn(e1, g2)));
+              tw[1] = __fadd_rn(tw[1], fm_fma(e0, g2, -__fmul_rn(e2, g0)));
+              tw[2] = __fadd_rn(tw[2], fm_fma(e1, g0, -__fmul_rn(e0, g1)));
+              tw[3] = __fsub_rn(tw[3], g0); tw[4] = __fsub_rn(tw[4], g1); tw[5] = __fsub_rn(tw[5], g2);
+            }
+          }
+          if (__ballot_sync(0xffffffffu, ok)) {
+            const float total_c = warp_sum_n<NRED>(c, lane);
+            if (slot.owner) tgt[ft * kTrackAcc + SLOT0 + slot.slot] += total_c;
+          }
+        }
+        // camera-space adjoint of the sampled points (unscaled), source K / twist sums; the sampled
+        // point is evaluated again instead of being kept in registers through the target loop
+        const TrackRec rs = load_rec(rsrec);
+#pragma unroll
+        for (int j = 0; j < kTrackPPT; ++j) {
+          if (pb + 32 * j >= total) continue;
+          const size_t sidx = row0 + s_list[pb + 32 * j];
+          const float2 sxy = __ldg(xy2 + sidx);
+          const Taps t = bilinear_taps(sxy.x, sxy.y, grid);
+          float q[3];
+          sample_surface(t, grid, rs.k, [D](int o) { return __ldg(D + o); }, q[0], q[1], q[2]);
+          const float G0 = G[j][0], G1 = G[j][1], G2 = G[j][2];
+          const float dq0 = fm_fma(rs.R[0], G0, fm_fma(rs.R[3], G1, rs.R[6] * G2));
+          const float dq1 = fm_fma(rs.R[1], G0, fm_fma(rs.R[4], G1, rs.R[7] * G2));
+          const float dq2 = fm_fma(rs.R[2], G0, fm_fma(rs.R[5], G1, rs.R[8] * G2));
+          dq_out[sidx * 3 + 0] = dq0; dq_out[sidx * 3 + 1] = dq1; dq_out[sidx * 3 + 2] = dq2;
+          const float e0 = dq0 * rs.k.ifx, e1 = dq1 * rs.k.ify;
+          acc[0] -= e0 * q[0]; acc[1] -= e1 * q[1]; acc[2] -= e0 * q[2]; acc[3] -= e1 * q[2];
+          const float c0 = Xw[j][0] - rs.t[0], c1 = Xw[j][1] - rs.t[1], c2 = Xw[j][2] - rs.t[2];
+          acc[4] += c1 * G2 - c2 * G1;
+          acc[5] += c2 * G0 - c0 * G2;
+          acc[6] += c0 * G1 - c1 * G0;
+          acc[7] += G0; acc[8] += G1; acc[9] += G2;
         }
       }
-      float total = 0.f;
-      if (__ballot_sync(0xffffffffu, ok)) total = warp_sum_n<NRED>(c, lane);
-      if (slot.owner) tgt[ft * kTrackAcc + SLOT0 + slot.slot] = total;
+      __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
-    lc[0] = lc2[0].x + lc2[0].y;
-    lc[1] = lc2[1].x + lc2[1].y;
-    // camera-space adjoint of the sampled points (unscaled), source K / twist sums
-    auto finish = [&](int p, const float* q, float X0, float X1, float X2, float G0, float G1, float G2, float k0,
-                      float k1, float k2, float k3) {
-      const size_t sidx = row0 + p;
-      const float dq0 = fm_fma(rs[0], G0, fm_fma(rs[3], G1, rs[6] * G2));
-      const float dq1 = fm_fma(rs[1], G0, fm_fma(rs[4], G1, rs[7] * G2));
-      const float dq2 = fm_fma(rs[2], G0, fm_fma(rs[5], G1, rs[8] * G2));
-      dq_out[sidx * 3 + 0] = dq0; dq_out[sidx * 3 + 1] = dq1; dq_out[sidx * 3 + 2] = dq2;
-      const float e0 = dq0 * ks.ifx, e1 = dq1 * ks.ify;
-      acc[0] += k0 - e0 * q[0]; acc[1] += k1 - e1 * q[1]; acc[2] += k2 - e0 * q[2]; acc[3] += k3 - e1 * q[2];
-      const float c0 = X0 - rs[9], c1 = X1 - rs[10], c2 = X2 - rs[11];
-      acc[4] += c1 * G2 - c2 * G1;
-      acc[5] += c2 * G0 - c0 * G2;
-      acc[6] += c0 * G1 - c1 * G0;
-      acc[7] += G0; acc[8] += G1; acc[9] += G2;
-    };
-    if (live_a) finish(pa, qa, Xw[0].x, Xw[1].x, Xw[2].x, G[0].x, G[1].x, G[2].x, kt[0].x, kt[1].x, kt[2].x, kt[3].x);
-    if (live_b) finish(pb, qb, Xw[0].y, Xw[1].y, Xw[2].y, G[0].y, G[1].y, G[2].y, kt[0].y, kt[1].y, kt[2].y, kt[3].y);
-  }
-  block_accumulate<2, kTrackThreads>(lc, sums, red);
-  block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
-  // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
-  // with a barrier, so every slice is complete)
-  const int live_warps = (half + 31) >> 5;
-  for (int i = threadIdx.x; i < si.rows * kTrackAcc; i += kTrackThreads) {
-    if (SHARED_K && i % kTrackAcc < 4) continue;  // those slots are not written in this mode
-    double t = 0.0;
-    for (int w = 0; w < live_warps; ++w) t += (double)s_tgt[(size_t)w * si.rows * kTrackAcc + i];
-    if (t != 0.0) atomicAdd(trackacc + (size_t)si.start_frame * kTrackAcc + i, t);
+    block_accumulate<2, kTrackThreads>(lc, sums, red);
+    block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
+    // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
+    // with a barrier, so every slice is complete)
+    for (int i = threadIdx.x; i < si.rows * kTrackAcc; i += kTrackThreads) {
+      if (SHARED_K && i % kTrackAcc < 4) continue;  // those slots are not written in this mode
+      double t = 0.0;
+#pragma unroll
+      for (int w = 0; w < NW; ++w) t += (double)s_tgt[(size_t)w * si.rows * kTrackAcc + i];
+      if (t != 0.0) atomicAdd(trackacc + (size_t)si.start_frame * kTrackAcc + i, t);
+    }
   }
 }
 
@@ -2813,10 +2875,12 @@ size_t fm_track_workspace_bytes(int F, long long total_samples) {
 }
 
 namespace {
-struct TrackWs { double* sums; double* acc; float* dq; unsigned char* flag; };
+// next_item: k_track_src's work counter, in the padding after the sums (zeroed with them)
+struct TrackWs { double* sums; int* next_item; double* acc; float* dq; unsigned char* flag; };
 TrackWs carve_track(void* base, int F, long long total) {
   char* p = (char*)base; size_t off = 0; TrackWs w;
-  w.sums = (double*)(p + off); off = align_up(off + 4 * sizeof(double), 256);
+  w.sums = (double*)(p + off); w.next_item = (int*)(p + off + 4 * sizeof(double));
+  off = align_up(off + 4 * sizeof(double), 256);
   w.acc = (double*)(p + off); off = align_up(off + (size_t)F * kTrackAcc * sizeof(double), 256);
   w.dq = (float*)(p + off); off = align_up(off + (size_t)total * 3 * sizeof(float), 256);
   w.flag = (unsigned char*)(p + off);
@@ -2842,11 +2906,19 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
     return fail_msg("fm_track_loss_fwd: bad source-frame range");
   cudaStream_t s = (cudaStream_t)stream;
   TrackWs w = carve_track(ws, F, total_samples);
-  cudaError_t e = cudaMemsetAsync(w.sums, 0, (char*)w.dq - (char*)w.sums, s);  // sums + accumulators
+  // sums, work counter, accumulators
+  cudaError_t e = cudaMemsetAsync(w.sums, 0, (char*)w.dq - (char*)w.sums, s);
   if (e != cudaSuccess) return fail("fm_track_loss_fwd: memset", e);
-  dim3 grid((max_points + kTrackPoints - 1) / kTrackPoints, max_rows, num_segments);
-  const size_t smem = (size_t)max_rows * (2 * kTrackRec + (kTrackThreads / 32) * kTrackAcc) * sizeof(float);
+  const int list_cap = max_points < kTrackListCap ? max_points : kTrackListCap;
+  const size_t smem = track_smem_bytes(max_rows, list_cap);
   if (smem > 200 * 1024) return fail_msg("fm_track_loss_fwd: segment too long for shared memory");
+  // a persistent grid: as many blocks as fit on the GPU at once (registers or shared memory)
+  const long long items = (long long)num_segments * max_rows * kTrackParts;
+  if (items > INT_MAX) return fail_msg("fm_track_loss_fwd: too many segment rows");
+  int per_sm = (int)((227 * 1024) / (smem + sizeof(double) * kTrackAcc * (kTrackThreads / 32) + 1024 + 64));
+  if (per_sm > FM_TRACK_BPS) per_sm = FM_TRACK_BPS;
+  if (per_sm < 1) per_sm = 1;
+  const int grid = persistent_grid(per_sm, items);
   if (smem > 48 * 1024) {
     cudaError_t ea = shared_intrinsics
         ? cudaFuncSetAttribute(k_track_src<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
@@ -2856,10 +2928,12 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
   if (shared_intrinsics)
     k_track_src<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping,
-                                                  delta, w.sums, w.flag, w.dq, w.acc, H, W, sh);
+                                                        delta, w.sums, w.flag, w.dq, w.acc, w.next_item, (int)items,
+                                                        max_rows, list_cap, H, W, sh);
   else
     k_track_src<false><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping,
-                                                   delta, w.sums, w.flag, w.dq, w.acc, H, W, sh);
+                                                         delta, w.sums, w.flag, w.dq, w.acc, w.next_item, (int)items,
+                                                         max_rows, list_cap, H, W, sh);
   FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src");
   if (loss) {
     k_track_loss<<<1, 1, 0, s>>>(w.sums, loss_weight, loss);
