@@ -555,20 +555,20 @@ def synthetic_tracks(f: int, n_points: int = 1225, interval: int = 5, radius: in
 
 
 def consistent_scene(f: int, h: int, w: int, seed: int = 0, focal: float = 0.85,
-                     dtype=torch.float64):
+                     dtype=torch.float64, rotation: float = 0.02, translation: float = 0.03):
     """"Parity set": one static surface (the inside of a sphere) seen by cameras that move by
-    a small SE(3) step per frame; depths are exact ray/sphere intersections and flows the
-    exact induced correspondences, so Procrustes is well conditioned and recovers the
-    motion up to bilinear-interpolation error.  Returns (depth (f,h,w), Flows, focal,
-    extrinsics (1,f,4,4))."""
+    an SE(3) step per frame (axis-angle ~ N(0, rotation^2), translation ~ N(0, translation^2)
+    per component); depths are exact ray/sphere intersections and flows the exact induced
+    correspondences, so Procrustes is well conditioned and recovers the motion up to
+    bilinear-interpolation error.  Returns (depth (f,h,w), Flows, focal, extrinsics (1,f,4,4))."""
     g = torch.Generator().manual_seed(seed)
     rel = torch.eye(4, dtype=torch.float64).repeat(f - 1, 1, 1)
-    ang = 0.02 * torch.randn(f - 1, 3, generator=g, dtype=torch.float64)
+    ang = rotation * torch.randn(f - 1, 3, generator=g, dtype=torch.float64)
     for i in range(f - 1):
         ax, ay, az = ang[i]
         skew = torch.tensor([[0, -az, ay], [az, 0, -ax], [-ay, ax, 0]], dtype=torch.float64)
         rel[i, :3, :3] = torch.linalg.matrix_exp(skew)
-    rel[:, :3, 3] = 0.03 * torch.randn(f - 1, 3, generator=g, dtype=torch.float64)
+    rel[:, :3, 3] = translation * torch.randn(f - 1, 3, generator=g, dtype=torch.float64)
     ext = pose_chain(rel[None])  # camera-to-world
     k = intrinsics_from_focal(torch.tensor(focal, dtype=torch.float64), h, w).expand(1, f, 3, 3)
     xy = pixel_grid(h, w, torch.float64)
@@ -589,3 +589,68 @@ def consistent_scene(f: int, h: int, w: int, seed: int = 0, focal: float = 0.85,
     flows = Flows(fwd.to(dtype), bwd.to(dtype), u(1, f - 1, h, w).to(dtype),
                   u(1, f - 1, h, w).to(dtype))
     return depth.to(dtype), flows, focal, ext
+
+
+def scene_tracks(depth: Tensor, ext: Tensor, focal: float, segments: Sequence[tuple[int, int]],
+                 n_points: int, seed: int = 0, p_occluded: float = 0.1,
+                 dtype=torch.float64) -> list[Tracks]:
+    """Point tracks consistent with a :func:`consistent_scene` (depth (f,h,w), camera-to-world
+    extrinsics (1,f,4,4)).  For each (start_frame, rows) segment, `n_points` pixel centres of the
+    first frame are unprojected with the scene depth and projected into every frame of the segment.
+    A point is visible where it lies in front of the camera and inside [0,1)^2, except for a random
+    fraction `p_occluded` of the samples.  The tracks agree with the scene up to the depth
+    interpolation, so their reprojection residuals are small (the Huber quadratic branch)."""
+    g = torch.Generator().manual_seed(seed + 2)
+    _, h, w = depth.shape
+    k = intrinsics_from_focal(torch.tensor(focal, dtype=torch.float64), h, w)
+    xy_all = pixel_grid(h, w, torch.float64).reshape(h * w, 2)
+    segs = []
+    for start, rows in segments:
+        pix = torch.randint(0, h * w, (n_points,), generator=g)
+        cam = unproject(xy_all[pix], depth[start].reshape(h * w)[pix].to(torch.float64), k)
+        world = matvec(ext[0, start], to_homogeneous(cam))
+        moved = matvec(torch.linalg.inv(ext[0, start:start + rows])[:, None], world[None])[..., :3]
+        xy = project_camera_space(moved, k)
+        front = moved[..., 2] > 0
+        vis = front & ((xy >= 0) & (xy < 1)).all(dim=-1)
+        vis &= torch.rand(rows, n_points, generator=g, dtype=torch.float64) >= p_occluded
+        xy = torch.where(front[..., None], xy, torch.full_like(xy, 2.0))
+        segs.append(Tracks(xy[None].to(dtype), vis[None], start))
+    return segs
+
+
+def flow_regime(kind: str, f: int, h: int, w: int, seed: int = 0, b: int = 1):
+    """Float64 depth (b,f,h,w), Flows, focal and camera-to-world extrinsics (b,f,4,4) or None, for
+    the flow regimes the hot path meets beyond :func:`synthetic_flows`' few-pixel noise:
+
+    - ``iid``: synthetic_flows (sigma 0.01), depth 1 + U(0,1);
+    - ``shift``: iid + a coherent (0.2, -0.2) backward motion (forward: the opposite), larger than
+      the scatter window's halo at widths above 80 px and heights above 60;
+    - ``leave``: iid + (0.3, 0): the right 30 % of every later frame maps past the right border;
+    - ``outliers``: 5 % of the flows replaced by N(0, 0.5^2), far outside any window;
+    - ``zoom``: iid + a divergent backward flow 0.6 (xy - 0.5) about the centre, so the taps of one
+      tile spread over 1.6x its extent and leave the frame near the borders;
+    - ``scene``: :func:`consistent_scene` with 0.08 rad / 0.3 steps per frame (about a fifth of
+      the correspondences leave the frame), one seed per batch item."""
+    if kind == "scene":
+        parts = [consistent_scene(f, h, w, seed=seed + i, rotation=0.08, translation=0.3) for i in range(b)]
+        flows = Flows(*(torch.cat([getattr(p[1], n) for p in parts])
+                        for n in ("forward", "backward", "forward_mask", "backward_mask")))
+        return torch.stack([p[0] for p in parts]), flows, parts[0][2], torch.cat([p[3] for p in parts])
+    fl = synthetic_flows(f, h, w, seed=seed, dtype=torch.float64, b=b)
+    g = torch.Generator().manual_seed(seed + 7)
+    depth = 1.0 + torch.rand(b, f, h, w, generator=g, dtype=torch.float64)
+    fwd, bwd = fl.forward, fl.backward
+    if kind in ("shift", "leave"):
+        s = torch.tensor([0.2, -0.2] if kind == "shift" else [0.3, 0.0], dtype=torch.float64)
+        fwd, bwd = fwd - s, bwd + s
+    elif kind == "outliers":
+        for t in (fwd, bwd):
+            m = torch.rand(t.shape[:-1], generator=g) < 0.05
+            t[m] = 0.5 * torch.randn(int(m.sum()), 2, generator=g, dtype=torch.float64)
+    elif kind == "zoom":
+        c = pixel_grid(h, w, torch.float64) - 0.5
+        fwd, bwd = fwd - (0.6 / 1.6) * c, bwd + 0.6 * c
+    elif kind != "iid":
+        raise ValueError(kind)
+    return depth, Flows(fwd.contiguous(), bwd.contiguous(), fl.forward_mask, fl.backward_mask), 0.85, None

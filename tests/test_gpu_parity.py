@@ -448,15 +448,16 @@ def test_random_subset_is_a_uniform_sample_without_replacement():
 
 
 def _oracle_flow_step(depth, wparam, flows64, focal=0.85, **kw):
-    """float64 oracle: loss, extrinsics and gradients for batched inputs (b, f, h, w)."""
+    """Oracle loss, extrinsics and gradients for batched inputs (b, f, h, w), in the dtype of
+    `depth` (float64: the arbiter; float32: the reference's own rounding noise)."""
     from oracle import flowmap_oracle as O
     b, f, h, w = depth.shape
     d = depth.clone().requires_grad_(True)
     wp = wparam.clone().requires_grad_(True)
-    foc = torch.tensor(focal, dtype=torch.float64, requires_grad=True)
+    foc = torch.tensor(focal, dtype=depth.dtype, requires_grad=True)
     weights = torch.sigmoid(100.0 * wp) if kw.get("use_weights", True) else torch.ones_like(wp)
     k = O.intrinsics_from_focal(foc, h, w).expand(b, f, 3, 3)
-    surf = O.unproject(O.pixel_grid(h, w, torch.float64), d, k[:, :, None, None])
+    surf = O.unproject(O.pixel_grid(h, w, depth.dtype), d, k[:, :, None, None])
     idx = torch.arange(h * w)
     ext = O.align_surfaces(surf, flows64.backward, weights, idx)
     loss = 1000.0 * O.flow_loss(surf, ext, k, flows64, kw.get("mapping", "huber"), 0.01)

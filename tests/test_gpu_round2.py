@@ -25,6 +25,30 @@ def test_splat_plan_path_matches_the_red_path(shape, kind):
         assert r["bitwise_repeatable"], r
 
 
+@pytest.mark.parametrize("kind", ["shift", "outliers"])
+def test_splat_plan_path_vs_float64_oracle(kind):
+    """The planned forward / backward on large coherent motion and on 5 % far outliers against the
+    float64 oracle itself, so that a bug shared with the RED path cannot hide behind the comparison
+    above: loss, poses, and the depth (whole, per frame, border band), weight-logit (whole, per pair)
+    and focal gradients within max(1e-4, 3x the float32 oracle's own error)."""
+    import ab_tiled
+    from oracle import flowmap_oracle as O
+    from flowmap_b200 import ops
+    from flow_regime_checks import check, errors, oracle_steps
+    f, h, w = 3, 136, 192
+    c = ab_tiled.make_case(f, h, w, kind)
+    plan = ops.SplatPlan(c["bwd"])
+    assert plan.status == 1, plan.status
+    r = ab_tiled.run_ops(c, f, h, w, plan)
+    cpu = {k: v.double().cpu() for k, v in c.items()}
+    refs = oracle_steps(cpu["depth"][None], cpu["wparam"][None],
+                        O.Flows(cpu["fwd"], cpu["bwd"], cpu["fmask"], cpu["bmask"]), 0.85)
+    out = dict(loss=r["loss"], ext=ops.pose_chain(r["rt"]).cpu(), g_depth=r["g_depth"].cpu(), g_w=r["g_w"].cpu(),
+               g_focal=r["g_focal"])
+    check(errors(out, refs[64]), errors(refs[32], refs[64]), f"splat plan {kind} {f}x{h}x{w}",
+          loss_tol=1e-4, pose_tol=2e-5, floor=1e-4)
+
+
 def test_degenerate_flows_fall_back_to_the_red_path():
     """A flow field whose taps pile up far outside every tile window exceeds the plan's overflow
     capacity: the plan reports it and FusedOverfitter silently keeps the global-RED kernels."""

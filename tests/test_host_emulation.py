@@ -176,3 +176,36 @@ def test_packed_two_point_term_equals_the_scalar_term(emu, mapping):
         ok = np.isfinite(out)
         assert (np.isfinite(out2) == ok).all()
         assert np.allclose(out2[ok], out[ok], rtol=2e-6, atol=1e-7), (case, out, out2)
+
+
+@pytest.fixture(scope="module")
+def regime_cases():
+    """Oracle results of the flow regimes, computed once per (regime, shape) for both kernel variants."""
+    return {}
+
+
+@pytest.mark.parametrize("lean", [False, True])
+@pytest.mark.parametrize("f,h,w", [(4, 40, 64), (4, 38, 63)])
+@pytest.mark.parametrize("kind", ["iid", "shift", "leave", "outliers", "zoom", "scene"])
+def test_emulated_step_in_flow_regimes_vs_float64_oracle(emu, regime_cases, kind, f, h, w, lean):
+    """The kernels' per-pixel code on flows with large coherent motion, taps that leave the frame,
+    outliers, zoom and a large-motion rigid scene (oracle.flow_regime): bilinear_taps' clipping to the
+    border and its adjoint, without any GPU scheduling.  Gradients within max(2e-5, 3x the float32
+    oracle's error), the depth gradient also on the one-pixel border band."""
+    from oracle import flowmap_oracle as O
+    from flow_regime_checks import check, errors, oracle_steps, start_point
+    key = (kind, f, h, w)
+    if key not in regime_cases:
+        depth, fl, focal, _ = O.flow_regime(kind, f, h, w, seed=3)
+        depth, focal = start_point(depth, focal, seed=5)
+        wparam = 0.01 * torch.randn(1, f - 1, h, w, generator=torch.Generator().manual_seed(4), dtype=torch.float64)
+        refs = oracle_steps(depth, wparam, fl, focal)
+        g = {"in_depth": depth[0].numpy(), "in_wparam": wparam[0].numpy(), "in_fwd": fl.forward.numpy(),
+             "in_bwd": fl.backward.numpy(), "in_fmask": fl.forward_mask.numpy(), "in_bmask": fl.backward_mask.numpy()}
+        regime_cases[key] = (g, focal, refs, errors(refs[32], refs[64], per_item=False))
+    g, focal, refs, noise = regime_cases[key]
+    r = run_emulated_step(emu, g, focal=focal, lean=lean)
+    out = dict(loss=r["loss"], ext=torch.as_tensor(r["extrinsics"]), g_depth=torch.as_tensor(r["g_depth"]),
+               g_w=torch.as_tensor(r["g_wparam"]), g_focal=r["g_focal"])
+    check(errors(out, refs[64], per_item=False), noise, f"{kind} {f}x{h}x{w} lean={lean}",
+          loss_tol=1e-4, pose_tol=1e-5, floor=2e-5)
