@@ -356,12 +356,14 @@ def tracking_loss(surfaces: Tensor, extrinsics: Tensor, k: Tensor,
 # --------------------------------------------------------------------------------------
 
 
-def softmin_focal(depths: Tensor, weights: Tensor, backward_flow: Tensor, indices: Tensor,
-                  candidates: Tensor):
-    """Candidate sweep of intrinsics_softmin.py:84-131 on the first frame pair.
+def softmin_residuals(depths: Tensor, weights: Tensor, backward_flow: Tensor, indices: Tensor,
+                      candidates: Tensor) -> Tensor:
+    """Weighted backward-flow residuals of the sweep of intrinsics_softmin.py:84-124 on the first
+    frame pair: Procrustes with each candidate's intrinsics at the points `indices`, then
+    (induced flow - flow) * weight there.
 
     depths (b, f, h, w), weights (b, f-1, h, w), backward_flow (b, f-1, h, w, 2),
-    indices (p,), candidates (n,).  Returns (K (b, 3, 3), softmin weights (b, n)).
+    indices (p,), candidates (n,).  Returns (b, n, p, 2).
     """
     b, _, h, w = depths.shape
     n = candidates.shape[0]
@@ -379,10 +381,35 @@ def softmin_focal(depths: Tensor, weights: Tensor, backward_flow: Tensor, indice
     flow = pos - xy.reshape(h * w, 2)[indices]
     flow_gt = backward_flow[:, :1].reshape(b, 1, h * w, 2)[:, :, indices]
     wsel = weights[:, :1].reshape(b, 1, h * w, 1)[:, :, indices]
-    err = ((flow - flow_gt) * wsel).abs().sum(dim=(-1, -2))  # (b, n)
+    return (flow - flow_gt) * wsel
+
+
+def softmin_errors(depths: Tensor, weights: Tensor, backward_flow: Tensor, indices: Tensor,
+                   candidates: Tensor) -> Tensor:
+    """Per-candidate flow errors of the sweep (intrinsics_softmin.py:125): the L1 norm of
+    :func:`softmin_residuals` over the points, (b, n)."""
+    return softmin_residuals(depths, weights, backward_flow, indices, candidates).abs().sum(dim=(-1, -2))
+
+
+def softmin_intrinsics(err: Tensor, candidates: Tensor, h: int, w: int):
+    """intrinsics_softmin.py:126-131: the softmin over the sweep's errors (b, n) weights the
+    candidates' intrinsics.  Returns (K (b, 3, 3), softmin weights (b, n))."""
+    cand_k = intrinsics_from_focal(candidates.to(err.dtype), h, w)  # (n, 3, 3)
     sm = F.softmin((err - err.min(dim=1, keepdim=True).values) * 10, dim=1)
     k = (cand_k[None] * sm[:, :, None, None]).sum(dim=1)
     return k, sm
+
+
+def softmin_focal(depths: Tensor, weights: Tensor, backward_flow: Tensor, indices: Tensor,
+                  candidates: Tensor):
+    """Candidate sweep of intrinsics_softmin.py:84-131 on the first frame pair:
+    :func:`softmin_intrinsics` of :func:`softmin_errors`.
+
+    Returns (K (b, 3, 3), softmin weights (b, n)).
+    """
+    _, _, h, w = depths.shape
+    err = softmin_errors(depths, weights, backward_flow, indices, candidates)
+    return softmin_intrinsics(err, candidates, h, w)
 
 
 # --------------------------------------------------------------------------------------
@@ -475,7 +502,11 @@ class OverfitOracle:
         return k[:, None].expand(b, self.f, 3, 3)
 
     def forward(self, flows: Flows, step: Optional[int] = None,
-                softmin_indices: Optional[Tensor] = None) -> ModelOutput:
+                softmin_indices: Optional[Tensor] = None,
+                procrustes_idx: Optional[Tensor] = None) -> ModelOutput:
+        """`procrustes_idx` replaces the point set that `procrustes_points` /
+        `procrustes_randomize` would select (a5): to compare with an implementation on the exact
+        indices it used."""
         c = self.cfg
         step = self.global_step if step is None else step
         depths, weights = explicit_backbone(self.depth, self.weights, c.weight_sensitivity)
@@ -484,7 +515,8 @@ class OverfitOracle:
         k = self._intrinsics(depths, weights, flows, step, softmin_indices)
         xy = pixel_grid(self.h, self.w, self.dtype)
         surfaces = unproject(xy, depths, k[:, :, None, None])
-        idx = procrustes_indices(self.h, self.w, c.procrustes_points, c.procrustes_randomize)
+        idx = procrustes_idx if procrustes_idx is not None else \
+            procrustes_indices(self.h, self.w, c.procrustes_points, c.procrustes_randomize)
         extrinsics = align_surfaces(surfaces, flows.backward, weights, idx)
         return ModelOutput(depths, surfaces, k, extrinsics, weights)
 
@@ -505,11 +537,12 @@ class OverfitOracle:
         return res
 
     def training_step(self, flows: Flows, tracks=None,
-                      softmin_indices: Optional[Tensor] = None) -> dict:
+                      softmin_indices: Optional[Tensor] = None,
+                      procrustes_idx: Optional[Tensor] = None) -> dict:
         """One optimiser step; returns the logged quantities (detached)."""
         step = self.global_step
         self.optimizer.zero_grad(set_to_none=True)
-        out = self.forward(flows, step, softmin_indices)
+        out = self.forward(flows, step, softmin_indices, procrustes_idx)
         parts = self.losses(out, flows, tracks, step)
         total = sum(parts.values())
         total.backward()

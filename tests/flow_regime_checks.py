@@ -18,16 +18,22 @@ def start_point(depth, focal, seed):
     return depth * (1.0 + 0.02 * torch.randn(depth.shape, generator=gen, dtype=depth.dtype)), 1.05 * focal
 
 
-def oracle_steps(depth, wparam, flows, focal=0.85, **kw):
+def oracle_steps(depth, wparam, flows, focal=0.85, indices=None, softmin=None, **kw):
     """{64: float64 result, 32: float32 result} of one flow-loss step (_oracle_flow_step) on
-    float64 inputs depth (b, f, h, w), wparam (b, f-1, h, w) and Flows."""
+    float64 inputs depth (b, f, h, w), wparam (b, f-1, h, w) and Flows.  `indices`: the Procrustes
+    point set (default: every pixel); `softmin=(indices, candidates)`: intrinsics from the candidate
+    sweep, g_focal None and g_err the gradient of the sweep's errors."""
     out = {}
     for bits, dt in ((64, torch.float64), (32, torch.float32)):
         fl = type(flows)(*(t.to(dt) for t in (flows.forward, flows.backward, flows.forward_mask,
                                              flows.backward_mask)))
-        loss, ext, gd, gw, gf = _oracle_flow_step(depth.to(dt), wparam.to(dt), fl, focal, **kw)
+        sm = None if softmin is None else (softmin[0], softmin[1].to(dt))
+        loss, ext, gd, gw, gf = _oracle_flow_step(depth.to(dt), wparam.to(dt), fl, focal, indices=indices,
+                                                  softmin=sm, **kw)
         out[bits] = dict(loss=float(loss), ext=ext.double(), g_depth=gd.double(), g_w=gw.double(),
-                         g_focal=float(gf))
+                         g_focal=float(gf) if softmin is None else None)
+        if softmin is not None:
+            out[bits]["g_err"] = gf.double()
     return out
 
 

@@ -447,22 +447,30 @@ def test_random_subset_is_a_uniform_sample_without_replacement():
     assert abs(float(a.double().mean()) - n_items / 2) < 5 * n_items / (12 * n) ** 0.5
 
 
-def _oracle_flow_step(depth, wparam, flows64, focal=0.85, **kw):
+def _oracle_flow_step(depth, wparam, flows64, focal=0.85, indices=None, softmin=None, **kw):
     """Oracle loss, extrinsics and gradients for batched inputs (b, f, h, w), in the dtype of
-    `depth` (float64: the arbiter; float32: the reference's own rounding noise)."""
+    `depth` (float64: the arbiter; float32: the reference's own rounding noise).  `indices`: the
+    Procrustes point set (default: every pixel).  `softmin=(indices, candidates)`: the intrinsics
+    come from the candidate sweep at those points instead of `focal`, and in place of the
+    focal-length gradient the gradient of the sweep's errors (b, n) is returned."""
     from oracle import flowmap_oracle as O
     b, f, h, w = depth.shape
     d = depth.clone().requires_grad_(True)
     wp = wparam.clone().requires_grad_(True)
     foc = torch.tensor(focal, dtype=depth.dtype, requires_grad=True)
     weights = torch.sigmoid(100.0 * wp) if kw.get("use_weights", True) else torch.ones_like(wp)
-    k = O.intrinsics_from_focal(foc, h, w).expand(b, f, 3, 3)
+    if softmin is None:
+        k = O.intrinsics_from_focal(foc, h, w).expand(b, f, 3, 3)
+    else:
+        err = O.softmin_errors(d, weights, flows64.backward, *softmin)
+        err.retain_grad()
+        k = O.softmin_intrinsics(err, softmin[1], h, w)[0][:, None].expand(b, f, 3, 3)
     surf = O.unproject(O.pixel_grid(h, w, depth.dtype), d, k[:, :, None, None])
-    idx = torch.arange(h * w)
+    idx = torch.arange(h * w) if indices is None else indices
     ext = O.align_surfaces(surf, flows64.backward, weights, idx)
     loss = 1000.0 * O.flow_loss(surf, ext, k, flows64, kw.get("mapping", "huber"), 0.01)
     loss.backward()
-    return loss.detach(), ext.detach(), d.grad, wp.grad, foc.grad
+    return loss.detach(), ext.detach(), d.grad, wp.grad, foc.grad if softmin is None else err.grad
 
 
 @pytest.mark.parametrize("b,f,h,w", [(2, 4, 16, 24), (1, 2, 12, 20), (1, 3, 18, 22), (3, 3, 7, 9)])
@@ -892,8 +900,9 @@ def test_fused_trajectory_odd_width_and_subsampled_procrustes(w, npts):
     with torch.no_grad():
         o.model.backbone.depth.copy_(depth.float())
         o.model.backbone.weights.copy_(wparam.float())
+    pts = None if o._indices is None else o._indices.cpu()  # the point set the kernels use
     for step in range(4):
-        ref = st.training_step(fl, trk)
+        ref = st.training_step(fl, trk, procrustes_idx=pts)
         loss, _ = o.training_step()
         assert abs(float(loss) - ref["loss"]) <= 2e-4 * abs(ref["loss"]), step
     assert rel_l2(o.model.backbone.depth.detach().cpu(), st.depth.detach()) <= 1e-5
