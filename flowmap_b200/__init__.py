@@ -23,6 +23,9 @@ def install() -> dict:
         so ``compute_bidirectional_flow`` runs on the kernels with the reference's predictor),
       * ``flowmap.export.colmap.export_to_colmap / write_colmap_model / read_colmap_model``
         (when that module imports; it needs ``plyfile``),
+      * ``flowmap.misc.ate.compute_ate`` -> flowmap_b200.ate.compute_ate, also the copy in
+        ``flowmap.visualization.visualizer_trajectory`` (when that module imports; it needs
+        ``matplotlib``),
 
     so that ``flowmap/overfit.py`` (Hydra/Lightning harness) runs unchanged.  Call it before
     ``flowmap.overfit`` is imported.  Backbones that are outside the hot path (MiDaS) keep
@@ -84,6 +87,16 @@ def install() -> dict:
             setattr(ref_colmap, name, getattr(my_export, name))
     except ImportError:
         pass
+    from . import ate as my_ate
+    # misc.ate and the copy visualization.visualizer_trajectory imported by name (that module needs
+    # matplotlib)
+    for mod in ("flowmap.misc.ate", "flowmap.visualization.visualizer_trajectory"):
+        try:
+            ref = importlib.import_module(mod)
+        except ImportError:
+            continue
+        replaced[f"{mod}.compute_ate"] = ref.compute_ate
+        ref.compute_ate = my_ate.compute_ate
     ref_back = importlib.import_module("flowmap.model.backbone")
     for key, cls in ref_back.BACKBONES.items():  # e.g. midas: produced by the reference
         my_model.BACKBONES.setdefault(key, cls)

@@ -47,6 +47,7 @@ SIGNATURES = {
                                      _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "fm_pose_chain": (c_int, [_P, _P, c_int, c_int, _P]),
     "fm_pose_chain_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, _P]),
+    "fm_trajectory_ate": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
     "fm_track_workspace_bytes": (c_size_t, [c_int, ctypes.c_longlong]),
     "fm_track_loss_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, ctypes.c_longlong,
                                   c_int, c_float, c_float, _P, _P, c_int, c_int, c_int, _P]),
@@ -104,7 +105,9 @@ class OverfitStepArgs(ctypes.Structure):
                 ("track_loss", _P),
                 ("ws", _P), ("track_ws", _P), ("focal_step", c_int), ("defer_adam", c_int),
                 ("phase", c_int), ("splat_plan", _P), ("splat_overflow_max", ctypes.c_uint),
-                ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P)]
+                ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P),
+                ("gt_positions", _P), ("gt_fx", c_float), ("gt_fy", c_float), ("metrics_log", _P),
+                ("metrics_capacity", c_int)]
 
 
 SIGNATURES["fm_overfit_step"] = (c_int, [ctypes.POINTER(OverfitStepArgs), _P])

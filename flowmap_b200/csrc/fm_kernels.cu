@@ -27,6 +27,7 @@
 #include <stdlib.h>
 
 #include "../../include/flowmap_b200.h"
+#include "fm_ate.cuh"
 #include "fm_host.h"
 #include "fm_pixel.cuh"
 
@@ -2260,6 +2261,79 @@ __global__ void k_clock_tick(StepClock* c, double lr, double b1, double b2, unsi
   c->seed = z ^ (z >> 31);
 }
 
+// ================================================================== trajectory metrics
+// scipy.spatial.procrustes ATE (fm_ate.cuh), one block per trajectory.  The block size fixes the
+// order of the float64 sums, so a trajectory's result does not depend on how it was batched, nor on
+// whether the fused step or fm_trajectory_ate evaluated it.
+constexpr int kAteThreads = 128;
+
+// Sums up to 9 doubles over the block; every thread receives the totals (in the same order).
+struct BlockSum {
+  double* sh;  // [kAteThreads / 32][9] shared
+  __device__ void operator()(double* v, int n) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int k = 0; k < n; ++k) {
+      v[k] = warp_sum(v[k]);
+      if (lane == 0) sh[warp * 9 + k] = v[k];
+    }
+    __syncthreads();
+    for (int k = 0; k < n; ++k) {
+      double t = 0.0;
+      for (int w = 0; w < kAteThreads / 32; ++w) t += sh[w * 9 + k];
+      v[k] = t;
+    }
+    __syncthreads();
+  }
+};
+
+// The row of the fused step's metrics ring (fm_overfit_step_args.metrics_log) that the block also
+// writes; log == NULL for plain fm_trajectory_ate.
+struct MetricsRow {
+  float* log;
+  int capacity;
+  const StepClock* clock;
+  const float *loss, *track_loss, *k4;  // track_loss NULL: no tracking loss in this step
+  float gt_fx, gt_fy;
+};
+
+__global__ void __launch_bounds__(kAteThreads)
+k_trajectory_ate(const float* __restrict__ gt, const float* __restrict__ pred, int pred_stride, int pred_cstride, int F,
+                 float* __restrict__ ate, float* __restrict__ aligned_gt, float* __restrict__ aligned_pred,
+                 int* __restrict__ status, MetricsRow row) {
+  __shared__ double s_red[kAteThreads / 32 * 9];
+  const size_t t = blockIdx.x;
+  float* ate_out = ate ? ate + t : nullptr;
+  if (row.log) {  // the fused step: columns flow loss, tracking loss, |fx error|, |fy error|, ATE
+    float* r = row.log + (size_t)((row.clock->step - 1u) % (unsigned)row.capacity) * 5;
+    if (threadIdx.x == 0) {
+      double fx = 0.0, fy = 0.0;
+      for (int f = 0; f < F; ++f) { fx += (double)row.k4[f * 4 + 0]; fy += (double)row.k4[f * 4 + 1]; }
+      r[0] = *row.loss;
+      r[1] = row.track_loss ? *row.track_loss : 0.f;
+      r[2] = (float)fabs((double)row.gt_fx - fx / F);
+      r[3] = (float)fabs((double)row.gt_fy - fy / F);
+      if (!gt) r[4] = NAN;
+    }
+    if (!gt) return;
+    ate_out = r + 4;
+  }
+  AtePoints x;
+  x.gt = gt + t * F * 3;
+  x.pred = pred + t * F * pred_stride;
+  x.gt_stride = 3;
+  x.pred_stride = pred_stride;
+  x.pred_cstride = pred_cstride;
+  x.F = F;
+  BlockSum red{s_red};
+  double v;
+  const int st = trajectory_ate(x, threadIdx.x, kAteThreads, red, v, aligned_gt ? aligned_gt + t * F * 3 : nullptr,
+                                aligned_pred ? aligned_pred + t * F * 3 : nullptr);
+  if (threadIdx.x == 0) {
+    *ate_out = (float)v;
+    if (status) status[t] = st;
+  }
+}
+
 // ================================================================== fused overfit step helpers
 // focal_lengths_to_intrinsics (intrinsics/common.py:6-20) for a shared focal length, as k4 rows.
 __global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restrict__ k4, int BF, int H, int W) {
@@ -2503,7 +2577,7 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 101; }
+int fm_version(void) { return 102; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -2805,6 +2879,18 @@ int fm_pose_chain(const float* rt, float* extrinsics, int B, int F, void* stream
   if (!rt || !extrinsics || B < 1 || F < 2) return fail_msg("fm_pose_chain: bad arguments");
   k_pose_chain<<<B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, B, F);
   FM_CHECK_LAUNCH("fm_pose_chain");
+  return 0;
+}
+
+int fm_trajectory_ate(const float* gt, const float* pred, int T, int F, float* ate, float* aligned_gt,
+                      float* aligned_pred, int* status, void* stream) {
+  if (!gt || !pred || !ate || !status || T < 0 || F < 1) return fail_msg("fm_trajectory_ate: bad arguments");
+  if (T == 0) return 0;
+  MetricsRow none;
+  memset(&none, 0, sizeof(none));
+  k_trajectory_ate<<<T, kAteThreads, 0, (cudaStream_t)stream>>>(gt, pred, 3, 1, F, ate, aligned_gt, aligned_pred,
+                                                                status, none);
+  FM_CHECK_LAUNCH("fm_trajectory_ate");
   return 0;
 }
 
@@ -3196,12 +3282,13 @@ int fm_softmin_focal_bwd(const float* softmin, const float* cand_focal, const fl
 struct SideLane { cudaStream_t stream; cudaEvent_t fork, join; int state; };  // state 0 new, 1 ready, -1 unavailable
 // One lane per (host thread, device): a thread's calls are sequential, so its events are never
 // re-recorded while a wait on them is still to be issued; other threads have their own.  The lane is
-// created on the first call with tracks (an eager warm-up step, not inside a capture).
-static SideLane* side_lane() {
-  static thread_local SideLane lanes[64];
+// created on the first call that uses it (an eager warm-up step, not inside a capture).  Lane 0
+// carries the tracking work, lane 1 the metrics log, which overlaps all of it.
+static SideLane* side_lane(int which = 0) {
+  static thread_local SideLane lanes[2][64];
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  SideLane& l = lanes[dev];
+  SideLane& l = lanes[which][dev];
   if (l.state == 0) {
     const bool ok = cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking) == cudaSuccess &&
                     cudaEventCreateWithFlags(&l.fork, cudaEventDisableTiming) == cudaSuccess &&
@@ -3219,6 +3306,8 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
+  if (a->metrics_log && (a->phase != FM_STEP_ALL || !a->clock || !a->extrinsics || a->metrics_capacity < 1))
+    return fail_msg("fm_overfit_step: metrics_log needs FM_STEP_ALL, a clock, extrinsics and metrics_capacity >= 1");
   cudaStream_t s = (cudaStream_t)stream;
   const int F = a->F, H = a->H, W = a->W, BP = F - 1;
   const size_t N = (size_t)H * W;
@@ -3273,6 +3362,34 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
         if ((e = cudaStreamWaitEvent(s, fwd_lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
       }
     }
+  }
+  // The metrics row of this step (model_wrapper_overfit.py:63-71 and metrics/ate): it reads only what
+  // the forward half produced and the rest of the step does not change (losses, k4, chained poses), so
+  // it runs on its own lane beside the backward and Adam and is joined before the call returns.
+  SideLane* mlane = nullptr;
+  if (a->metrics_log) {
+    mlane = side_lane(1);
+    cudaStream_t ms = s;
+    if (mlane) {
+      if ((e = cudaEventRecord(mlane->fork, s)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
+      if ((e = cudaStreamWaitEvent(mlane->stream, mlane->fork, 0)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
+      ms = mlane->stream;
+    }
+    // the camera centres: the tracking loss chained the poses already, a flow-only step chains them here
+    if (!a->tracks && (rc = fm_pose_chain(a->rt, a->extrinsics, 1, F, ms))) return rc;
+    MetricsRow row;
+    row.log = a->metrics_log;
+    row.capacity = a->metrics_capacity;
+    row.clock = (const StepClock*)a->clock;
+    row.loss = a->loss;
+    row.track_loss = a->tracks ? a->track_loss : nullptr;
+    row.k4 = k4;
+    row.gt_fx = a->gt_fx;
+    row.gt_fy = a->gt_fy;
+    k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr, nullptr,
+                                                nullptr, row);
+    FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
+    if (mlane && (e = cudaEventRecord(mlane->join, mlane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   }
   if (a->phase == FM_STEP_FORWARD) return 0;
   // d total / d (flow loss) and d total / d (tracking loss) of a split step (device scalars, NULL = 1)
@@ -3352,6 +3469,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
   }
   if (defer && a->step > 0 && a->weight_logits && !fuse_w) return fail_msg("fm_overfit_step: defer_adam needs the fused weight update");
+  if (mlane && (e = cudaStreamWaitEvent(s, mlane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   return 0;
 }
 

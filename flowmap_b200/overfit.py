@@ -243,6 +243,7 @@ class FusedOverfitter(Overfitter):
             a.track_g_k4, a.track_loss, a.track_ws = P(self._tg_k4), P(self._track_loss), P(self._tws)
         self._args, self._ctypes = a, ctypes
         self._lib = lib()
+        self._mlog = None  # per-step metrics ring (enable_metrics_log)
 
     def _set_plan_args(self, a):
         pl = self._plan
@@ -472,15 +473,20 @@ class FusedOverfitter(Overfitter):
             self._clock.tick(tick_focal=not sweep)
         a.tracks = self._ctypes.pointer(self._pk_c) if track_on else None
         a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
-        if sweep:
-            self._step_softmin(update)
-        else:
-            a.focal = self._focal.data_ptr()
-            a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
-            with torch.cuda.device(self.rt.device):
-                check(self._lib.fm_overfit_step(self._ctypes.byref(a),
-                                                torch.cuda.current_stream().cuda_stream),
-                      "fm_overfit_step")
+        # the metrics row is indexed by the step clock, which only update steps advance
+        a.metrics_log = self._mlog.data_ptr() if (update and self._mlog is not None) else None
+        try:
+            if sweep:
+                self._step_softmin(update)
+            else:
+                a.focal = self._focal.data_ptr()
+                a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
+                with torch.cuda.device(self.rt.device):
+                    check(self._lib.fm_overfit_step(self._ctypes.byref(a),
+                                                    torch.cuda.current_stream().cuda_stream),
+                          "fm_overfit_step")
+        finally:
+            a.metrics_log = None
         if track_on:
             torch.add(self._loss, self._track_loss, out=self._total)
         else:
@@ -546,6 +552,56 @@ class FusedOverfitter(Overfitter):
         """(F, 4) = (fx, fy, cx, cy) used by the last step."""
         return self._k4
 
+    METRIC_NAMES = ("train/loss/flow", "train/loss/tracking", "train/intrinsics/fx_error",
+                    "train/intrinsics/fy_error", "metrics/ate")
+
+    def enable_metrics_log(self, capacity: int):
+        """Log, from inside every update step, what the reference logs for it: the weighted flow and
+        tracking losses (loss.py:40: 0 before the tracking loss is enabled), the focal-length errors
+        (model_wrapper_overfit.py:63-71) against the frame means of `batch.intrinsics`, and the ATE of
+        the step's camera centres against `batch.extrinsics[0, :, :3, 3]` (metrics/ate of
+        VisualizerTrajectory, scipy.spatial.procrustes semantics, fm_trajectory_ate).  Columns without
+        ground truth are NaN.  The rows live in a device ring of `capacity` steps, written without host
+        synchronisation; read them with metrics_log().
+
+        Row k describes update k (0-based, global_step = k when it ran): the poses and intrinsics that
+        update evaluated, before its Adam step -- the values the reference's training_step logs at
+        global_step k.  The reference's validation after update k (experiment/dump_ate.yaml's
+        val_check_interval: 1) evaluates the updated parameters: that is row k + 1."""
+        if capacity < 1:
+            raise ValueError("flowmap_b200: the metrics log needs a capacity >= 1")
+        b, dev = self.batch, self.rt.device
+        _, f, _, _, _ = b.videos.shape
+        nan = float("nan")
+        self._mlog_gt = None if b.extrinsics is None else \
+            b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
+        if b.intrinsics is None:
+            fx = fy = nan
+        else:
+            k = b.intrinsics[0].double()
+            fx, fy = float(k[:, 0, 0].mean()), float(k[:, 1, 1].mean())
+        if getattr(self, "_ext", None) is None:  # flow-only steps chain the poses for the log
+            self._ext = torch.empty(1, f, 4, 4, device=dev)
+        self._mlog = torch.full((capacity, 5), nan, device=dev)
+        self._mlog_first = self.optimizer_steps
+        a = self._args
+        a.extrinsics = self._ext.data_ptr()
+        a.gt_positions = None if self._mlog_gt is None else self._mlog_gt.data_ptr()
+        a.gt_fx, a.gt_fy, a.metrics_capacity = fx, fy, capacity
+        self._graphs.clear()  # captured steps were recorded without the log
+        self._eager_runs.clear()
+
+    def metrics_log(self) -> dict:
+        """The logged rows of the update steps run since enable_metrics_log (the last `capacity` of
+        them), in step order, as CPU float32 tensors keyed by the reference's log names.  One host
+        synchronisation."""
+        if self._mlog is None:
+            raise ValueError("flowmap_b200: the metrics log is off (enable_metrics_log)")
+        cap = self._mlog.shape[0]
+        steps = torch.arange(max(self._mlog_first, self.optimizer_steps - cap), self.optimizer_steps)
+        rows = self._mlog[(steps % cap).to(self._mlog.device)].cpu()
+        return {name: rows[:, i] for i, name in enumerate(self.METRIC_NAMES)}
+
 
 class ShardedFusedOverfitter(FusedOverfitter):
     """Pair-sharded :class:`FusedOverfitter` (flowmap_b200.parallel, SURVEY 8(e)).
@@ -597,6 +653,10 @@ class ShardedFusedOverfitter(FusedOverfitter):
             self._tws = torch.empty(lib().fm_track_workspace_bytes(F, pk.total), dtype=torch.uint8, device=dev)
             self._treduce = self._tws[:lib().fm_track_reduce_bytes(F)].view(torch.float64)
             self._src_range = parallel.source_frame_range(plan)
+
+    def enable_metrics_log(self, capacity: int):
+        raise ValueError("flowmap_b200: the per-step metrics log covers the single-GPU FusedOverfitter; a "
+                         "pair-sharded rank holds only part of the trajectory")
 
     def _mask_sum(self, flows: Flows) -> Tensor:
         from . import parallel

@@ -166,6 +166,16 @@ int fm_pose_chain(const float* rt, float* extrinsics, int B, int F, void* stream
 int fm_pose_chain_bwd(const float* rt, const float* extrinsics, const float* g_extrinsics,
                       float* g_rt, int B, int F, void* stream);
 
+/* misc/ate.py:7-25 compute_ate (scipy.spatial.procrustes) on T independent trajectories of F points,
+ * gt / pred (T, F, 3), one block per trajectory, float64 inside: both sets centred and scaled to unit
+ * Frobenius norm, R = U V^T from the SVD of gt^T pred (reflections allowed), s = sum of the singular
+ * values; aligned_pred = s * pred R^T, ate[t] = sqrt(mean((aligned_gt - aligned_pred)^2)).
+ * aligned_gt / aligned_pred (T, F, 3) may be NULL.  status[t] = 0, or 1 where scipy raises "Input
+ * matrices must contain >1 unique points" (a set is exactly one point after centring in float64);
+ * ate[t] is NaN then.  No host synchronisation.  A trajectory's results do not depend on T. */
+int fm_trajectory_ate(const float* gt, const float* pred, int T, int F, float* ate, float* aligned_gt,
+                      float* aligned_pred, int* status, void* stream);
+
 /* loss_tracking.py:28-61 LossTracking + projection.py:255-298 compute_track_flow, all
  * segments in one launch (batch size 1, as tracking/__init__.py:92-93 asserts).
  * Packing: samples of segment s are stored row-major (frame row, point) starting at
@@ -342,6 +352,18 @@ typedef struct {
                                     same principal points as k4, any focal lengths): the step then starts at the
                                     pose solve and rescales the sums to its own K.  Lets the caller run the
                                     moment pass beside the work that produces the focal length (the softmin sweep). */
+  /* Per-step metrics log (model_wrapper_overfit.py:63-71 train/loss/<name>, train/intrinsics/f[xy]_error;
+     visualizer_trajectory.py metrics/ate).  metrics_log == NULL: off.  Otherwise (needs FM_STEP_ALL, `clock`
+     and `extrinsics`) the step writes row (clock.step - 1) mod metrics_capacity of the (metrics_capacity, 5)
+     float ring: weighted flow loss, weighted tracking loss (0 without tracks), |gt_fx - mean_f k4[f,0]|,
+     |gt_fy - mean_f k4[f,1]|, and fm_trajectory_ate of the translations of the chained poses (written to
+     `extrinsics`, also without tracks) against gt_positions.  The row describes the parameters this step
+     evaluated, before its Adam update.  It is computed on a side stream beside the backward half: one
+     extra launch with tracks, two without (the pose chain). */
+  const float* gt_positions;     /* (F,3) ground-truth camera centres, or NULL: ATE column is NaN */
+  float gt_fx, gt_fy;            /* frame means of the normalised GT intrinsics, NaN: columns NaN */
+  float* metrics_log;            /* (metrics_capacity, 5) ring, or NULL = off */
+  int metrics_capacity;
 } fm_overfit_step_args;
 #define FM_STEP_ALL 0
 #define FM_STEP_FORWARD 1
