@@ -5,6 +5,7 @@
 // pair-pixel + 8 B per frame-pixel (SURVEY 8(d)).
 //
 // Version-1 structure (one launch per phase over all pairs):
+//   k_pair_shift   phase A0 per-pair conditioning shift: weighted mean depth of 32 x 32 samples
 //   k_moments      phase A  weighted moment sums per pair (bilinear gather of the earlier
 //                           frame at xy + backward flow), fp32 per thread -> fp64 block
 //                           reduction -> fp64 atomics                (projection.py:213-249)
@@ -67,6 +68,8 @@ struct Workspace {
   double* loss;      // [4]
   PairState* state;  // [BP]
   PairAdjoint* adj;  // [BP]
+  float* zshift;     // [BP] conditioning shift of the moment pass (k_pair_shift)
+  float* pshift;     // [BP][3] conditioning shift of explicit point sets (k_points_shift)
   size_t bytes;
 };
 
@@ -83,6 +86,8 @@ Workspace carve(void* base, int B, int F) {
   w.loss = (double*)(p + off); off = align_up(off + 4 * sizeof(double), 256);
   w.state = (PairState*)(p + off); off = align_up(off + BP * sizeof(PairState), 256);
   w.adj = (PairAdjoint*)(p + off); off = align_up(off + BP * sizeof(PairAdjoint), 256);
+  w.zshift = (float*)(p + off); off = align_up(off + BP * sizeof(float), 256);
+  w.pshift = (float*)(p + off); off = align_up(off + BP * 3 * sizeof(float), 256);
   w.bytes = off;
   return w;
 }
@@ -324,14 +329,46 @@ __device__ __forceinline__ PairAddr pair_addr(const PairLayout& l, int pair, int
   a.weight = rb * l.weight_bs + (long long)i * N;
   return a;
 }
-__device__ __forceinline__ PairGeom pair_geom(const float* depth, const float* k4, const PairAddr& pa,
-                                              int H, int W) {
+// z0: the pair's stored conditioning shift (the forward reads it from Workspace::zshift, the
+// backward from its PairAdjoint, which the solve filled from the same value).
+__device__ __forceinline__ PairGeom pair_geom(const float* k4, const PairAddr& pa, int H, int W, float z0) {
   PairGeom g;
   g.ka = make_cam(load_k4(k4, pa.k4_frame_a));
   g.kb = make_cam(load_k4(k4, pa.k4_frame_a + 1));
   g.grid = make_grid(H, W);
-  g.z0 = __ldg(depth + pa.depth_a + (size_t)H * W + (size_t)(H / 2) * W + W / 2);
+  g.z0 = z0;
   return g;
+}
+
+// The conditioning shift of every moment pair (shift_sample / shift_from_sums in fm_pixel.cuh): one
+// block per pair, kShiftSamples gathers of the later frame's depth and the pair's weights.
+__global__ void __launch_bounds__(kThreads)
+k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
+             float* __restrict__ zshift, PairLayout lay, int H, int W) {
+  __shared__ double smem[3][kThreads / 32];
+  const int pair = blockIdx.x, N = H * W;
+  const PairAddr pa = pair_addr(lay, pair, N);
+  const float* db = depth + pa.depth_a + N;
+  const float* wt = weights ? weights + pa.weight : nullptr;
+  double s[3] = {0.0, 0.0, 0.0};  // w z, w, z
+  for (int i = threadIdx.x; i < kShiftSamples; i += kThreads) {
+    const int j = shift_sample(i, H, W);
+    const double z = (double)__ldg(db + j), w = wt ? (double)weight_of(__ldg(wt + j), wsens) : 1.0;
+    s[0] += w * z; s[1] += w; s[2] += z;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double v = warp_sum(s[k]);
+    if (lane == 0) smem[k][warp] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[3] = {0.0, 0.0, 0.0};
+    for (int k = 0; k < 3; ++k)
+      for (int w = 0; w < kThreads / 32; ++w) t[k] += smem[k][w];
+    zshift[pair] = shift_from_sums(t[0], t[1], t[2]);
+  }
 }
 
 template <int VEC>
@@ -339,12 +376,12 @@ __global__ void __launch_bounds__(kThreads, 3)
 k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
           const float* __restrict__ bflow, const float* __restrict__ weights,
           const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
-          float wsens, PairLayout lay, int H, int W) {
+          const float* __restrict__ zshift, float wsens, PairLayout lay, int H, int W) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int pair = blockIdx.y;
   const int N = H * W;
   const PairAddr pa = pair_addr(lay, pair, N);
-  const PairGeom g = pair_geom(depth, k4, pa, H, W);
+  const PairGeom g = pair_geom(k4, pa, H, W, __ldg(zshift + pair));
   const float* da = opaque_ptr(depth + pa.depth_a);
   const float* db = da + N;
   const float* fl = bflow + pa.flow;
@@ -374,7 +411,8 @@ template <int VEC, int LX>
 __global__ void __launch_bounds__(kThreads, 3)
 k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
                 const float* __restrict__ bflow, const float* __restrict__ weights,
-                double* __restrict__ moments, float wsens, PairLayout lay, int H, int W, int BP, int rounds) {
+                double* __restrict__ moments, const float* __restrict__ zshift, float wsens, PairLayout lay,
+                int H, int W, int BP, int rounds) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int N = H * W;
   constexpr int kChunk = kThreads * VEC;
@@ -389,7 +427,7 @@ k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
     const int pair = i / chunks, cb = i - pair * chunks;
     const int ce = (cb + (range.i1 - i) < chunks) ? cb + (range.i1 - i) : chunks;
     const PairAddr pa = pair_addr(lay, pair, N);
-    const PairGeom g = pair_geom(depth, k4, pa, H, W);
+    const PairGeom g = pair_geom(k4, pa, H, W, __ldg(zshift + pair));
     const float* da = opaque_ptr(depth + pa.depth_a);
     const float* db = da + N;
     const float* fl = bflow + pa.flow;
@@ -443,14 +481,14 @@ k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
 // other focal lengths) before the step's own K was known.  Points scale per axis with the focal
 // ratio (p = S_b p', q = S_a q', S = diag(fx'/fx, fy'/fy, 1); the conditioning shift is along z), so
 // the 16 sums are rescaled exactly here -- and written back for later readers of the workspace.
-__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ depth,
+__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ zshift,
                         float* __restrict__ rt, PairState* __restrict__ state, int BP, PairLayout lay,
                         int H, int W, const float* __restrict__ moments_k4 = nullptr,
                         const float* __restrict__ k4 = nullptr) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   const PairAddr pa = pair_addr(lay, pair, H * W);
-  const double z0 = (double)__ldg(depth + pa.depth_a + (size_t)H * W + (size_t)(H / 2) * W + W / 2);
+  const double z0 = (double)zshift[pair];  // the shift the moment pass used
   double m[kNumMoments];
   for (int k = 0; k < kNumMoments; ++k) m[k] = moments[(size_t)pair * kNumMoments + k];
   if (moments_k4) {
@@ -809,7 +847,7 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4,
   __syncthreads();
   const PairAdjoint ad = s_adj;
   const PairAddr pa = pair_addr(lay, pair, N);
-  const PairGeom g = pair_geom(depth, k4, pa, H, W);
+  const PairGeom g = pair_geom(k4, pa, H, W, ad.shift[2]);
   const int a = pa.k4_frame_a;
   if (adam.on && adam.consts) { adam.step_size = __ldg(adam.consts); adam.bc2_sqrt = __ldg(adam.consts + 1); }
   const float* da = opaque_ptr(depth + pa.depth_a);
@@ -934,7 +972,7 @@ k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4
     __syncthreads();
     const PairAdjoint ad = s_adj;
     const PairAddr pa = pair_addr(lay, pair, N);
-    const PairGeom g = pair_geom(depth, k4, pa, H, W);
+    const PairGeom g = pair_geom(k4, pa, H, W, ad.shift[2]);
     const float* da = opaque_ptr(depth + pa.depth_a);
     float* gda = g_depth + pa.depth_a;
     auto scatter = [gda, W](int y0, int x0, float v0, float v1) { red_pair<false>(gda + y0 * W, x0, W, v0, v1); };
@@ -1052,7 +1090,7 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
     if (threadIdx.x < sizeof(PairAdjoint) / 4)
       reinterpret_cast<float*>(&s_adj)[threadIdx.x] = reinterpret_cast<const float*>(adj + pair)[threadIdx.x];
     if (threadIdx.x == 32) {
-      const PairGeom pg = pair_geom(depth, k4, pa, H, W);
+      const PairGeom pg = pair_geom(k4, pa, H, W, adj[pair].shift[2]);
       s_geom = pg;
       const int e = fix_exponent(tap_magnitude(adj[pair], pg));
       s_fix[0] = fix_pow2(e);
@@ -1935,14 +1973,13 @@ __global__ void k_sweep_base_k4(const float* __restrict__ cand_k4, float* __rest
   base_k4[t] = cand_k4[(size_t)b * n * 8 + e];  // frames 0/1 of candidate 0
 }
 
-__global__ void k_sweep_scale_solve(const double* __restrict__ base_moments, const float* __restrict__ depth,
+__global__ void k_sweep_scale_solve(const double* __restrict__ base_moments, const float* __restrict__ base_zshift,
                                     const float* __restrict__ cand_k4, float* __restrict__ rt,
-                                    PairState* __restrict__ state, int B, int n, PairLayout lay, int H, int W) {
+                                    PairState* __restrict__ state, int B, int n) {
   const int item = blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= B * n) return;
   const int b = item / n;
-  const PairAddr pa = pair_addr(lay, item, H * W);
-  const double z0 = (double)__ldg(depth + pa.depth_a + (size_t)H * W + (size_t)(H / 2) * W + W / 2);
+  const double z0 = (double)base_zshift[b];  // the shift of the real pair's moment pass (along z: S_n keeps it)
   const double sx = (double)cand_k4[(size_t)b * n * 8 + 0] / (double)cand_k4[(size_t)item * 8 + 0];
   const double sy = (double)cand_k4[(size_t)b * n * 8 + 1] / (double)cand_k4[(size_t)item * 8 + 1];
   const double sc[3] = {sx, sy, 1.0};
@@ -2109,30 +2146,67 @@ __global__ void k_softmin_focal_bwd(const float* __restrict__ sm, const float* _
 // ================================================================== standalone API kernels
 // flowmap/model/procrustes.py:7-51 on explicit point sets (*batch, n, 3): moments -> solve ->
 // [R|t]; backward: closed-form per-point adjoints.  One item per blockIdx.y.
+//
+// Conditioning shift of an item: the weighted mean of (p + q) / 2 over up to kShiftSamples evenly
+// spaced points (unweighted if their weights sum to zero), subtracted from p and q before the
+// moments, as the image path subtracts its z0.  One block per item.
+__global__ void __launch_bounds__(kThreads)
+k_points_shift(const float* __restrict__ p, const float* __restrict__ q, const float* __restrict__ w,
+               float* __restrict__ shift, int n) {
+  __shared__ double smem[7][kThreads / 32];
+  const int item = blockIdx.x;
+  const int cnt = n < kShiftSamples ? n : kShiftSamples;
+  double s[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // w c (3), w, c (3)
+  for (int i = threadIdx.x; i < cnt; i += kThreads) {
+    const long long j = (long long)i * n / cnt;
+    const size_t o = ((size_t)item * n + j) * 3;
+    const double wj = (double)__ldg(w + (size_t)item * n + j);
+    for (int c = 0; c < 3; ++c) {
+      const double m = 0.5 * ((double)__ldg(p + o + c) + (double)__ldg(q + o + c));
+      s[c] += wj * m; s[4 + c] += m;
+    }
+    s[3] += wj;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 7; ++k) {
+    const double v = warp_sum(s[k]);
+    if (lane == 0) smem[k][warp] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int k = 0; k < 7; ++k)
+      for (int v = 0; v < kThreads / 32; ++v) t[k] += smem[k][v];
+    for (int c = 0; c < 3; ++c) shift[item * 3 + c] = shift_from_sums(t[c], t[3], t[4 + c], cnt);
+  }
+}
+
 __global__ void __launch_bounds__(kThreads)
 k_points_moments(const float* __restrict__ p, const float* __restrict__ q, const float* __restrict__ w,
-                 double* __restrict__ moments, int n) {
+                 const float* __restrict__ shift, double* __restrict__ moments, int n) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int item = blockIdx.y;
+  const float c0 = __ldg(shift + item * 3), c1 = __ldg(shift + item * 3 + 1), c2 = __ldg(shift + item * 3 + 2);
   float acc[kNumMoments];
 #pragma unroll
   for (int i = 0; i < kNumMoments; ++i) acc[i] = 0.f;
   for (int j = blockIdx.x * kThreads + threadIdx.x; j < n; j += gridDim.x * kThreads) {
     const size_t o = ((size_t)item * n + j) * 3;
-    const float pp[3] = {__ldg(p + o), __ldg(p + o + 1), __ldg(p + o + 2)};
-    const float qq[3] = {__ldg(q + o), __ldg(q + o + 1), __ldg(q + o + 2)};
+    const float pp[3] = {__ldg(p + o) - c0, __ldg(p + o + 1) - c1, __ldg(p + o + 2) - c2};
+    const float qq[3] = {__ldg(q + o) - c0, __ldg(q + o + 1) - c1, __ldg(q + o + 2) - c2};
     moments_add(acc, __ldg(w + (size_t)item * n + j), pp, qq);
   }
   block_accumulate<kNumMoments>(acc, moments + (size_t)item * kNumMoments, smem);
 }
 
-__global__ void k_points_solve(const double* __restrict__ moments, float* __restrict__ rt,
-                               PairState* __restrict__ state, int items) {
+__global__ void k_points_solve(const double* __restrict__ moments, const float* __restrict__ pshift,
+                               float* __restrict__ rt, PairState* __restrict__ state, int items) {
   const int item = blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= items) return;
   double m[kNumMoments];
   for (int k = 0; k < kNumMoments; ++k) m[k] = moments[(size_t)item * kNumMoments + k];
-  const double shift[3] = {0.0, 0.0, 0.0};
+  const double shift[3] = {(double)pshift[item * 3], (double)pshift[item * 3 + 1], (double)pshift[item * 3 + 2]};
   PairState st;
   float out[12];
   procrustes_solve(m, shift, out, st);
@@ -2148,8 +2222,11 @@ k_points_distribute(const float* __restrict__ p, const float* __restrict__ q, co
   const PairAdjoint ad = adj[item];
   for (int j = blockIdx.x * kThreads + threadIdx.x; j < n; j += gridDim.x * kThreads) {
     const size_t o = ((size_t)item * n + j) * 3;
-    const float dp[3] = {__ldg(p + o) - ad.pbar[0], __ldg(p + o + 1) - ad.pbar[1], __ldg(p + o + 2) - ad.pbar[2]};
-    const float dq[3] = {__ldg(q + o) - ad.qbar[0], __ldg(q + o + 1) - ad.qbar[1], __ldg(q + o + 2) - ad.qbar[2]};
+    // the shifted points of the moment pass minus their (shifted) centroids
+    const float dp[3] = {(__ldg(p + o) - ad.shift[0]) - ad.pbar[0], (__ldg(p + o + 1) - ad.shift[1]) - ad.pbar[1],
+                         (__ldg(p + o + 2) - ad.shift[2]) - ad.pbar[2]};
+    const float dq[3] = {(__ldg(q + o) - ad.shift[0]) - ad.qbar[0], (__ldg(q + o + 1) - ad.shift[1]) - ad.qbar[1],
+                         (__ldg(q + o + 2) - ad.shift[2]) - ad.qbar[2]};
     float wb, pb[3], qb[3];
     point_adjoint(ad, __ldg(w + (size_t)item * n + j), dp, dq, wb, pb, qb);
     gp[o] = pb[0]; gp[o + 1] = pb[1]; gp[o + 2] = pb[2];
@@ -2522,12 +2599,14 @@ bool tiled_shape_ok(int F, int H, int W) { return F >= 2 && W % 4 == 0 && H >= 1
 // Phase A through the plan: moments of all pairs (+ the step's correspondence weights into the
 // plan's scratch for phase D), then the solve.
 int launch_moments_tiled(const float* depth, const float* k4, const float* bflow, const float* weights, float wsens,
-                         const tiled::Plan& pl, double* moments, int F, int H, int W, cudaStream_t s) {
+                         const tiled::Plan& pl, double* moments, const float* zshift, int F, int H, int W,
+                         cudaStream_t s) {
   CUtensorMap tm;
   int rc = make_window_map(&tm, depth, W, H, F);
   if (rc) return rc;
   tiled::MomArgs b;
   b.depth = depth; b.k4 = k4; b.bflow = bflow; b.weights = weights; b.wscratch = pl.wscratch; b.moments = moments;
+  b.zshift = zshift;
   b.tinfo = pl.tiles; b.wsens = wsens; b.F = F; b.H = H; b.W = W; b.tiles_x = pl.tiles_x;
   b.tiles = pl.tiles_x * pl.tiles_y; b.n_items = (F - 1) * b.tiles;
   int grid = sm_count() * 3;
@@ -2646,35 +2725,37 @@ static int procrustes_fwd_impl(const float* depth, const float* k4, const float*
   if (moments_k4) {  // fm_procrustes_moments already ran with those intrinsics
     if (plan || indices || layout) return fail_msg("fm_procrustes_fwd: precomputed moments serve the dense path");
     if (!solve) return 0;
-    k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, depth, rt, w.state, BP, lay, H, W, moments_k4, k4);
+    k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, moments_k4, k4);
     FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
     return 0;
   }
   cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
+  k_pair_shift<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift");
   if (plan) {
     const tiled::Plan pl = tiled::plan_carve(plan, F, H, W);
-    const int rc = launch_moments_tiled(depth, k4, backward_flow, weights, wsens, pl, w.moments, F, H, W, s);
+    const int rc = launch_moments_tiled(depth, k4, backward_flow, weights, wsens, pl, w.moments, w.zshift, F, H, W, s);
     if (rc) return rc;
   } else if (indices) {
     dim3 grid(blocks_for_points(num_indices), BP);
-    k_moments<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, wsens, lay, H, W);
+    k_moments<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, w.zshift, wsens, lay, H, W);
   } else if (patch_shape_ok(H, W)) {
     const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
     const int pg = persistent_grid(3, items);
-    k_moments_dense<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
+    k_moments_dense<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
   } else if (W % 4 == 0) {
     const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
     const int pg = persistent_grid(3, items);
-    k_moments_dense<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
+    k_moments_dense<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
   } else {
     const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
     const int pg = persistent_grid(3, items);
-    k_moments_dense<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, wsens, lay, H, W, BP, procrustes_rounds(H, W, items / 4, pg, true));
+    k_moments_dense<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items / 4, pg, true));
   }
   if (!plan) FM_CHECK_LAUNCH("fm_procrustes_fwd: k_moments");
   if (!solve) return 0;
-  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, depth, rt, w.state, BP, lay, H, W);
+  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W);
   FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
   return 0;
 }
@@ -3103,10 +3184,12 @@ int fm_align_rigid_fwd(const float* p, const float* q, const float* weights, flo
   Workspace w = carve(ws, items, 2);
   cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)items * kNumMoments * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_align_rigid_fwd: memset", e);
+  k_points_shift<<<items, kThreads, 0, s>>>(p, q, weights, w.pshift, n);
+  FM_CHECK_LAUNCH("fm_align_rigid_fwd: k_points_shift");
   dim3 grid(blocks_for(n, 1), items);
-  k_points_moments<<<grid, kThreads, 0, s>>>(p, q, weights, w.moments, n);
+  k_points_moments<<<grid, kThreads, 0, s>>>(p, q, weights, w.pshift, w.moments, n);
   FM_CHECK_LAUNCH("fm_align_rigid_fwd: k_points_moments");
-  k_points_solve<<<(items + 63) / 64, 64, 0, s>>>(w.moments, rt, w.state, items);
+  k_points_solve<<<(items + 63) / 64, 64, 0, s>>>(w.moments, w.pshift, rt, w.state, items);
   FM_CHECK_LAUNCH("fm_align_rigid_fwd: k_points_solve");
   return 0;
 }
@@ -3193,14 +3276,17 @@ int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_
   if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
   k_sweep_base_k4<<<(B * 8 + 127) / 128, 128, 0, s>>>(cand_k4, base_k4, B, num_candidates);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_base_k4");
+  float* base_zshift = w.zshift + items;  // one conditioning shift per batch element, for all candidates
+  k_pair_shift<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, lay1, H, W);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_pair_shift");
   {  // ONE moment pass (candidate 0); every candidate's moments are a rescaling of it
     dim3 grid(blocks_for_points(num_indices), B);
     k_moments<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
-                                          base_moments, weight_sensitivity, lay1, H, W);
+                                          base_moments, base_zshift, weight_sensitivity, lay1, H, W);
     FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_moments");
   }
-  k_sweep_scale_solve<<<(items + 63) / 64, 64, 0, s>>>(base_moments, depth, cand_k4, rt, w.state, B,
-                                                      num_candidates, lay, H, W);
+  k_sweep_scale_solve<<<(items + 63) / 64, 64, 0, s>>>(base_moments, base_zshift, cand_k4, rt, w.state, B,
+                                                      num_candidates);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_scale_solve");
   e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);

@@ -17,6 +17,35 @@ struct PairGeom {
   float z0;  // conditioning shift (0, 0, z0) applied to p and q before accumulation
 };
 
+// The conditioning shift z0 of a pair: the mean of the later frame's depth over a fixed grid of
+// kShiftGrid x kShiftGrid pixels, weighted by the pair's correspondence weights (unweighted if
+// those sum to zero).  The moment sums cancel down to the covariance, so z0 has to be close to the
+// depth of the weighted cloud: one pixel is not (the image centre of a forward-moving video is the
+// far horizon, hundreds of times the foreground depth, at weight ~0).  Computed once per forward
+// and stored; the solve, the backward and the sweep's candidates read the stored value.
+constexpr int kShiftGrid = 32;
+constexpr int kShiftSamples = kShiftGrid * kShiftGrid;
+
+// Pixel (linear index) of sample i: cell centres of a kShiftGrid x kShiftGrid grid over the frame.
+FM_HD int shift_sample(int i, int H, int W) {
+  const int gy = i / kShiftGrid, gx = i - gy * kShiftGrid;
+  const int r = (int)(((long long)(2 * gy + 1) * H) / (2 * kShiftGrid));
+  const int c = (int)(((long long)(2 * gx + 1) * W) / (2 * kShiftGrid));
+  return r * W + c;
+}
+
+// z0 from the sums over `count` samples of w * depth, w and depth, rounded to 4 significant bits.  z0
+// only has to lie near the cloud's depth; a coarse value is also the same for weights that differ in
+// their last bits (the fused step's sigmoid and torch's, or two runs that differ by float atomics), so
+// the paths and runs round the moment sums identically.
+FM_HD float shift_from_sums(double swz, double sw, double sz, int count = kShiftSamples) {
+  const double z = sw > 0.0 ? swz / sw : sz / count;
+  if (!isfinite(z)) return 0.0f;
+  int e;
+  const double m = frexp(z, &e);
+  return (float)ldexp(round(m * 16.0) / 16.0, e);
+}
+
 // Later point p (frame b, pixel (r, c)) and earlier point q (frame a sampled at
 // xy + backward flow), both shifted by (0, 0, z0).  projection.py:222-242.
 template <typename LoadA>
@@ -504,7 +533,7 @@ FM_HD void distribute_point(const PairGeom& g, const PairAdjoint& ad, float x, f
 // Order of magnitude of the largest tap value distribute_point scatters for a pair, from its
 // constants alone (an estimate, not a bound): a tap value is a bilinear weight times
 // qb . (rx, ry, 1) with qb = w (Cbar dp + ad.qb), w <= 1, |dp| of the order of the depth times a
-// ray (the centre depth z0 stands in for the depth), and no ray component larger than R, the
+// ray (the conditioning depth z0, the weighted cloud's mean depth, stands in for the depth), and no ray component larger than R, the
 // largest over the image of either frame.
 FM_HD float ray_bound(const Cam& k) {
   return fmaxf(fmaxf(fabsf(k.cx), fabsf(1.0f - k.cx)) * fabsf(k.ifx),

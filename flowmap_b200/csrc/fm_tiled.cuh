@@ -469,6 +469,7 @@ __device__ __forceinline__ void q_from_taps(const Taps& t, const GridDims& grid,
 struct MomArgs {
   const float* depth; const float* k4; const float* bflow; const float* weights;
   float* wscratch; double* moments; const TileInfo* tinfo;
+  const float* zshift;  // [F - 1] conditioning shift per pair (k_pair_shift)
   float wsens;
   int F, H, W, tiles_x, tiles, n_items;
 };
@@ -539,7 +540,7 @@ k_moments_tiled(const __grid_constant__ CUtensorMap tm_depth, const MomArgs a) {
     if (pair != geom_pair) {
       g.ka = make_cam(load_k4(a.k4, pair));
       g.kb = make_cam(load_k4(a.k4, pair + 1));
-      g.z0 = __ldg(a.depth + (size_t)(pair + 1) * N + (size_t)(a.H / 2) * a.W + a.W / 2);
+      g.z0 = __ldg(a.zshift + pair);
       geom_pair = pair;
     }
     const float* da = a.depth + (size_t)pair * N;

@@ -26,6 +26,7 @@ softmin (intrinsics_softmin.py:129) and optim.Adam (model_wrapper_overfit.py:105
 
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
@@ -687,3 +688,52 @@ def flow_regime(kind: str, f: int, h: int, w: int, seed: int = 0, b: int = 1):
     elif kind != "iid":
         raise ValueError(kind)
     return depth, Flows(fwd.contiguous(), bwd.contiguous(), fl.forward_mask, fl.backward_mask), 0.85, None
+
+
+DEPTH_REGIMES = ("centre_far", "centre_far_weighted", "horizon", "centre_near", "scale_small", "scale_large",
+                 "corner_weights")
+
+
+def depth_regime(kind: str, f: int, h: int, w: int, seed: int = 0, b: int = 1):
+    """Float64 depth (b,f,h,w), Flows, focal and weight logits (b,f-1,h,w) for depth maps whose
+    centre pixel is not typical of the frame, and for depth scales and weight layouts far from the
+    defaults.  Everything starts from ``flow_regime("iid")`` with logits 0.01 N(0, 1); a logit of -1
+    is a weight of sigmoid(-100), about 0, and of +1 a weight of about 1 (sensitivity 100).
+
+    - ``centre_far``: pixel (h//2, w//2) of every frame at depth 1000, logits -1 on the 9 x 9 block
+      around it, so the outlier sits where the image centre is but takes no part in the fit;
+    - ``centre_far_weighted``: the same with ordinary weights on the block, so the outlier is fitted;
+    - ``horizon``: rows 0 .. h//2 + 2 (the centre pixel among them) at depth 200, the rows below at
+      1 + 2 U(0,1), logits -1 on the band and on the ceil(0.04 h) rows below it (whose flows reach
+      into it): the vanishing point of a forward-moving video;
+    - ``centre_near``: the centre pixel at 0.01, logits -1 on its 9 x 9 block;
+    - ``scale_small`` / ``scale_large``: the whole depth x 1e-2 / x 1e2 (a free gauge of FlowMap);
+    - ``corner_weights``: logits +1 on the top-left block of h//6 x w//5 pixels, -1 elsewhere, so
+      the weighted cloud sits far off the optical axis."""
+    depth, fl, focal, _ = flow_regime("iid", f, h, w, seed=seed, b=b)
+    g = torch.Generator().manual_seed(seed + 11)
+    logits = 0.01 * torch.randn(b, f - 1, h, w, generator=g, dtype=torch.float64)
+    cy, cx = h // 2, w // 2
+    block = (slice(max(cy - 4, 0), cy + 5), slice(max(cx - 4, 0), cx + 5))
+    if kind in ("centre_far", "centre_far_weighted"):
+        depth[:, :, cy, cx] = 1000.0
+        if kind == "centre_far":
+            logits[:, :, block[0], block[1]] = -1.0
+    elif kind == "horizon":
+        far = h // 2 + 3
+        depth[:, :, :far] = 200.0
+        depth[:, :, far:] = 1.0 + 2.0 * torch.rand(b, f, h - far, w, generator=g, dtype=torch.float64)
+        # weight ~0 also on the rows below the band whose backward flows (0.01 h px) reach into it: the
+        # 200-deep taps of their bilinear samples would make the fit ill-posed even in float64
+        logits[:, :, : far + math.ceil(0.04 * h)] = -1.0
+    elif kind == "centre_near":
+        depth[:, :, cy, cx] = 0.01
+        logits[:, :, block[0], block[1]] = -1.0
+    elif kind in ("scale_small", "scale_large"):
+        depth = depth * (1e-2 if kind == "scale_small" else 1e2)
+    elif kind == "corner_weights":
+        logits[:] = -1.0
+        logits[:, :, : max(h // 6, 1), : max(w // 5, 1)] = 1.0
+    else:
+        raise ValueError(kind)
+    return depth.contiguous(), fl, focal, logits.contiguous()

@@ -63,10 +63,14 @@ def errors(out, ref, per_item=True):
     return e
 
 
-def check(errs, noise, label, loss_tol, pose_tol, floor):
+def check(errs, noise, label, loss_tol, pose_tol, floor, relative_fixed=False):
     """Loss and poses against fixed tolerances; every gradient metric against
-    max(floor, 3 x the float32 oracle's own error in the same metric)."""
+    max(floor, 3 x the float32 oracle's own error in the same metric).  relative_fixed: the loss and
+    pose tolerances too become max(tol, 3 x the float32 oracle's error), for inputs so badly
+    conditioned that float32 itself misses the fixed ones."""
     print(label, "errors vs float64 oracle:", _fmt(errs), "| float32 oracle:", _fmt(noise))
+    if relative_fixed:
+        loss_tol, pose_tol = max(loss_tol, 3 * noise["loss"]), max(pose_tol, 3 * noise["pose"])
     assert errs["loss"] <= loss_tol, (label, "loss", errs["loss"])
     assert errs["pose"] <= pose_tol, (label, "pose", errs["pose"])
     for key in ("depth", "depth_border", "weights", "focal", "depth_frame", "weights_pair"):

@@ -19,13 +19,25 @@ static K4 k4_of(const float* k4, int frame) {
   return k;
 }
 
-static PairGeom geom(const float* depth, const float* k4, int pair, int F, int H, int W, int& a) {
+// z0: the pair's conditioning shift (pair_shift below in the forward, the saved state's in the backward)
+static PairGeom geom(const float* k4, int pair, int F, int H, int W, float z0, int& a) {
   int bi = pair / (F - 1), i = pair - bi * (F - 1);
   a = bi * F + i;
   PairGeom g;
   g.ka = make_cam(k4_of(k4, a)); g.kb = make_cam(k4_of(k4, a + 1)); g.grid = make_grid(H, W);
-  g.z0 = depth[(size_t)(a + 1) * H * W + (size_t)(H / 2) * W + W / 2];
+  g.z0 = z0;
   return g;
+}
+
+// k_pair_shift: the weighted mean depth of the later frame db over the shift samples (weights wt or 1)
+static float pair_shift(const float* db, const float* wt, int H, int W) {
+  double s[3] = {0, 0, 0};
+  for (int i = 0; i < kShiftSamples; ++i) {
+    const int j = shift_sample(i, H, W);
+    const double z = db[j], w = wt ? wt[j] : 1.0;
+    s[0] += w * z; s[1] += w; s[2] += z;
+  }
+  return shift_from_sums(s[0], s[1], s[2]);
 }
 
 extern "C" {
@@ -73,8 +85,10 @@ void emu_procrustes_fwd(const float* depth, const float* k4, const float* bflow,
                         int H, int W) {
   const int N = H * W, BP = B * (F - 1);
   for (int pair = 0; pair < BP; ++pair) {
+    const int bi = pair / (F - 1), a0 = bi * F + pair - bi * (F - 1);
+    const float z0 = pair_shift(depth + (size_t)(a0 + 1) * N, weights ? weights + (size_t)pair * N : nullptr, H, W);
     int a;
-    PairGeom g = geom(depth, k4, pair, F, H, W, a);
+    PairGeom g = geom(k4, pair, F, H, W, z0, a);
     const float* da = depth + (size_t)a * N; const float* db = da + N;
     double m[kNumMoments] = {0};
     const int cnt = indices ? n_idx : N;
@@ -191,10 +205,10 @@ void emu_procrustes_bwd(const float* depth, const float* k4, const float* bflow,
                         float* g_depth, float* g_weights, double* k4acc, int B, int F, int H, int W) {
   const int N = H * W, BP = B * (F - 1);
   for (int pair = 0; pair < BP; ++pair) {
-    int a;
-    PairGeom g = geom(depth, k4, pair, F, H, W, a);
     PairAdjoint ad;
     procrustes_adjoint(state[pair], g_rt + (size_t)pair * 12, ad);
+    int a;
+    PairGeom g = geom(k4, pair, F, H, W, ad.shift[2], a);
     const float* da = depth + (size_t)a * N; const float* db = da + N;
     float* gda = g_depth + (size_t)a * N; float* gdb = gda + N;
     const int cnt = indices ? n_idx : N;
