@@ -78,6 +78,9 @@ SIGNATURES = {
     "fm_step_clock_tick": (c_int, [_P, c_double, c_double, c_double, ctypes.c_ulonglong, c_int, _P]),
     "fm_adam_step_clock": (c_int, [_P, _P, _P, _P, c_size_t, _P, c_int, c_double, c_double, c_double, _P]),
     "fm_random_subset_clock": (c_int, [_P, ctypes.c_longlong, c_int, _P, _P]),
+    "fm_procrustes_moments_batched": (c_int, [_P, _P, _P, _P, c_float, _P, c_int, c_int, c_int, c_int, _P]),
+    "fm_adam_step_clock_frames": (c_int, [_P, _P, _P, _P, c_size_t, c_int, c_int, c_int, c_int, _P, c_int,
+                                          c_double, c_double, c_double, _P]),
 }
 
 
@@ -107,7 +110,7 @@ class OverfitStepArgs(ctypes.Structure):
                 ("phase", c_int), ("splat_plan", _P), ("splat_overflow_max", ctypes.c_uint),
                 ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P),
                 ("gt_positions", _P), ("gt_fx", c_float), ("gt_fy", c_float), ("metrics_log", _P),
-                ("metrics_capacity", c_int)]
+                ("metrics_capacity", c_int), ("B", c_int), ("gt_fxfy", _P)]
 
 
 SIGNATURES["fm_overfit_step"] = (c_int, [ctypes.POINTER(OverfitStepArgs), _P])

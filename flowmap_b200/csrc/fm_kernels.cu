@@ -70,6 +70,7 @@ struct Workspace {
   PairAdjoint* adj;  // [BP]
   float* zshift;     // [BP] conditioning shift of the moment pass (k_pair_shift)
   float* pshift;     // [BP][3] conditioning shift of explicit point sets (k_points_shift)
+  double* track_sums;  // [B][2] per-video tracking loss sum / valid count (fused step, B > 1)
   size_t bytes;
 };
 
@@ -88,6 +89,7 @@ Workspace carve(void* base, int B, int F) {
   w.adj = (PairAdjoint*)(p + off); off = align_up(off + BP * sizeof(PairAdjoint), 256);
   w.zshift = (float*)(p + off); off = align_up(off + BP * sizeof(float), 256);
   w.pshift = (float*)(p + off); off = align_up(off + BP * 3 * sizeof(float), 256);
+  w.track_sums = (double*)(p + off); off = align_up(off + (size_t)B * 2 * sizeof(double), 256);
   w.bytes = off;
   return w;
 }
@@ -712,6 +714,59 @@ k_flow_lean(const float* __restrict__ depth, const float* __restrict__ k4, const
   }
 }
 
+// k_flow_lean for B independent videos (fm_overfit_step_args.B > 1): mask_sum holds one normaliser per
+// video and frame f of video b is scaled by its own (LossFlow instead normalises a batch by one sum).
+// A separate kernel, so that k_flow_lean keeps its code.
+template <int VEC, bool FOCAL, int MINB>
+__global__ void __launch_bounds__(kThreads, MINB)
+k_flow_lean_videos(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
+                   const float* __restrict__ fflow, const float* __restrict__ bflow,
+                   const float* __restrict__ fmask, const float* __restrict__ bmask,
+                   const double* __restrict__ mask_sum, int mapping, float delta, float loss_weight,
+                   float* __restrict__ g_depth, double* __restrict__ leanacc, int F, int H, int W, int BF) {
+  __shared__ double smem[kFlowLeanVals * (kThreads / 32)];
+  const int N = H * W;
+  constexpr int kChunk = kThreads * VEC;
+  const int chunks = (N + kChunk - 1) / kChunk;
+  const ItemRange range = block_item_range((long long)BF * chunks);
+  const RobustCfg rc = make_robust(mapping, delta, H, W);
+  const GridDims grid = make_grid(H, W);
+#pragma unroll 1
+  for (int it = range.i0; it < range.i1;) {
+    const int frame = it / chunks, cb = it - frame * chunks;
+    const int ce = (cb + (range.i1 - it) < chunks) ? cb + (range.i1 - it) : chunks;
+    const int bi = frame / F, i = frame - bi * F;
+    double den = mask_sum[bi];
+    if (den == 0.0) den = 1.0;  // loss_flow.py:70 "valid_sum or 1", per video
+    const float g = (float)((double)loss_weight / den);
+    const bool hasF = i < F - 1, hasB = i > 0;
+    FlowFrameLean f;
+    f.kk = make_cam(load_k4(k4, frame));
+    f.kn = make_cam(load_k4(k4, hasF ? frame + 1 : frame));
+    f.kp = make_cam(load_k4(k4, hasB ? frame - 1 : frame));
+    const int pairF = bi * (F - 1) + i, pairB = pairF - 1;
+    Rt tf, tb;
+    if (hasF) tf = load_rt(rt, pairF);
+    if (hasB) tb = load_rt(rt, pairB);
+    fill_lean(f, hasF ? &tf : nullptr, hasB ? &tb : nullptr);
+    const float* D = depth + (size_t)frame * N;
+    const float* ff = fflow + (size_t)(hasF ? pairF : 0) * N * 2;
+    const float* mf = fmask + (size_t)(hasF ? pairF : 0) * N;
+    const float* fb = bflow + (size_t)(hasB ? pairB : 0) * N * 2;
+    const float* mb = bmask + (size_t)(hasB ? pairB : 0) * N;
+    float* gd = g_depth + (size_t)frame * N;
+    float acc[kFlowLeanVals];
+#pragma unroll
+    for (int k = 0; k < kFlowLeanVals; ++k) acc[k] = 0.f;
+    if (hasF && hasB) flow_frame_body_lean<VEC, true, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    else if (hasF) flow_frame_body_lean<VEC, true, false, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    else flow_frame_body_lean<VEC, false, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    // lean slots live in the upper half of the frame's accumulator row until k_flow_lean_convert
+    block_accumulate<kFlowLeanVals>(acc, leanacc + (size_t)frame * kFlowAcc, smem);
+    it += ce - cb;
+  }
+}
+
 // Rewrites each frame's lean accumulators (slots 0-13) into the standard layout in place.
 __global__ void k_flow_lean_convert(double* __restrict__ flowacc, const float* __restrict__ rt,
                                     const float* __restrict__ k4, int focal_mode, int B, int F, int H, int W) {
@@ -782,6 +837,23 @@ __global__ void k_flow_finalize(const double* __restrict__ flowacc, const float*
       for (int w = 0; w < (int)((blockDim.x + 31) >> 5); ++w) tot += part[w];
       *loss = (float)tot;
     }
+  }
+}
+
+// The batched fused step's flow losses: block b sums the F per-frame loss terms of video b into loss[b],
+// in the order in which k_flow_finalize's block 0 sums them for one video (launched with 128 threads).
+__global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __restrict__ loss, int F) {
+  __shared__ double part[32];
+  const double* acc = flowacc + (size_t)blockIdx.x * F * kFlowAcc;
+  double s = 0.0;
+  for (int k = threadIdx.x; k < F; k += blockDim.x) s += acc[(size_t)k * kFlowAcc];
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tot = 0.0;
+    for (int w = 0; w < (int)((blockDim.x + 31) >> 5); ++w) tot += part[w];
+    loss[blockIdx.x] = (float)tot;
   }
 }
 
@@ -1482,6 +1554,24 @@ k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m
     FM_ADAM1(pp, gg, mm, vv)
     p[i] = pp; m[i] = mm; v[i] = vv;
   }
+}
+
+// k_adam on the frames lo <= f < hi of each video of F frames (frame_elems values per frame): the part of
+// a batched (B, F, ...) parameter whose gradient is final, without slice views.  blockIdx.y = one
+// (video, frame) row, so the index arithmetic stays out of the element loop.
+__global__ void __launch_bounds__(kThreads)
+k_adam_frames(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+              size_t frame_elems, int F, int lo, int hi, float beta1, float beta2, float omb1, float omb2,
+              float eps, const float* __restrict__ consts) {
+  const float step_size = __ldg(consts), bc2_sqrt = __ldg(consts + 1);
+  const int span = hi - lo, b = blockIdx.y / span, f = lo + (blockIdx.y - b * span);
+  const size_t o = ((size_t)b * F + f) * frame_elems;
+  p += o; g += o; m += o; v += o;
+  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < frame_elems; i += (size_t)gridDim.x * kThreads) {
+    float pp = p[i], gg = g[i], mm = m[i], vv = v[i];
+    FM_ADAM1(pp, gg, mm, vv)
+    p[i] = pp; m[i] = mm; v[i] = vv;
+  }
 #undef FM_ADAM1
 }
 
@@ -1669,22 +1759,22 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
   return ((size_t)max_rows * (kTrackRec + (kTrackThreads / 32) * kTrackAcc) + (size_t)list_cap) * sizeof(float);
 }
 
-template <bool SHARED_K>
-__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS)
-k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,
-            const int* __restrict__ seg, const float* __restrict__ txy,
-            const unsigned char* __restrict__ tvis, int mapping, float delta, double* __restrict__ sums,
-            unsigned char* __restrict__ flag, float* __restrict__ dq_out,
-            double* __restrict__ trackacc, int* __restrict__ next_item, int num_items, int max_rows,
-            int list_cap, int H, int W, TrackShard sh) {
-  extern __shared__ float4 sm4[];
+// VIDEOS (the batched fused step): the segments of video b have start frames in [b F, (b + 1) F), F =
+// video_frames, and its loss sum / valid count go to sums[2 b], sums[2 b + 1].
+template <bool SHARED_K, bool VIDEOS>
+__device__ __forceinline__ void track_src_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                               const float* __restrict__ ext, const int* __restrict__ seg,
+                                               const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
+                                               int mapping, float delta, double* __restrict__ sums,
+                                               unsigned char* __restrict__ flag, float* __restrict__ dq_out,
+                                               double* __restrict__ trackacc, int* __restrict__ next_item,
+                                               int num_items, int max_rows, int list_cap, int H, int W,
+                                               TrackShard sh, int video_frames, float4* sm4, double* red,
+                                               int* s_wbase, int* s_item) {
   float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
   constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
   constexpr int SLOT0 = kTrackAcc - NRED;  // twist values live in slots 4..9 either way
-  __shared__ double red[kTrackAcc * NW];
-  __shared__ int s_wbase[NW];
-  __shared__ int s_item[2];
   float* s_tgt = sm + (size_t)max_rows * kTrackRec;  // [warp][target row][kTrackAcc]
   int* s_list = reinterpret_cast<int*>(s_tgt + (size_t)NW * max_rows * kTrackAcc);
   const GridDims grid = make_grid(H, W);
@@ -1878,7 +1968,7 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
       }
       __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
-    block_accumulate<2, kTrackThreads>(lc, sums, red);
+    block_accumulate<2, kTrackThreads>(lc, VIDEOS ? sums + 2 * (si.start_frame / video_frames) : sums, red);
     block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
     // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
     // with a barrier, so every slice is complete)
@@ -1892,6 +1982,34 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
   }
 }
 
+#define FM_TRACK_SRC_PARAMS                                                                                  \
+  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,            \
+      const int* __restrict__ seg, const float* __restrict__ txy, const unsigned char* __restrict__ tvis, \
+      int mapping, float delta, double* __restrict__ sums, unsigned char* __restrict__ flag,              \
+      float* __restrict__ dq_out, double* __restrict__ trackacc, int* __restrict__ next_item, int num_items, \
+      int max_rows, int list_cap, int H, int W, TrackShard sh
+#define FM_TRACK_SRC_ARGS \
+  depth, k4, ext, seg, txy, tvis, mapping, delta, sums, flag, dq_out, trackacc, next_item, num_items, max_rows, list_cap, H, W, sh
+// shared memory is declared by the kernels (a device function's would move the dynamic part)
+#define FM_TRACK_SRC_SHARED                 \
+  extern __shared__ float4 sm4[];          \
+  __shared__ double red[kTrackAcc * (kTrackThreads / 32)]; \
+  __shared__ int s_wbase[kTrackThreads / 32]; \
+  __shared__ int s_item[2];
+template <bool SHARED_K>
+__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src(FM_TRACK_SRC_PARAMS) {
+  FM_TRACK_SRC_SHARED
+  track_src_body<SHARED_K, false>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item);
+}
+template <bool SHARED_K>
+__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_videos(FM_TRACK_SRC_PARAMS, int video_frames) {
+  FM_TRACK_SRC_SHARED
+  track_src_body<SHARED_K, true>(FM_TRACK_SRC_ARGS, video_frames, sm4, red, s_wbase, s_item);
+}
+#undef FM_TRACK_SRC_SHARED
+#undef FM_TRACK_SRC_PARAMS
+#undef FM_TRACK_SRC_ARGS
+
 __device__ __forceinline__ double track_scale(const double* sums, float loss_weight, const float* go) {
   double cnt = sums[1];
   if (cnt == 0.0) cnt = 1.0;  // loss_tracking.py:61 "valid_sum or 1"
@@ -1902,19 +2020,28 @@ __global__ void k_track_loss(const double* __restrict__ sums, float loss_weight,
   *loss = (float)(track_scale(sums, loss_weight, nullptr) * sums[0]);
 }
 
-// scale * (stored camera-space adjoint) -> the four depth taps of every source sample.
-__global__ void __launch_bounds__(kThreads)
-k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
-              const unsigned char* __restrict__ flag, const float* __restrict__ dq,
-              const double* __restrict__ sums, float loss_weight, const float* __restrict__ go,
-              float* __restrict__ g_depth, int H, int W, TrackShard sh) {
+// The batched fused step's tracking losses: thread b reads video b's loss sum / valid count.
+__global__ void k_track_video_loss(const double* __restrict__ sums, float loss_weight, float* __restrict__ loss, int B) {
+  const int b = threadIdx.x;
+  if (b < B) loss[b] = (float)(track_scale(sums + 2 * b, loss_weight, nullptr) * sums[2 * b]);
+}
+
+// scale * (stored camera-space adjoint) -> the four depth taps of every source sample.  VIDEOS: the scale
+// of the segment's video (start frame / video_frames), see track_src_body.
+template <bool VIDEOS>
+__device__ __forceinline__ void track_apply_body(const float* __restrict__ k4, const int* __restrict__ seg,
+                                                 const float* __restrict__ txy, const unsigned char* __restrict__ flag,
+                                                 const float* __restrict__ dq, const double* __restrict__ sums,
+                                                 float loss_weight, const float* __restrict__ go,
+                                                 float* __restrict__ g_depth, int H, int W, TrackShard sh,
+                                                 int video_frames) {
   const SegInfo si = load_seg(seg, blockIdx.z);
   const int row = blockIdx.y;
   const int p = blockIdx.x * kThreads + threadIdx.x;
   if (row >= si.rows || p >= si.n || !sh.owns(si.start_frame + row)) return;
   const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p;
   if (!flag[sidx]) return;
-  const float scale = (float)track_scale(sums, loss_weight, go);
+  const float scale = (float)track_scale(VIDEOS ? sums + 2 * (si.start_frame / video_frames) : sums, loss_weight, go);
   const int frame = si.start_frame + row;
   const GridDims grid = make_grid(H, W);
   const Cam ks = make_cam(load_k4(k4, frame));
@@ -1930,13 +2057,31 @@ k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const f
   red_add(gd + t.y1 * W + t.x1, t.w11 * (dq0 * rx1 + dq1 * ry1 + dq2));
 }
 
-__global__ void k_track_finalize(const double* __restrict__ trackacc, const double* __restrict__ sums,
-                                 float loss_weight, const float* __restrict__ go,
-                                 const float* __restrict__ ext, float* __restrict__ g_ext,
-                                 float* __restrict__ g_k4, int F) {
+__global__ void __launch_bounds__(kThreads)
+k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
+              const unsigned char* __restrict__ flag, const float* __restrict__ dq,
+              const double* __restrict__ sums, float loss_weight, const float* __restrict__ go,
+              float* __restrict__ g_depth, int H, int W, TrackShard sh) {
+  track_apply_body<false>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh, 0);
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_track_apply_videos(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
+                     const unsigned char* __restrict__ flag, const float* __restrict__ dq,
+                     const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
+                     TrackShard sh, int video_frames) {
+  track_apply_body<true>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, video_frames);
+}
+
+// VIDEOS: frames f of B * video_frames, scaled by the sums of video f / video_frames.
+template <bool VIDEOS>
+__device__ __forceinline__ void track_finalize_body(const double* __restrict__ trackacc, const double* __restrict__ sums,
+                                                    float loss_weight, const float* __restrict__ go,
+                                                    const float* __restrict__ ext, float* __restrict__ g_ext,
+                                                    float* __restrict__ g_k4, int F, int video_frames) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
-  const double sc = track_scale(sums, loss_weight, go);
+  const double sc = track_scale(VIDEOS ? sums + 2 * (f / video_frames) : sums, loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
   for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
   const float* P = ext + (size_t)f * 16;
@@ -1950,6 +2095,19 @@ __global__ void k_track_finalize(const double* __restrict__ trackacc, const doub
   }
   o[3] = (float)(sc * a[7]); o[7] = (float)(sc * a[8]); o[11] = (float)(sc * a[9]);
   o[12] = o[13] = o[14] = o[15] = 0.f;
+}
+
+__global__ void k_track_finalize(const double* __restrict__ trackacc, const double* __restrict__ sums,
+                                 float loss_weight, const float* __restrict__ go,
+                                 const float* __restrict__ ext, float* __restrict__ g_ext,
+                                 float* __restrict__ g_k4, int F) {
+  track_finalize_body<false>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F, 0);
+}
+
+__global__ void k_track_finalize_videos(const double* __restrict__ trackacc, const double* __restrict__ sums,
+                                        float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
+                                        float* __restrict__ g_k4, int BF, int video_frames) {
+  track_finalize_body<true>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, BF, video_frames);
 }
 
 // ================================================================== focal-length sweep
@@ -2411,6 +2569,41 @@ k_trajectory_ate(const float* __restrict__ gt, const float* __restrict__ pred, i
   }
 }
 
+// The batched fused step's metrics rows: block b writes video b of row (step - 1) % capacity of the
+// (capacity, B, 5) ring, with what k_trajectory_ate writes for one video (the same float64 sums in the
+// same order).  gt (B, F, 3); a video whose first position is NaN has no ground truth (ATE NaN);
+// gt_fxfy (B, 2) frame means of the ground-truth intrinsics (NaN: no ground truth).
+__global__ void __launch_bounds__(kAteThreads)
+k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, int F, MetricsRow row,
+                 const float* __restrict__ gt_fxfy) {
+  __shared__ double s_red[kAteThreads / 32 * 9];
+  const size_t b = blockIdx.x;
+  float* r = row.log + ((size_t)((row.clock->step - 1u) % (unsigned)row.capacity) * gridDim.x + b) * 5;
+  const bool has_gt = gt && !isnan(gt[b * F * 3]);
+  if (threadIdx.x == 0) {
+    const float* k4 = row.k4 + b * F * 4;
+    double fx = 0.0, fy = 0.0;
+    for (int f = 0; f < F; ++f) { fx += (double)k4[f * 4 + 0]; fy += (double)k4[f * 4 + 1]; }
+    r[0] = row.loss[b];
+    r[1] = row.track_loss ? row.track_loss[b] : 0.f;
+    r[2] = (float)fabs((double)gt_fxfy[2 * b] - fx / F);
+    r[3] = (float)fabs((double)gt_fxfy[2 * b + 1] - fy / F);
+    if (!has_gt) r[4] = NAN;
+  }
+  if (!has_gt) return;
+  AtePoints x;
+  x.gt = gt + b * F * 3;
+  x.pred = pred + b * F * 16;
+  x.gt_stride = 3;
+  x.pred_stride = 16;
+  x.pred_cstride = 4;
+  x.F = F;
+  BlockSum red{s_red};
+  double v;
+  trajectory_ate(x, threadIdx.x, kAteThreads, red, v, nullptr, nullptr);
+  if (threadIdx.x == 0) r[4] = (float)v;
+}
+
 // ================================================================== fused overfit step helpers
 // focal_lengths_to_intrinsics (intrinsics/common.py:6-20) for a shared focal length, as k4 rows.
 __global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restrict__ k4, int BF, int H, int W) {
@@ -2423,10 +2616,22 @@ __global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restri
   k4[t * 4 + 3] = 0.5f;
 }
 
+// k_k4_from_focal for B videos with one focal length each: frame t of the (B*F, 4) rows reads focal[t / F].
+__global__ void k_k4_from_focals(const float* __restrict__ focal, float* __restrict__ k4, int BF, int F, int H,
+                                 int W) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= BF) return;
+  const float scaled = focal[t / F] * sqrtf((float)H * (float)W);
+  k4[t * 4 + 0] = scaled / (float)W;
+  k4[t * 4 + 1] = scaled / (float)H;
+  k4[t * 4 + 2] = 0.5f;
+  k4[t * 4 + 3] = 0.5f;
+}
+
 // d loss / d focal from the per-frame k4 gradients (flow-loss part + Procrustes part).
-__global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                             const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int B,
-                             int F, int H, int W, const float* __restrict__ flow_scale = nullptr) {
+__device__ __forceinline__ void focal_grad_block(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                                                 const float* __restrict__ extra_g_k4, float* __restrict__ g_focal,
+                                                 int B, int F, int H, int W, const float* __restrict__ flow_scale) {
   double sx = 0.0, sy = 0.0;
   const double fs = flow_scale ? (double)*flow_scale : 1.0;  // d total / d flow loss (the Procrustes part in k4acc carries it already)
   for (int t = threadIdx.x; t < B * F; t += blockDim.x) {
@@ -2445,6 +2650,22 @@ __global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __r
     const double sc = sqrt((double)H * (double)W);
     *g_focal = (float)(ax * sc / W + ay * sc / H);
   }
+}
+
+__global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                             const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int B,
+                             int F, int H, int W, const float* __restrict__ flow_scale = nullptr) {
+  focal_grad_block(k4acc, flowacc, extra_g_k4, g_focal, B, F, H, W, flow_scale);
+}
+
+// One focal length per video (the batched fused step): block b writes g_focal[b] from video b's frames,
+// summed in the order k_focal_grad uses for one video.
+__global__ void k_focal_grad_videos(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                                    const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int F, int H,
+                                    int W) {
+  const size_t f0 = (size_t)blockIdx.x * F;
+  focal_grad_block(k4acc + f0 * 4, flowacc + f0 * kFlowAcc, extra_g_k4 ? extra_g_k4 + f0 * 4 : nullptr,
+                   g_focal + blockIdx.x, 1, F, H, W, nullptr);
 }
 
 // ---------------------------------------------------------------- launch geometry
@@ -2521,7 +2742,8 @@ namespace {
 int launch_flow(const float* depth, const float* k4, const float* rt, const float* ff, const float* fb,
                 const float* mf, const float* mb, const double* mask_sum, int mapping, float delta,
                 float loss_weight, int intrinsics_mode, float* g_depth, double* flowacc, int B, int F,
-                int H, int W, cudaStream_t s) {
+                int H, int W, cudaStream_t s, bool per_video = false) {
+  if (per_video && intrinsics_mode == 0) return fail_msg("launch_flow: per-video normalisers need shared intrinsics");
   const int BF = B * F;
   const int vec = (W % 4 == 0) ? 4 : 1;
   dim3 grid(blocks_for(H * W, vec), BF);
@@ -2533,7 +2755,15 @@ int launch_flow(const float* depth, const float* k4, const float* rt, const floa
   }
   const bool focal = intrinsics_mode == 1;
   const int pg = persistent_grid(2, (long long)BF * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
-  if (vec == 4) {
+  if (per_video) {  // mask_sum holds B normalisers
+    if (vec == 4) {
+      if (focal) k_flow_lean_videos<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+      else k_flow_lean_videos<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+    } else {
+      if (focal) k_flow_lean_videos<1, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+      else k_flow_lean_videos<1, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+    }
+  } else if (vec == 4) {
     if (focal) k_flow_lean<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
     else k_flow_lean<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
   } else {
@@ -2656,7 +2886,7 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 102; }
+int fm_version(void) { return 103; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -2770,7 +3000,13 @@ int fm_procrustes_fwd(const float* depth, const float* k4, const float* backward
 int fm_procrustes_moments(const float* depth, const float* k4, const float* backward_flow,
                           const float* weights, float weight_sensitivity, void* ws, int F, int H, int W,
                           void* stream) {
-  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, 1, F,
+  return fm_procrustes_moments_batched(depth, k4, backward_flow, weights, weight_sensitivity, ws, 1, F, H, W, stream);
+}
+
+int fm_procrustes_moments_batched(const float* depth, const float* k4, const float* backward_flow,
+                                  const float* weights, float weight_sensitivity, void* ws, int B, int F, int H,
+                                  int W, void* stream) {
+  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, B, F,
                              H, W, stream, nullptr, nullptr, nullptr, /*solve=*/false);
 }
 
@@ -3007,6 +3243,25 @@ int fm_adam_step_clock(float* param, const float* grad, float* exp_avg, float* e
   return 0;
 }
 
+int fm_adam_step_clock_frames(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t frame_elems,
+                              int B, int F, int frame_lo, int frame_hi, const void* clock, int focal_clock,
+                              double beta1_d, double beta2_d, double eps_d, void* stream) {
+  if (!param || !grad || !exp_avg || !exp_avg_sq || !clock || B < 1 || F < 1 || frame_lo < 0 || frame_hi > F)
+    return fail_msg("fm_adam_step_clock_frames: bad arguments");
+  if (frame_hi <= frame_lo || frame_elems == 0) return 0;
+  const int rows = B * (frame_hi - frame_lo);
+  if (rows > 65535) return fail_msg("fm_adam_step_clock_frames: too many frames");
+  size_t nx = (frame_elems + kThreads * 4 - 1) / (kThreads * 4);
+  if (nx < 1) nx = 1;
+  if (nx > 1024) nx = 1024;
+  const StepClock* c = (const StepClock*)clock;
+  k_adam_frames<<<dim3((unsigned)nx, (unsigned)rows), kThreads, 0, (cudaStream_t)stream>>>(
+      param, grad, exp_avg, exp_avg_sq, frame_elems, F, frame_lo, frame_hi, (float)beta1_d, (float)beta2_d,
+      (float)(1.0 - beta1_d), (float)(1.0 - beta2_d), (float)eps_d, focal_clock ? &c->focal_step_size : &c->step_size);
+  FM_CHECK_LAUNCH("fm_adam_step_clock_frames");
+  return 0;
+}
+
 int fm_random_subset_clock(const void* clock, long long N, int n, int64_t* out, void* stream) {
   if (!clock || N < 1 || n < 1 || n > N || !out) return fail_msg("fm_random_subset_clock: bad arguments");
   k_random_subset<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(0ull, N, n, out, &((const StepClock*)clock)->seed);
@@ -3060,11 +3315,15 @@ size_t fm_track_reduce_bytes(int F) {
   return align_up(4 * sizeof(double), 256) + align_up((size_t)F * kTrackAcc * sizeof(double), 256);
 }
 
-int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* extrinsics, const int* segments,
-                              int num_segments, int max_rows, int max_points, const float* track_xy,
-                              const unsigned char* track_vis, long long total_samples, int mapping, float delta,
-                              float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
-                              int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream) {
+// vsums != NULL (the batched fused step): the frames are B videos of F / B frames, and each video's loss
+// sum and valid count go to vsums[2 b], vsums[2 b + 1] (zeroed here) instead of the head of ws; `loss`
+// then receives B values.
+static int track_fwd_impl(const float* depth, const float* k4, const float* extrinsics, const int* segments,
+                          int num_segments, int max_rows, int max_points, const float* track_xy,
+                          const unsigned char* track_vis, long long total_samples, int mapping, float delta,
+                          float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
+                          int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream,
+                          double* vsums = nullptr, int B = 1) {
   if (!depth || !k4 || !extrinsics || !segments || !track_xy || !track_vis || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_fwd: bad arguments");
@@ -3076,6 +3335,8 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
   // sums, work counter, accumulators
   cudaError_t e = cudaMemsetAsync(w.sums, 0, (char*)w.dq - (char*)w.sums, s);
   if (e != cudaSuccess) return fail("fm_track_loss_fwd: memset", e);
+  if (vsums && (e = cudaMemsetAsync(vsums, 0, (size_t)B * 2 * sizeof(double), s)) != cudaSuccess)
+    return fail("fm_track_loss_fwd: memset", e);
   const int list_cap = max_points < kTrackListCap ? max_points : kTrackListCap;
   const size_t smem = track_smem_bytes(max_rows, list_cap);
   if (smem > 200 * 1024) return fail_msg("fm_track_loss_fwd: segment too long for shared memory");
@@ -3093,6 +3354,19 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
     if (ea != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ea);
   }
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
+  if (vsums) {  // one focal length per video: shared intrinsics
+    static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_videos<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
+    k_track_src_videos<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
+                                                               mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
+                                                               (int)items, max_rows, list_cap, H, W, sh, F / B);
+    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_videos");
+    if (loss) {
+      k_track_video_loss<<<1, 32 * ((B + 31) / 32), 0, s>>>(vsums, loss_weight, loss, B);
+      FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_video_loss");
+    }
+    return 0;
+  }
   if (shared_intrinsics)
     k_track_src<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping,
                                                         delta, w.sums, w.flag, w.dq, w.acc, w.next_item, (int)items,
@@ -3107,6 +3381,16 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
     FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_loss");
   }
   return 0;
+}
+
+int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* extrinsics, const int* segments,
+                              int num_segments, int max_rows, int max_points, const float* track_xy,
+                              const unsigned char* track_vis, long long total_samples, int mapping, float delta,
+                              float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
+                              int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream) {
+  return track_fwd_impl(depth, k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, track_vis,
+                        total_samples, mapping, delta, loss_weight, loss, ws, F, H, W, depth_frame0, src_frame_lo,
+                        src_frame_hi, shared_intrinsics, stream);
 }
 
 int fm_track_loss_fwd(const float* depth, const float* k4, const float* extrinsics, const int* segments,
@@ -3132,7 +3416,8 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
                           int max_rows, int max_points, const float* track_xy, long long total_samples,
                           float loss_weight, const float* grad_out, float* g_depth, float* g_extrinsics,
                           float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
-                          int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream) {
+                          int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream,
+                          const double* vsums = nullptr, int B = 1) {
   if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !g_k4 || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_bwd: bad arguments");
@@ -3141,6 +3426,15 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
   TrackWs w = carve_track(ws, F, total_samples);
   dim3 grid((max_points + kThreads - 1) / kThreads, max_rows, num_segments);
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
+  if (vsums) {  // per-video scales (track_fwd_impl); grad_out is 1 in the batched step
+    k_track_apply_videos<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
+                                                             g_depth, H, W, sh, F / B);
+    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply_videos");
+    k_track_finalize_videos<<<(F + 63) / 64, 64, 0, s>>>(w.acc, vsums, loss_weight, extrinsics, g_extrinsics, g_k4,
+                                                         F, F / B);
+    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize_videos");
+    return 0;
+  }
   k_track_apply<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, w.sums, loss_weight,
                                                     grad_out, g_depth, H, W, sh);
   FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply");
@@ -3387,8 +3681,15 @@ static SideLane* side_lane(int which = 0) {
 
 int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   if (!a || !a->depth || !a->fflow || !a->bflow || !a->fmask || !a->bmask || !a->mask_sum ||
-      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 || bad_dims(1, a->F, a->H, a->W))
+      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 || bad_dims(a->B > 1 ? a->B : 1, a->F, a->H, a->W))
     return fail_msg("fm_overfit_step: bad arguments");
+  // B independent videos of one shape: every per-video scalar is an array of B values
+  const int B = a->B > 1 ? a->B : 1;
+  if (B > 1 && (a->phase != FM_STEP_ALL || a->splat_plan))
+    return fail_msg("fm_overfit_step: B > 1 serves whole steps without a splat plan");
+  if (B > 1 && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
+    return fail_msg("fm_overfit_step: B > 1 does not fuse the logit update of a deferred step (pass step = 0)");
+  if (B > 1 && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step: B > 1 metrics need gt_fxfy");
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
@@ -3397,7 +3698,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   const int F = a->F, H = a->H, W = a->W, BP = F - 1;
   const size_t N = (size_t)H * W;
-  Workspace w = carve(a->ws, 1, F);
+  Workspace w = carve(a->ws, B, F);
   int rc;
   cudaError_t e;
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
@@ -3406,13 +3707,16 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
-    if (a->focal) {
+    if (a->focal && B == 1) {
       k_k4_from_focal<<<(F + 63) / 64, 64, 0, s>>>(a->focal, k4, F, H, W);
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
+    } else if (a->focal) {
+      k_k4_from_focals<<<(B * F + 63) / 64, 64, 0, s>>>(a->focal, k4, B * F, F, H, W);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
     if ((rc = procrustes_fwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                  a->indices, a->num_indices, a->rt, a->ws, 1, F, H, W, stream, nullptr, plan,
+                                  a->indices, a->num_indices, a->rt, a->ws, B, F, H, W, stream, nullptr, plan,
                                   (a->indices || plan) ? nullptr : a->moments_k4)))
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
@@ -3424,24 +3728,31 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       if ((e = cudaStreamWaitEvent(fwd_lane->stream, fwd_lane->fork, 0)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
     }
     // LossFlow forward + direct gradients (loss_flow.py:31-70)
-    e = cudaMemsetAsync(w.flowacc, 0, (size_t)F * kFlowAcc * sizeof(double), s);
+    e = cudaMemsetAsync(w.flowacc, 0, (size_t)B * F * kFlowAcc * sizeof(double), s);
     if (e != cudaSuccess) return fail("fm_overfit_step: memset", e);
     if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum,
-                          a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, 1, F,
-                          H, W, s)))
+                          a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, B, F,
+                          H, W, s, /*per_video=*/B > 1)))
       return rc;
-    k_flow_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.flowacc, a->rt, a->loss, nullptr, nullptr, 1, F);
-    FM_CHECK_LAUNCH("fm_overfit_step: k_flow_finalize");
+    if (B == 1) {
+      k_flow_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.flowacc, a->rt, a->loss, nullptr, nullptr, 1, F);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_finalize");
+    } else {
+      k_flow_video_loss<<<B, 128, 0, s>>>(w.flowacc, a->loss, F);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss");
+    }
     // LossTracking (loss_tracking.py:28-61) on the chained poses: the forward sweep belongs to the
     // forward half of a split step, its scaling / scatter to the backward half
     if (a->tracks) {
       const fm_packed_tracks* t = a->tracks;
       void* ts = fwd_lane ? (void*)fwd_lane->stream : stream;
-      if ((rc = fm_pose_chain(a->rt, a->extrinsics, 1, F, ts))) return rc;
-      // one focal length (or constant intrinsics) for all frames: only the summed K gradient is used
-      if ((rc = fm_track_loss_fwd_sharded(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
-                                          t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
-                                          a->track_weight, a->track_loss, a->track_ws, F, H, W, 0, 0, F, 1, ts)))
+      if ((rc = fm_pose_chain(a->rt, a->extrinsics, B, F, ts))) return rc;
+      // one focal length (or constant intrinsics) for all frames: only the summed K gradient is used.
+      // B > 1: the segments of video b start at frames b F + s, and its sums go to w.track_sums[b]
+      if ((rc = track_fwd_impl(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
+                               t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
+                               a->track_weight, a->track_loss, a->track_ws, B * F, H, W, 0, 0, B * F, 1, ts,
+                               B > 1 ? w.track_sums : nullptr, B)))
         return rc;
       if (fwd_lane) {
         if ((e = cudaEventRecord(fwd_lane->join, fwd_lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -3462,7 +3773,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       ms = mlane->stream;
     }
     // the camera centres: the tracking loss chained the poses already, a flow-only step chains them here
-    if (!a->tracks && (rc = fm_pose_chain(a->rt, a->extrinsics, 1, F, ms))) return rc;
+    if (!a->tracks && (rc = fm_pose_chain(a->rt, a->extrinsics, B, F, ms))) return rc;
     MetricsRow row;
     row.log = a->metrics_log;
     row.capacity = a->metrics_capacity;
@@ -3472,9 +3783,14 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     row.k4 = k4;
     row.gt_fx = a->gt_fx;
     row.gt_fy = a->gt_fy;
-    k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr, nullptr,
-                                                nullptr, row);
-    FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
+    if (B == 1) {
+      k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr,
+                                                  nullptr, nullptr, row);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
+    } else {
+      k_metrics_videos<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, F, row, a->gt_fxfy);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_videos");
+    }
     if (mlane && (e = cudaEventRecord(mlane->join, mlane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   }
   if (a->phase == FM_STEP_FORWARD) return 0;
@@ -3483,7 +3799,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   const float* tscale = a->phase == FM_STEP_BACKWARD ? a->track_grad_scale : nullptr;
   if (fscale) {  // the direct flow-loss gradient in g_depth was computed for scale 1; scale it before
     // the tracking loss adds its own (differently scaled) part
-    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, (size_t)F * N);
+    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, (size_t)B * F * N);
     FM_CHECK_LAUNCH("fm_overfit_step: k_scale_inplace");
   }
   const float* g_rt = a->phase == FM_STEP_BACKWARD ? a->g_rt : nullptr;           // the caller's
@@ -3502,22 +3818,25 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     }
     if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
                              t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
-                             a->track_ws, F, H, W, 0, 0, F, s, apply_stream)))
+                             a->track_ws, B * F, H, W, 0, 0, B * F, s, apply_stream, B > 1 ? w.track_sums : nullptr,
+                             B)))
       return rc;
     if (lane && (e = cudaEventRecord(lane->join, lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
-    if ((rc = fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, 1, F, stream))) return rc;
+    if ((rc = fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, F, stream))) return rc;
     g_rt = a->g_rt;
     track_g_k4 = a->track_g_k4;
   }
   // backward through Procrustes: adjoint constants, per-point distribution
   if (a->indices && a->g_weights) {  // subsampled Procrustes: sparse weight gradient, dense buffer
-    e = cudaMemsetAsync(a->g_weights, 0, (size_t)BP * N * sizeof(float), s);
+    e = cudaMemsetAsync(a->g_weights, 0, (size_t)B * BP * N * sizeof(float), s);
     if (e != cudaSuccess) return fail("fm_overfit_step: memset g_weights", e);
   }
   AdamFuse af;
   memset(&af, 0, sizeof(af));
   const bool defer = a->defer_adam != 0;  // softmin stage: the sweep's backward still adds gradients
-  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0;
+  // B > 1 with defer_adam = 1 would have to defer pair 0 of EVERY video (first_pair counts pairs of the
+  // whole batch): that step leaves the logits to the caller instead
+  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(B > 1 && a->defer_adam == 1);
   const StepClock* clock = (const StepClock*)a->clock;
   if (fuse_w) {  // the weight gradient is final inside k_distribute: update the logits there
     af.consts = clock ? &clock->step_size : nullptr;
@@ -3530,7 +3849,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   }
   if ((rc = procrustes_bwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
                                 a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
-                                a->g_k4, a->ws, 1, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
+                                a->g_k4, a->ws, B, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
                                 a->splat_overflow_max, /*depth_prescaled=*/fscale != nullptr)))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -3540,19 +3859,27 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       return clock ? fm_adam_step_clock(p, g, m, v, n, clock, focal_clock, a->beta1, a->beta2, a->eps, stream)
                    : fm_adam_step(p, g, m, v, n, a->lr, a->beta1, a->beta2, a->eps, step, stream);
     };
-    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, (size_t)F * N, a->step, 0))) return rc;
+    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, (size_t)B * F * N, a->step, 0))) return rc;
     if (a->weight_logits && !fuse_w &&
-        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, (size_t)BP * N, a->step, 0)))
+        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, (size_t)B * BP * N, a->step, 0)))
       return rc;
-    if (a->focal) {
+  }
+  if (a->focal) {  // d loss / d focal, then (update steps) its Adam
+    if (B == 1) {
       k_focal_grad<<<1, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, 1, F, H, W, fscale);
       FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
-      if ((rc = adam(a->focal, a->g_focal, a->m_focal, a->v_focal, 1, a->focal_step > 0 ? a->focal_step : a->step, 1)))
+    } else {  // whole steps only: no fscale
+      k_focal_grad_videos<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, F, H, W);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad_videos");
+    }
+    if (a->step > 0 && !defer) {
+      const int fstep = a->focal_step > 0 ? a->focal_step : a->step;
+      if ((rc = clock ? fm_adam_step_clock(a->focal, a->g_focal, a->m_focal, a->v_focal, B, clock, 1, a->beta1,
+                                           a->beta2, a->eps, stream)
+                      : fm_adam_step(a->focal, a->g_focal, a->m_focal, a->v_focal, B, a->lr, a->beta1, a->beta2,
+                                     a->eps, fstep, stream)))
         return rc;
     }
-  } else if (a->focal) {
-    k_focal_grad<<<1, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, 1, F, H, W, fscale);
-    FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
   }
   if (defer && a->step > 0 && a->weight_logits && !fuse_w) return fail_msg("fm_overfit_step: defer_adam needs the fused weight update");
   if (mlane && (e = cudaStreamWaitEvent(s, mlane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);

@@ -389,6 +389,19 @@ def adam_step_clock(param: Tensor, grad: Tensor, exp_avg: Tensor, exp_avg_sq: Te
               "fm_adam_step_clock")
 
 
+def adam_step_clock_frames(param: Tensor, grad: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, lo: int, hi: int,
+                           clock: StepClock, eps: float = 1e-8) -> None:
+    """adam_step_clock on the frames lo <= f < hi of every video of a (B, F, ...) parameter, in one launch."""
+    for t in (param, grad, exp_avg, exp_avg_sq):
+        if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous() or t.shape != param.shape:
+            raise ValueError("flowmap_b200: adam_step needs contiguous CUDA float32 tensors of one shape")
+    b, f = param.shape[:2]
+    with torch.cuda.device(param.device):
+        check(lib().fm_adam_step_clock_frames(_ptr(param), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq),
+                                              param[0, 0].numel(), b, f, lo, hi, clock.ptr, 0, clock.betas[0],
+                                              clock.betas[1], eps, _stream()), "fm_adam_step_clock_frames")
+
+
 def random_subset_clock(clock: StepClock, num_items: int, out: Tensor) -> Tensor:
     """random_subset seeded by the current tick of `clock`, into the caller's int64 buffer."""
     with torch.cuda.device(out.device):
@@ -398,19 +411,32 @@ def random_subset_clock(clock: StepClock, num_items: int, out: Tensor) -> Tensor
 
 
 class PackedTracks:
-    """All segments of a list[Tracks] in the flat layout fm_track_loss_* expects."""
+    """All segments of a list[Tracks] in the flat layout fm_track_loss_* expects.
 
-    def __init__(self, tracks, device):
+    Several videos (the batched fused step): `tracks` is a list of B such lists and `video_frames` the
+    frame count F of every video; segment s of video b is packed with start frame b * F + s.start_frame,
+    so the segments of one video address its rows of the (B * F) frame arrays and never cross videos."""
+
+    def __init__(self, tracks, device, video_frames: Optional[int] = None):
+        videos = [tracks] if video_frames is None else tracks
         segs, xy, vis, off = [], [], [], 0
-        for t in tracks:
-            b, f, n, _ = t.xy.shape
-            if b != 1:
-                raise ValueError("flowmap_b200: tracking supports batch size 1 "
-                                 "(flowmap/tracking/__init__.py:92-93)")
-            segs.append((off, f, n, int(t.start_frame)))
-            xy.append(t.xy[0].reshape(-1, 2))
-            vis.append(t.visibility[0].reshape(-1))
-            off += f * n
+        for b, video in enumerate(videos):
+            for t in video:
+                _, f, n, _ = t.xy.shape
+                if t.xy.shape[0] != 1:
+                    raise ValueError("flowmap_b200: tracking supports batch size 1 "
+                                     "(flowmap/tracking/__init__.py:92-93)")
+                start = int(t.start_frame)
+                if video_frames is not None:
+                    if start < 0 or start + f > video_frames:
+                        raise ValueError(f"flowmap_b200: a track segment of video {b} leaves its {video_frames} frames")
+                    start += b * video_frames
+                segs.append((off, f, n, start))
+                xy.append(t.xy[0].reshape(-1, 2))
+                vis.append(t.visibility[0].reshape(-1))
+                off += f * n
+        if not segs:
+            raise ValueError("flowmap_b200: no track segments")
         self.total = off
         self.num_segments = len(segs)
         self.max_rows = max(s[1] for s in segs)

@@ -143,64 +143,94 @@ class FusedOverfitter(Overfitter):
     bilinear scatter of the Procrustes adjoint is transposed once per Flows into a static plan and
     evaluated as a gather with TMA-staged windows -- no atomics, bit-reproducible gradients.  It is
     parity-green but has been slower per backward than the default global-RED kernel
-    (tools/ab_tiled.py compares the two), hence opt-in."""
+    (tools/ab_tiled.py compares the two), hence opt-in.
+
+    Several videos: `batch.videos` of shape (B, F, 3, H, W) with B > 1 (and Flows of shape
+    (B, F-1, ...)) runs B INDEPENDENT overfits in one step.  Video b gets what a one-video
+    FusedOverfitter on video b with the same cfg and step clock seed gets: its flow loss is normalised
+    by its own mask sum, and its gradients, Adam moments, focal length, softmin window and poses are its
+    own.  training_step() returns the (B,) per-video totals, whose sum is the objective.  This differs
+    on purpose from the reference's LossFlow at b > 1 (pretraining), which normalises a batch by ONE
+    pooled mask sum.  Shared by the batch: the Procrustes point subset and the softmin point sample of
+    each step.  The parameters live in (B, ...) buffers; `models[b]` is video b's Model, whose
+    parameters are views into them.  `tracks` is then a list of B segment lists (one per video; its
+    tracking loss is normalised by its own valid count), and the metrics log holds (steps, B) values.
+    B > 1 does not serve the splat plan."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):
-        super().__init__(cfg, batch, flows, tracks, device, model=model)
+        b, f, _, h, w = batch.videos.shape
+        if b > 1:
+            if model is not None:
+                raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
+            if use_splat_plan:
+                raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
+            if tracks is not None and len(tracks) != b:
+                raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({b})")
+            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+                if tuple(getattr(flows, name).shape[:2]) != (b, f - 1):
+                    raise ValueError(f"flowmap_b200: flows.{name} must hold (B, F-1) = ({b}, {f - 1}) pairs")
+        super().__init__(cfg, batch, flows, tracks if b == 1 else None, device, model=model)
         from ._lib import OverfitStepArgs, PackedTracksC, lib
         import ctypes
-        if batch.videos.shape[0] != 1:
-            raise ValueError("flowmap_b200: the fused step optimises one video (batch size 1), as "
-                             "flowmap/overfit.py does")
+        self.B = b
+        if b > 1 and tracks is not None:
+            self.tracks = [[t.to(device) for t in video] for video in tracks]
         # the kernels read raw pointers: canonical (contiguous float32) copies, kept alive here
         # (FlowPredictor.rescale_flow returns a permuted view, flow_predictor.py:40-49)
         self.flows = Flows(*(ops._canon(getattr(self.flows, n), n)
                              for n in ("forward", "backward", "forward_mask", "backward_mask")))
         dev = self.flows.forward.device
-        _, f, _, h, w = batch.videos.shape
         self._use_plan = use_splat_plan and cfg.procrustes_points is None and not cfg.procrustes_randomize
         self._plan = ops.SplatPlan(self.flows.backward) if self._use_plan else None
-        bb = self.model.backbone
-        self._depth, self._wlog = bb.depth.data, bb.weights.data
         self._softmin = cfg.intrinsics == "softmin"
+        self.models = [self.model]
+        if b > 1:  # sets _depth, _wlog and (where it is a parameter) _focal
+            self.models += [build_model_and_losses(cfg, f, (h, w))[0].to(device) for _ in range(b - 1)]
+            self._bind_batched_parameters()
+        else:
+            self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
         if self._softmin:
             intr = self.model.intrinsics
-            self._focal = (intr.intrinsics_regressed.focal_length.data if cfg.regression_after
-                           is not None else torch.zeros((), device=dev))
+            if b == 1:
+                self._focal = (intr.intrinsics_regressed.focal_length.data if cfg.regression_after
+                               is not None else torch.zeros((), device=dev))
+            elif cfg.regression_after is None:
+                self._focal = torch.zeros(b, device=dev)
             n = cfg.softmin_candidates
             self._cand_f = intr.focal_length_candidates.float().contiguous()
-            self._cand_k4 = ops.candidate_k4(self._cand_f, h, w, 1)
-            self._sw_err = torch.empty(1, n, device=dev)
-            self._sw_sm = torch.empty(1, n, device=dev)
-            self._sw_gerr = torch.empty(1, n, device=dev)
-            self._sw_rt = torch.empty(n, 3, 4, device=dev)
-            self._sw_focal = torch.zeros(1, device=dev)
-            self._sw_ws = torch.empty(lib().fm_softmin_workspace_bytes(1, n), dtype=torch.uint8,
+            self._cand_k4 = ops.candidate_k4(self._cand_f, h, w, b)
+            self._sw_err = torch.empty(b, n, device=dev)
+            self._sw_sm = torch.empty(b, n, device=dev)
+            self._sw_gerr = torch.empty(b, n, device=dev)
+            self._sw_rt = torch.empty(b * n, 3, 4, device=dev)
+            self._sw_focal = torch.zeros(b, device=dev)
+            self._sw_ws = torch.empty(lib().fm_softmin_workspace_bytes(b, n), dtype=torch.uint8,
                                       device=dev)
             # candidate 0's intrinsics for every frame: what the early moment pass of a sweep step uses
-            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(f, 4).contiguous()
+            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(b * f, 4).contiguous()
             self.window = []
             self.injected_indices = None
-        else:
+        elif b == 1:
             self._focal = self.model.intrinsics.focal_length.data
         z = lambda t: torch.zeros_like(t)  # noqa: E731
         self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog),
                        z(self._focal), z(self._focal)]
         self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
         self._g_focal = torch.zeros_like(self._focal)
-        self._k4 = torch.empty(f, 4, device=dev)
-        self._g_k4 = torch.empty(f, 4, device=dev)
-        self.rt = torch.empty(1, f - 1, 3, 4, device=dev)
-        self._loss = torch.zeros((), device=dev)
-        self._track_loss = torch.zeros((), device=dev)
-        self._ws = ops.workspace(1, f, h, w, dev)
-        self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
+        self._k4 = torch.empty(b * f, 4, device=dev)
+        self._g_k4 = torch.empty(b * f, 4, device=dev)
+        self.rt = torch.empty(b, f - 1, 3, 4, device=dev)
+        self._loss = torch.zeros(() if b == 1 else (b,), device=dev)
+        self._track_loss = torch.zeros_like(self._loss)
+        self._ws = ops.workspace(b, f, h, w, dev)
+        self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask) if b == 1 else \
+            self._video_mask_sums(self.flows)
         self._indices = self.model.extrinsics.select_indices(h, w, dev) \
             if not cfg.procrustes_randomize else None
         a = OverfitStepArgs()
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        a.F, a.H, a.W = f, h, w
+        a.F, a.H, a.W, a.B = f, h, w, b
         a.depth = P(self._depth)
         a.weight_logits = P(self._wlog) if cfg.use_correspondence_weights else None
         a.weight_sensitivity = cfg.weight_sensitivity
@@ -219,7 +249,7 @@ class FusedOverfitter(Overfitter):
         self._clock = ops.StepClock(dev, cfg.lr)
         self._side_stream = torch.cuda.Stream(device=dev)  # parallel branch of the step (see _step_softmin)
         a.clock = self._clock.ptr
-        self._total = torch.zeros((), device=dev)
+        self._total = torch.zeros_like(self._loss)
         self._idx_buf = torch.empty(min(cfg.softmin_points, h * w), dtype=torch.int64, device=dev) \
             if self._softmin else None
         self.use_cuda_graph = False  # opt-in: replay the update step as ONE CUDA graph launch
@@ -228,15 +258,15 @@ class FusedOverfitter(Overfitter):
         self._packed = None
         if cfg.use_tracking:
             assert self.tracks is not None
-            pk = ops.PackedTracks(self.tracks, dev)
+            pk = ops.PackedTracks(self.tracks, dev, f if b > 1 else None)
             self._packed = pk
             self._pk_c = PackedTracksC(P(pk.seg), P(pk.xy), P(pk.vis), pk.num_segments,
                                        pk.max_rows, pk.max_points, pk.total)
-            self._ext = torch.empty(1, f, 4, 4, device=dev)
-            self._g_ext = torch.empty(1, f, 4, 4, device=dev)
-            self._g_rt = torch.empty(1, f - 1, 3, 4, device=dev)
-            self._tg_k4 = torch.empty(f, 4, device=dev)
-            self._tws = torch.empty(lib().fm_track_workspace_bytes(f, pk.total), dtype=torch.uint8,
+            self._ext = torch.empty(b, f, 4, 4, device=dev)
+            self._g_ext = torch.empty(b, f, 4, 4, device=dev)
+            self._g_rt = torch.empty(b, f - 1, 3, 4, device=dev)
+            self._tg_k4 = torch.empty(b * f, 4, device=dev)
+            self._tws = torch.empty(lib().fm_track_workspace_bytes(b * f, pk.total), dtype=torch.uint8,
                                     device=dev)
             a.track_weight = cfg.tracking_weight
             a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
@@ -274,7 +304,43 @@ class FusedOverfitter(Overfitter):
         self._eager_runs.clear()
 
     def _mask_sum(self, flows: Flows) -> Tensor:
+        if self.B > 1:
+            return self._video_mask_sums(flows)
         return ops.mask_sum(flows.forward_mask, flows.backward_mask)
+
+    @staticmethod
+    def _video_mask_sums(flows: Flows) -> Tensor:
+        """(B,) float64: each video's own flow-loss normaliser."""
+        fm, bm = flows.forward_mask, flows.backward_mask
+        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(fm.shape[0])])
+
+    def _bind_batched_parameters(self):
+        """B > 1: the videos' parameters move into (B, ...) buffers that the step updates in place; each
+        video's Model keeps views of its rows, so state_dict() and the exports read them without a copy."""
+        def stack(params):
+            buf = torch.stack([p.data for p in params]).contiguous()
+            for i, p in enumerate(params):
+                p.data = buf[i]
+            return buf
+        self._depth = stack([m.backbone.depth for m in self.models])
+        self._wlog = stack([m.backbone.weights for m in self.models])
+        if self.cfg.intrinsics != "softmin":
+            self._focal = stack([m.intrinsics.focal_length for m in self.models])
+        elif self.cfg.regression_after is not None:
+            self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
+
+    def _adam_frames(self, i: int, lo: int, hi: int):
+        """Adam (step clock) on frames lo <= f < hi of every video of parameter i (0 depth, 1 weight logits)."""
+        p, g = ((self._depth, self._g_depth), (self._wlog, self._g_w))[i]
+        m, v = self._state[2 * i], self._state[2 * i + 1]
+        if self.B == 1:
+            ops.adam_step_clock(p[lo:hi], g[lo:hi], m[lo:hi], v[lo:hi], self._clock)
+        else:
+            ops.adam_step_clock_frames(p, g, m, v, lo, hi, self._clock)
+
+    def _window_entry(self) -> Tensor:
+        """The sweep's focal estimate for the hand-over window: a scalar, or (B,) for B videos."""
+        return self._sw_focal[0].clone() if self.B == 1 else self._sw_focal.clone()
 
     def _softmin_stage(self) -> bool:
         c = self.cfg
@@ -286,7 +352,7 @@ class FusedOverfitter(Overfitter):
         the step itself with that focal length, the sweep's backward, then Adam."""
         from ._lib import check
         c, a, L = self.cfg, self._args, self._lib
-        _, f, _, h, w = self.batch.videos.shape
+        b, f, _, h, w = self.batch.videos.shape
         dev = self.rt.device
         st = torch.cuda.current_stream().cuda_stream
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
@@ -301,8 +367,8 @@ class FusedOverfitter(Overfitter):
         with torch.cuda.device(dev):
             if early_moments:
                 self._side_stream.wait_stream(cur)
-                check(L.fm_procrustes_moments(P(self._depth), P(self._k4_base), P(self.flows.backward), wl, sens,
-                                              P(self._ws), f, h, w, st), "fm_procrustes_moments")
+                check(L.fm_procrustes_moments_batched(P(self._depth), P(self._k4_base), P(self.flows.backward), wl,
+                                                      sens, P(self._ws), b, f, h, w, st), "fm_procrustes_moments")
             with torch.cuda.stream(self._side_stream if early_moments else cur):
                 sst = torch.cuda.current_stream().cuda_stream
                 idx = self.injected_indices
@@ -314,16 +380,17 @@ class FusedOverfitter(Overfitter):
                 idx = idx.contiguous()
                 check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
                                              idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                             P(self._sw_rt), P(self._sw_ws), 1, f, h, w, sst),
+                                             P(self._sw_rt), P(self._sw_ws), b, f, h, w, sst),
                       "fm_softmin_sweep_fwd")
-                check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, 1, P(self._sw_sm),
+                check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, b, P(self._sw_sm),
                                          P(self._sw_focal), sst), "fm_softmin_focal")
             if early_moments:
                 cur.wait_stream(self._side_stream)
             a.moments_k4 = P(self._k4_base) if early_moments else None
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
-            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0
+            # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
+            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and b == 1
             a.focal = P(self._sw_focal)
             a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
             a.defer_adam = 1 if fuse else 0
@@ -340,23 +407,19 @@ class FusedOverfitter(Overfitter):
                 side = self._side_stream
                 side.wait_stream(cur)
                 with torch.cuda.stream(side):
-                    ops.adam_step_clock(self._depth[2:], self._g_depth[2:], self._state[0][2:], self._state[1][2:],
-                                        self._clock)
+                    self._adam_frames(0, 2, f)
             check(L.fm_softmin_focal_bwd(P(self._sw_sm), P(self._cand_f), P(self._sw_focal),
-                                         P(self._g_focal), n, 1, P(self._sw_gerr), st),
+                                         P(self._g_focal), n, b, P(self._sw_gerr), st),
                   "fm_softmin_focal_bwd")
             check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
                                          idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
                                          P(self._sw_gerr), P(self._g_depth),
-                                         P(self._g_w) if wl else None, P(self._sw_ws), 1, f, h, w, st),
+                                         P(self._g_w) if wl else None, P(self._sw_ws), b, f, h, w, st),
                   "fm_softmin_sweep_bwd")
         if update:
-            ops.adam_step_clock(self._depth[:2], self._g_depth[:2], self._state[0][:2], self._state[1][:2],
-                                self._clock)
+            self._adam_frames(0, 0, 2)
             if c.use_correspondence_weights:
-                k = 1 if fuse else self._wlog.shape[0]  # pair 0 only when the rest was fused
-                ops.adam_step_clock(self._wlog[:k], self._g_w[:k], self._state[2][:k], self._state[3][:k],
-                                    self._clock)
+                self._adam_frames(1, 0, 1 if fuse else f - 1)  # pair 0 only when the rest was fused
             if side is not None:
                 cur.wait_stream(side)
 
@@ -514,7 +577,8 @@ class FusedOverfitter(Overfitter):
                 self._eager_runs[key] = self._eager_runs.get(key, 0) + 1
 
     def training_step(self, update: bool = True):
-        """Returns (total loss (device tensor), relative poses rt (1, F-1, 3, 4))."""
+        """Returns (total loss (device tensor: a scalar, or the (B,) per-video totals), relative poses
+        rt (B, F-1, 3, 4))."""
         c, a = self.cfg, self._args
         if c.procrustes_randomize:
             _, _, _, h, w = self.batch.videos.shape
@@ -526,7 +590,8 @@ class FusedOverfitter(Overfitter):
         if update:
             self._clock.set(self.optimizer_steps, self.focal_steps)
             if self._softmin and not sweep and self.global_step == c.regression_after:
-                self._focal.copy_(torch.stack(self.window).mean())  # hand-over: seed the regressed focal length once
+                # hand-over: seed the regressed focal length (each video's) once
+                self._focal.copy_(torch.stack(self.window).mean(0))
         window_on = sweep and c.regression_after is not None and \
             self.global_step >= c.regression_after - c.regression_window
         key = (track_on, sweep, self.global_step >= c.flow_enable_after)
@@ -535,7 +600,7 @@ class FusedOverfitter(Overfitter):
         self._run_body(key, graphable, lambda upd=update: self._step_body(upd, track_on, sweep), not sweep)
         if update:
             if window_on:
-                self.window.append(self._sw_focal[0].clone())
+                self.window.append(self._window_entry())
             self.global_step += 1
             self.optimizer_steps += 1
             self.focal_steps += int(not sweep)
@@ -549,8 +614,8 @@ class FusedOverfitter(Overfitter):
         return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
 
     def intrinsics_k4(self) -> Tensor:
-        """(F, 4) = (fx, fy, cx, cy) used by the last step."""
-        return self._k4
+        """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for B videos."""
+        return self._k4 if self.B == 1 else self._k4.view(self.B, -1, 4)
 
     METRIC_NAMES = ("train/loss/flow", "train/loss/tracking", "train/intrinsics/fx_error",
                     "train/intrinsics/fy_error", "metrics/ate")
@@ -570,37 +635,46 @@ class FusedOverfitter(Overfitter):
         val_check_interval: 1) evaluates the updated parameters: that is row k + 1."""
         if capacity < 1:
             raise ValueError("flowmap_b200: the metrics log needs a capacity >= 1")
-        b, dev = self.batch, self.rt.device
+        b, dev, B = self.batch, self.rt.device, self.B
         _, f, _, _, _ = b.videos.shape
         nan = float("nan")
-        self._mlog_gt = None if b.extrinsics is None else \
-            b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
-        if b.intrinsics is None:
+        if B == 1:
+            self._mlog_gt = None if b.extrinsics is None else \
+                b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
+            if b.intrinsics is None:
+                fx = fy = nan
+            else:
+                k = b.intrinsics[0].double()
+                fx, fy = float(k[:, 0, 0].mean()), float(k[:, 1, 1].mean())
+        else:  # per video; a video whose ground truth is NaN gets NaN columns
+            self._mlog_gt = None if b.extrinsics is None else \
+                b.extrinsics[:, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
+            self._mlog_fxfy = torch.full((B, 2), nan) if b.intrinsics is None else \
+                torch.stack((b.intrinsics[:, :, 0, 0].double().mean(1), b.intrinsics[:, :, 1, 1].double().mean(1)), 1)
+            self._mlog_fxfy = self._mlog_fxfy.to(device=dev, dtype=torch.float32).contiguous()
             fx = fy = nan
-        else:
-            k = b.intrinsics[0].double()
-            fx, fy = float(k[:, 0, 0].mean()), float(k[:, 1, 1].mean())
         if getattr(self, "_ext", None) is None:  # flow-only steps chain the poses for the log
-            self._ext = torch.empty(1, f, 4, 4, device=dev)
-        self._mlog = torch.full((capacity, 5), nan, device=dev)
+            self._ext = torch.empty(B, f, 4, 4, device=dev)
+        self._mlog = torch.full((capacity, 5) if B == 1 else (capacity, B, 5), nan, device=dev)
         self._mlog_first = self.optimizer_steps
         a = self._args
         a.extrinsics = self._ext.data_ptr()
         a.gt_positions = None if self._mlog_gt is None else self._mlog_gt.data_ptr()
         a.gt_fx, a.gt_fy, a.metrics_capacity = fx, fy, capacity
+        a.gt_fxfy = None if B == 1 else self._mlog_fxfy.data_ptr()
         self._graphs.clear()  # captured steps were recorded without the log
         self._eager_runs.clear()
 
     def metrics_log(self) -> dict:
         """The logged rows of the update steps run since enable_metrics_log (the last `capacity` of
-        them), in step order, as CPU float32 tensors keyed by the reference's log names.  One host
-        synchronisation."""
+        them), in step order, as CPU float32 tensors keyed by the reference's log names: (steps,), or
+        (steps, B) with B videos.  One host synchronisation."""
         if self._mlog is None:
             raise ValueError("flowmap_b200: the metrics log is off (enable_metrics_log)")
         cap = self._mlog.shape[0]
         steps = torch.arange(max(self._mlog_first, self.optimizer_steps - cap), self.optimizer_steps)
         rows = self._mlog[(steps % cap).to(self._mlog.device)].cpu()
-        return {name: rows[:, i] for i, name in enumerate(self.METRIC_NAMES)}
+        return {name: rows[..., i] for i, name in enumerate(self.METRIC_NAMES)}
 
 
 class ShardedFusedOverfitter(FusedOverfitter):
@@ -627,6 +701,8 @@ class ShardedFusedOverfitter(FusedOverfitter):
         from dataclasses import replace
         from . import parallel
         from ._lib import lib
+        if batch.videos.shape[0] != 1:
+            raise ValueError("flowmap_b200: pair sharding optimises one video (batch size 1)")
         super().__init__(replace(cfg, use_tracking=False), batch, flows, None, device)
         self.cfg = cfg
         self.plan, self.group = plan, group

@@ -246,6 +246,12 @@ int fm_step_clock_tick(void* clock, double lr, double beta1, double beta2, unsig
 int fm_adam_step_clock(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t count,
                        const void* clock, int focal_clock, double beta1, double beta2, double eps, void* stream);
 int fm_random_subset_clock(const void* clock, long long N, int n, int64_t* out, void* stream);
+/* fm_adam_step_clock on the frames frame_lo <= f < frame_hi of each video of a (B, F, frame_elems)
+ * parameter: one launch for the same frames of every video (the batched step's softmin stage, where the
+ * sweep still adds to frames 0 / 1 of each video while the others are final). */
+int fm_adam_step_clock_frames(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t frame_elems,
+                              int B, int F, int frame_lo, int frame_hi, const void* clock, int focal_clock,
+                              double beta1, double beta2, double eps, void* stream);
 
 /* intrinsics_softmin.py:84-131, the candidate sweep on the first frame pair.  For each of
  * the num_candidates intrinsics in cand_k4 (B*num_candidates, 2, 4: one k4 row per virtual
@@ -364,6 +370,19 @@ typedef struct {
   float gt_fx, gt_fy;            /* frame means of the normalised GT intrinsics, NaN: columns NaN */
   float* metrics_log;            /* (metrics_capacity, 5) ring, or NULL = off */
   int metrics_capacity;
+  /* Number of videos (0 or 1: one).  B > 1 optimises B independent videos of the same (F, H, W) in one
+     step: every per-frame / per-pair buffer above has the (B, F, ...) / (B, F-1, ...) layout, and focal,
+     mask_sum, loss, track_loss, g_focal, m_focal and v_focal hold B values.  Video b's flow loss is
+     normalised by its own mask_sum[b] and its tracking loss by its own valid count ("or 1" per video);
+     its gradients are those of a one-video step on video b.  (The reference's LossFlow normalises a batch
+     by ONE pooled mask sum; this is B overfit runs, not a pooled batch.)  Tracks: the segments of video b
+     carry start frames b * F + s (they never cross videos); track_ws is fm_track_workspace_bytes(B * F,
+     total_samples).  The metrics ring is (metrics_capacity, B, 5), gt_positions (B, F, 3) with a NaN
+     first position for a video without ground truth.  B > 1 needs phase FM_STEP_ALL and no splat plan,
+     and refuses defer_adam = 1 together with step > 0 and weight logits (the caller updates the logits
+     after the sweep's backward). */
+  int B;
+  const float* gt_fxfy;          /* B > 1 with metrics_log: (B, 2) frame means of the GT intrinsics, NaN: none */
 } fm_overfit_step_args;
 #define FM_STEP_ALL 0
 #define FM_STEP_FORWARD 1
@@ -383,6 +402,10 @@ int fm_overfit_step(const fm_overfit_step_args* args, void* stream);
 int fm_procrustes_moments(const float* depth, const float* k4, const float* backward_flow,
                           const float* weights, float weight_sensitivity, void* ws, int F, int H, int W,
                           void* stream);
+/* The same for B videos (depth (B,F,H,W), k4 (B*F,4), ...): the moment pass of a B-video step. */
+int fm_procrustes_moments_batched(const float* depth, const float* k4, const float* backward_flow,
+                                  const float* weights, float weight_sensitivity, void* ws, int B, int F, int H,
+                                  int W, void* stream);
 
 /* ---- stages either side of the hot path (SURVEY 8(f) rank 4) ---------------------------- */
 
