@@ -113,7 +113,26 @@ class OverfitStepArgs(ctypes.Structure):
                 ("metrics_capacity", c_int), ("B", c_int), ("gt_fxfy", _P)]
 
 
+class VideoLayout(ctypes.Structure):
+    """fm_video_layout: videos of different lengths packed along the frame axis (device tables)"""
+    _fields_ = [("B", c_int), ("T", c_int), ("frame_offset", _P), ("frame_video", _P), ("pair_video", _P)]
+
+
+_L = ctypes.POINTER(VideoLayout)
 SIGNATURES["fm_overfit_step"] = (c_int, [ctypes.POINTER(OverfitStepArgs), _P])
+SIGNATURES.update({
+    "fm_overfit_step_videos": (c_int, [ctypes.POINTER(OverfitStepArgs), _L, _P]),
+    "fm_workspace_bytes_videos": (c_size_t, [c_int, c_int]),
+    "fm_procrustes_moments_videos": (c_int, [_P, _P, _P, _P, c_float, _P, _L, c_int, c_int, _P]),
+    "fm_softmin_sweep_fwd_videos": (c_int, [_P, _P, c_float, _P, _P, c_int, _P, c_int, _P, _P, _P, _L, c_int,
+                                            c_int, _P]),
+    "fm_softmin_sweep_bwd_videos": (c_int, [_P, _P, c_float, _P, _P, c_int, _P, c_int, _P, _P, _P, _P, _P, _L,
+                                            c_int, c_int, _P]),
+    "fm_adam_step_clock_frames_videos": (c_int, [_P, _P, _P, _P, c_size_t, _L, c_int, c_int, c_int, _P, c_int,
+                                                 c_double, c_double, c_double, _P]),
+    "fm_pose_chain_videos": (c_int, [_P, _P, _L, _P]),
+    "fm_pose_chain_bwd_videos": (c_int, [_P, _P, _P, _P, _L, _P]),
+})
 
 
 class FlowmapLibraryError(RuntimeError):

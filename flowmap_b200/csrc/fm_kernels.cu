@@ -76,8 +76,8 @@ struct Workspace {
 
 __host__ __device__ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-Workspace carve(void* base, int B, int F) {
-  const size_t BP = (size_t)B * (F - 1), BF = (size_t)B * F;
+// B videos with BF frames and BP frame pairs in all (videos of different lengths: fm_video_layout)
+Workspace carve_rows(void* base, int B, size_t BF, size_t BP) {
   char* p = (char*)base;
   size_t off = 0;
   Workspace w;
@@ -93,6 +93,23 @@ Workspace carve(void* base, int B, int F) {
   w.bytes = off;
   return w;
 }
+
+Workspace carve(void* base, int B, int F) { return carve_rows(base, B, (size_t)B * F, (size_t)B * (F - 1)); }
+
+// Videos of different lengths packed along the frame axis (fm_video_layout): video b owns the frames
+// [frame_offset[b], frame_offset[b + 1]) of the (T, ...) buffers and the pairs [frame_offset[b] - b,
+// frame_offset[b + 1] - b - 1) of the (P, ...) ones, P = T - B.  Pair p of video b joins frames p + b and
+// p + b + 1, so no pair crosses two videos.  The ragged kernels find a frame's or a pair's video in these
+// tables where their uniform siblings divide by F or F - 1.
+struct Videos {
+  const int* frame_offset;  // [B + 1]
+  const int* frame_video;   // [T]
+  const int* pair_video;    // [P]
+  __device__ __forceinline__ int of_frame(int t) const { return __ldg(frame_video + t); }
+  __device__ __forceinline__ int of_pair(int p) const { return __ldg(pair_video + p); }
+  __device__ __forceinline__ int first(int b) const { return __ldg(frame_offset + b); }
+  __device__ __forceinline__ int frames(int b) const { return __ldg(frame_offset + b + 1) - __ldg(frame_offset + b); }
+};
 
 // ---------------------------------------------------------------- small device helpers
 __device__ __forceinline__ K4 load_k4(const float* k4, int frame) {
@@ -331,6 +348,29 @@ __device__ __forceinline__ PairAddr pair_addr(const PairLayout& l, int pair, int
   a.weight = rb * l.weight_bs + (long long)i * N;
   return a;
 }
+// The ragged layouts (Videos): every pair of the packed (P, ...) buffers, or -- the focal-length sweep --
+// `cand` virtual items per video that all read its pair 0 (k4 rows: two per virtual item, as in the
+// uniform sweep).
+struct RaggedPairs { Videos v; };
+struct RaggedSweep { Videos v; int cand; };
+__device__ __forceinline__ PairAddr pair_addr(const RaggedPairs& l, int pair, int N) {
+  const int fa = pair + l.v.of_pair(pair);
+  PairAddr a;
+  a.k4_frame_a = fa;
+  a.depth_a = (long long)fa * N;
+  a.flow = (long long)pair * N * 2;
+  a.weight = (long long)pair * N;
+  return a;
+}
+__device__ __forceinline__ PairAddr pair_addr(const RaggedSweep& l, int item, int N) {
+  const int b = item / l.cand, fa = l.v.first(b), p = fa - b;
+  PairAddr a;
+  a.k4_frame_a = item * 2;
+  a.depth_a = (long long)fa * N;
+  a.flow = (long long)p * N * 2;
+  a.weight = (long long)p * N;
+  return a;
+}
 // z0: the pair's stored conditioning shift (the forward reads it from Workspace::zshift, the
 // backward from its PairAdjoint, which the solve filled from the same value).
 __device__ __forceinline__ PairGeom pair_geom(const float* k4, const PairAddr& pa, int H, int W, float z0) {
@@ -344,9 +384,12 @@ __device__ __forceinline__ PairGeom pair_geom(const float* k4, const PairAddr& p
 
 // The conditioning shift of every moment pair (shift_sample / shift_from_sums in fm_pixel.cuh): one
 // block per pair, kShiftSamples gathers of the later frame's depth and the pair's weights.
-__global__ void __launch_bounds__(kThreads)
-k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
-             float* __restrict__ zshift, PairLayout lay, int H, int W) {
+// Each Procrustes kernel below is a force-inlined body templated on its pair layout, instantiated as the
+// uniform kernel (PairLayout) and as a `_ragged` kernel of its own name (RaggedPairs / RaggedSweep).
+template <class Lay>
+__device__ __forceinline__ void pair_shift_body(const float* __restrict__ depth, const float* __restrict__ weights,
+                                                float wsens, float* __restrict__ zshift, const Lay& lay, int H,
+                                                int W) {
   __shared__ double smem[3][kThreads / 32];
   const int pair = blockIdx.x, N = H * W;
   const PairAddr pa = pair_addr(lay, pair, N);
@@ -373,12 +416,24 @@ k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights,
   }
 }
 
-template <int VEC>
-__global__ void __launch_bounds__(kThreads, 3)
-k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
-          const float* __restrict__ bflow, const float* __restrict__ weights,
-          const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
-          const float* __restrict__ zshift, float wsens, PairLayout lay, int H, int W) {
+__global__ void __launch_bounds__(kThreads)
+k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
+             float* __restrict__ zshift, PairLayout lay, int H, int W) {
+  pair_shift_body(depth, weights, wsens, zshift, lay, H, W);
+}
+template <class Lay>
+__global__ void __launch_bounds__(kThreads)
+k_pair_shift_ragged(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
+                    float* __restrict__ zshift, Lay lay, int H, int W) {
+  pair_shift_body(depth, weights, wsens, zshift, lay, H, W);
+}
+
+template <int VEC, class Lay>
+__device__ __forceinline__ void moments_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                             const float* __restrict__ bflow, const float* __restrict__ weights,
+                                             const int64_t* __restrict__ indices, int num_indices,
+                                             double* __restrict__ moments, const float* __restrict__ zshift,
+                                             float wsens, const Lay& lay, int H, int W) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int pair = blockIdx.y;
   const int N = H * W;
@@ -409,12 +464,28 @@ k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
   block_accumulate<kNumMoments>(acc, moments + (size_t)pair * kNumMoments, smem);
 }
 
-template <int VEC, int LX>
+template <int VEC>
 __global__ void __launch_bounds__(kThreads, 3)
-k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
-                const float* __restrict__ bflow, const float* __restrict__ weights,
-                double* __restrict__ moments, const float* __restrict__ zshift, float wsens, PairLayout lay,
-                int H, int W, int BP, int rounds) {
+k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
+          const float* __restrict__ bflow, const float* __restrict__ weights,
+          const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
+          const float* __restrict__ zshift, float wsens, PairLayout lay, int H, int W) {
+  moments_body<VEC>(depth, k4, bflow, weights, indices, num_indices, moments, zshift, wsens, lay, H, W);
+}
+template <int VEC, class Lay>
+__global__ void __launch_bounds__(kThreads, 3)
+k_moments_ragged(const float* __restrict__ depth, const float* __restrict__ k4,
+                 const float* __restrict__ bflow, const float* __restrict__ weights,
+                 const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
+                 const float* __restrict__ zshift, float wsens, Lay lay, int H, int W) {
+  moments_body<VEC>(depth, k4, bflow, weights, indices, num_indices, moments, zshift, wsens, lay, H, W);
+}
+
+template <int VEC, int LX, class Lay>
+__device__ __forceinline__ void moments_dense_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                                   const float* __restrict__ bflow, const float* __restrict__ weights,
+                                                   double* __restrict__ moments, const float* __restrict__ zshift,
+                                                   float wsens, const Lay& lay, int H, int W, int BP, int rounds) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int N = H * W;
   constexpr int kChunk = kThreads * VEC;
@@ -478,15 +549,33 @@ k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
   }
 }
 
+template <int VEC, int LX>
+__global__ void __launch_bounds__(kThreads, 3)
+k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
+                const float* __restrict__ bflow, const float* __restrict__ weights,
+                double* __restrict__ moments, const float* __restrict__ zshift, float wsens, PairLayout lay,
+                int H, int W, int BP, int rounds) {
+  moments_dense_body<VEC, LX>(depth, k4, bflow, weights, moments, zshift, wsens, lay, H, W, BP, rounds);
+}
+template <int VEC, int LX>
+__global__ void __launch_bounds__(kThreads, 3)
+k_moments_dense_ragged(const float* __restrict__ depth, const float* __restrict__ k4,
+                       const float* __restrict__ bflow, const float* __restrict__ weights,
+                       double* __restrict__ moments, const float* __restrict__ zshift, float wsens, RaggedPairs lay,
+                       int H, int W, int BP, int rounds) {
+  moments_dense_body<VEC, LX>(depth, k4, bflow, weights, moments, zshift, wsens, lay, H, W, BP, rounds);
+}
+
 // ================================================================== phase B: solve
 // moments_k4 != NULL: the sums were accumulated with the intrinsics moments_k4 (same principal points,
 // other focal lengths) before the step's own K was known.  Points scale per axis with the focal
 // ratio (p = S_b p', q = S_a q', S = diag(fx'/fx, fy'/fy, 1); the conditioning shift is along z), so
 // the 16 sums are rescaled exactly here -- and written back for later readers of the workspace.
-__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ zshift,
-                        float* __restrict__ rt, PairState* __restrict__ state, int BP, PairLayout lay,
-                        int H, int W, const float* __restrict__ moments_k4 = nullptr,
-                        const float* __restrict__ k4 = nullptr) {
+template <class Lay>
+__device__ __forceinline__ void solve_body(double* __restrict__ moments, const float* __restrict__ zshift,
+                                           float* __restrict__ rt, PairState* __restrict__ state, int BP,
+                                           const Lay& lay, int H, int W, const float* __restrict__ moments_k4,
+                                           const float* __restrict__ k4) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   const PairAddr pa = pair_addr(lay, pair, H * W);
@@ -510,6 +599,18 @@ __global__ void k_solve(double* __restrict__ moments, const float* __restrict__ 
   procrustes_solve(m, shift, out, st);
   for (int k = 0; k < 12; ++k) rt[(size_t)pair * 12 + k] = out[k];
   state[pair] = st;
+}
+
+__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ zshift,
+                        float* __restrict__ rt, PairState* __restrict__ state, int BP, PairLayout lay,
+                        int H, int W, const float* __restrict__ moments_k4 = nullptr,
+                        const float* __restrict__ k4 = nullptr) {
+  solve_body(moments, zshift, rt, state, BP, lay, H, W, moments_k4, k4);
+}
+__global__ void k_solve_ragged(double* __restrict__ moments, const float* __restrict__ zshift,
+                               float* __restrict__ rt, PairState* __restrict__ state, int BP, RaggedPairs lay,
+                               int H, int W, const float* __restrict__ moments_k4, const float* __restrict__ k4) {
+  solve_body(moments, zshift, rt, state, BP, lay, H, W, moments_k4, k4);
 }
 
 // ================================================================== phase C: flow loss
@@ -767,22 +868,87 @@ k_flow_lean_videos(const float* __restrict__ depth, const float* __restrict__ k4
   }
 }
 
+
+// k_flow_lean_videos for videos of different lengths: the frame's video from the tables of `v`.  Its own
+// copy of the kernel: as a body shared with k_flow_lean_videos, the table lookups changed that kernel's code.
+template <int VEC, bool FOCAL, int MINB>
+__global__ void __launch_bounds__(kThreads, MINB)
+k_flow_lean_ragged(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
+                   const float* __restrict__ fflow, const float* __restrict__ bflow,
+                   const float* __restrict__ fmask, const float* __restrict__ bmask,
+                   const double* __restrict__ mask_sum, int mapping, float delta, float loss_weight,
+                   float* __restrict__ g_depth, double* __restrict__ leanacc, int H, int W, int BF, Videos v) {
+  __shared__ double smem[kFlowLeanVals * (kThreads / 32)];
+  const int N = H * W;
+  constexpr int kChunk = kThreads * VEC;
+  const int chunks = (N + kChunk - 1) / kChunk;
+  const ItemRange range = block_item_range((long long)BF * chunks);
+  const RobustCfg rc = make_robust(mapping, delta, H, W);
+  const GridDims grid = make_grid(H, W);
+#pragma unroll 1
+  for (int it = range.i0; it < range.i1;) {
+    const int frame = it / chunks, cb = it - frame * chunks;
+    const int ce = (cb + (range.i1 - it) < chunks) ? cb + (range.i1 - it) : chunks;
+    const int bi = v.of_frame(frame), i = frame - v.first(bi), F = v.frames(bi);
+    double den = mask_sum[bi];
+    if (den == 0.0) den = 1.0;  // loss_flow.py:70 "valid_sum or 1", per video
+    const float g = (float)((double)loss_weight / den);
+    const bool hasF = i < F - 1, hasB = i > 0;
+    FlowFrameLean f;
+    f.kk = make_cam(load_k4(k4, frame));
+    f.kn = make_cam(load_k4(k4, hasF ? frame + 1 : frame));
+    f.kp = make_cam(load_k4(k4, hasB ? frame - 1 : frame));
+    const int pairF = frame - bi, pairB = pairF - 1;
+    Rt tf, tb;
+    if (hasF) tf = load_rt(rt, pairF);
+    if (hasB) tb = load_rt(rt, pairB);
+    fill_lean(f, hasF ? &tf : nullptr, hasB ? &tb : nullptr);
+    const float* D = depth + (size_t)frame * N;
+    const float* ff = fflow + (size_t)(hasF ? pairF : 0) * N * 2;
+    const float* mf = fmask + (size_t)(hasF ? pairF : 0) * N;
+    const float* fb = bflow + (size_t)(hasB ? pairB : 0) * N * 2;
+    const float* mb = bmask + (size_t)(hasB ? pairB : 0) * N;
+    float* gd = g_depth + (size_t)frame * N;
+    float acc[kFlowLeanVals];
+#pragma unroll
+    for (int k = 0; k < kFlowLeanVals; ++k) acc[k] = 0.f;
+    if (hasF && hasB) flow_frame_body_lean<VEC, true, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    else if (hasF) flow_frame_body_lean<VEC, true, false, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    else flow_frame_body_lean<VEC, false, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
+    // lean slots live in the upper half of the frame's accumulator row until k_flow_lean_convert
+    block_accumulate<kFlowLeanVals>(acc, leanacc + (size_t)frame * kFlowAcc, smem);
+    it += ce - cb;
+  }
+}
+
 // Rewrites each frame's lean accumulators (slots 0-13) into the standard layout in place.
-__global__ void k_flow_lean_convert(double* __restrict__ flowacc, const float* __restrict__ rt,
-                                    const float* __restrict__ k4, int focal_mode, int B, int F, int H, int W) {
+template <bool RAGGED>
+__device__ __forceinline__ void flow_lean_convert_body(double* __restrict__ flowacc, const float* __restrict__ rt,
+                                                       const float* __restrict__ k4, int focal_mode, int BF, int F,
+                                                       int H, int W, const Videos& v) {
   const int frame = blockIdx.x * blockDim.x + threadIdx.x;
-  if (frame >= B * F) return;
-  const int bi = frame / F, i = frame - bi * F;
+  if (frame >= BF) return;
+  const int bi = RAGGED ? v.of_frame(frame) : frame / F, i = RAGGED ? frame - v.first(bi) : frame - bi * F;
   double lean[kFlowLeanVals], out[kFlowVals];
   double* row = flowacc + (size_t)frame * kFlowAcc;
   for (int k = 0; k < kFlowLeanVals; ++k) lean[k] = row[k];
-  const int pairF = bi * (F - 1) + i;
-  const float* rtF = i < F - 1 ? rt + (size_t)pairF * 12 : nullptr;
+  const int pairF = RAGGED ? frame - bi : bi * (F - 1) + i;
+  const float* rtF = i < (RAGGED ? v.frames(bi) : F) - 1 ? rt + (size_t)pairF * 12 : nullptr;
   const float* rtB = i > 0 ? rt + (size_t)(pairF - 1) * 12 : nullptr;
   const double s = sqrt((double)H * (double)W);
   const double focal = (double)k4[(size_t)frame * 4] * (double)W / s;
   lean_to_standard<double>(lean, rtF, rtB, focal, (double)W / s, focal_mode != 0, out);
   for (int k = 0; k < kFlowVals; ++k) row[k] = out[k];
+}
+
+__global__ void k_flow_lean_convert(double* __restrict__ flowacc, const float* __restrict__ rt,
+                                    const float* __restrict__ k4, int focal_mode, int B, int F, int H, int W) {
+  flow_lean_convert_body<false>(flowacc, rt, k4, focal_mode, B * F, F, H, W, Videos{});
+}
+__global__ void k_flow_lean_convert_ragged(double* __restrict__ flowacc, const float* __restrict__ rt,
+                                           const float* __restrict__ k4, int focal_mode, int T, int H, int W,
+                                           Videos v) {
+  flow_lean_convert_body<true>(flowacc, rt, k4, focal_mode, T, 0, H, W, v);
 }
 
 // Assemble dL/d[R|t] of pair p (float64, 12 values) from the per-frame accumulators.
@@ -798,6 +964,18 @@ __device__ inline void flow_pose_grad(const double* flowacc, const PairState* st
   for (int r = 0; r < 3; ++r) {
     for (int c = 0; c < 3; ++c) g[r * 4 + c] = fa[1 + r * 3 + c] + fb[13 + r * 3 + c];
     g[r * 4 + 3] = fb[22 + r] - (R[r * 3 + 0] * fa[10] + R[r * 3 + 1] * fa[11] + R[r * 3 + 2] * fa[12]);
+  }
+}
+// flow_pose_grad for videos of different lengths: pair p's earlier frame is p + (its video).
+__device__ inline void flow_pose_grad_ragged(const double* flowacc, const PairState* st, int pair, const Videos& v,
+                                             double* g) {
+  const int a = pair + v.of_pair(pair);
+  const double* fa = flowacc + (size_t)a * kFlowAcc;
+  const double* fb = fa + kFlowAcc;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) g[r * 4 + c] = fa[1 + r * 3 + c] + fb[13 + r * 3 + c];
+    g[r * 4 + 3] = fb[22 + r] - (st[pair].R[r * 3 + 0] * fa[10] + st[pair].R[r * 3 + 1] * fa[11] +
+                                 st[pair].R[r * 3 + 2] * fa[12]);
   }
 }
 
@@ -842,9 +1020,9 @@ __global__ void k_flow_finalize(const double* __restrict__ flowacc, const float*
 
 // The batched fused step's flow losses: block b sums the F per-frame loss terms of video b into loss[b],
 // in the order in which k_flow_finalize's block 0 sums them for one video (launched with 128 threads).
-__global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __restrict__ loss, int F) {
+// (k_flow_video_loss_ragged: video b's frames start at frame_offset[b] and number its own F.)
+__device__ __forceinline__ void flow_video_loss_body(const double* __restrict__ acc, float* __restrict__ loss, int F) {
   __shared__ double part[32];
-  const double* acc = flowacc + (size_t)blockIdx.x * F * kFlowAcc;
   double s = 0.0;
   for (int k = threadIdx.x; k < F; k += blockDim.x) s += acc[(size_t)k * kFlowAcc];
   s = warp_sum(s);
@@ -855,6 +1033,12 @@ __global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __r
     for (int w = 0; w < (int)((blockDim.x + 31) >> 5); ++w) tot += part[w];
     loss[blockIdx.x] = (float)tot;
   }
+}
+__global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __restrict__ loss, int F) {
+  flow_video_loss_body(flowacc + (size_t)blockIdx.x * F * kFlowAcc, loss, F);
+}
+__global__ void k_flow_video_loss_ragged(const double* __restrict__ flowacc, float* __restrict__ loss, Videos v) {
+  flow_video_loss_body(flowacc + (size_t)v.first(blockIdx.x) * kFlowAcc, loss, v.frames(blockIdx.x));
 }
 
 // ================================================================== phase D1: adjoint solve
@@ -890,6 +1074,25 @@ __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* _
   adj[pair] = out;
 }
 
+// k_adjoint for videos of different lengths (no focal_moments: the splat plan serves one video).
+__global__ void k_adjoint_ragged(const double* __restrict__ flowacc, const PairState* __restrict__ state,
+                                 const float* __restrict__ g_rt, int include_flow, const float* __restrict__ flow_scale,
+                                 PairAdjoint* __restrict__ adj, int BP, Videos v) {
+  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pair >= BP) return;
+  double g[12];
+  for (int k = 0; k < 12; ++k) g[k] = 0.0;
+  if (include_flow) {
+    flow_pose_grad_ragged(flowacc, state, pair, v, g);
+    const double s = flow_scale ? (double)*flow_scale : 1.0;
+    for (int k = 0; k < 12; ++k) g[k] *= s;
+  }
+  if (g_rt) for (int k = 0; k < 12; ++k) g[k] += (double)g_rt[(size_t)pair * 12 + k];
+  PairAdjoint out;
+  procrustes_adjoint(state[pair], g, out);
+  adj[pair] = out;
+}
+
 // ================================================================== phase D2: distribute
 // Optional Adam update of the weight logits inside phase D2 (dense path): their gradient is
 // final there and the kernel is bound by its scatter, not HBM, so the 28 B/parameter of a separate
@@ -902,14 +1105,13 @@ struct AdamFuse {
   const float* consts;  // device {step_size, bc2_sqrt} of a step clock (CUDA-graph replays), or NULL
 };
 
-template <int VEC>
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute(const float* __restrict__ depth, const float* __restrict__ k4,
-             const float* __restrict__ bflow, float* weights,
-             const int64_t* __restrict__ indices, int num_indices,
-             const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
-             float* __restrict__ g_weights, double* __restrict__ k4acc, float wsens, PairLayout lay,
-             AdamFuse adam, int H, int W) {
+template <int VEC, class Lay>
+__device__ __forceinline__ void distribute_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                                const float* __restrict__ bflow, float* weights,
+                                                const int64_t* __restrict__ indices, int num_indices,
+                                                const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
+                                                float* __restrict__ g_weights, double* __restrict__ k4acc,
+                                                float wsens, Lay lay, AdamFuse adam, int H, int W) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   const int pair = blockIdx.y;
@@ -952,6 +1154,24 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4,
   // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
   block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
 }
+
+#define FM_DISTRIBUTE_PARAMS                                                                                  \
+  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
+      const int64_t* __restrict__ indices, int num_indices, const PairAdjoint* __restrict__ adj,               \
+      float* __restrict__ g_depth, float* __restrict__ g_weights, double* __restrict__ k4acc, float wsens
+template <int VEC>
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute(FM_DISTRIBUTE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W) {
+  distribute_body<VEC>(depth, k4, bflow, weights, indices, num_indices, adj, g_depth, g_weights, k4acc, wsens, lay,
+                       adam, H, W);
+}
+template <int VEC, class Lay>
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute_ragged(FM_DISTRIBUTE_PARAMS, Lay lay, AdamFuse adam, int H, int W) {
+  distribute_body<VEC>(depth, k4, bflow, weights, indices, num_indices, adj, g_depth, g_weights, k4acc, wsens, lay,
+                       adam, H, W);
+}
+#undef FM_DISTRIBUTE_PARAMS
 
 // Per-pixel work of the dense phase D2 for the VEC consecutive pixels of row r from column c0
 // (linear index base in the frame, wi = base + the pair's offset in the weight-shaped arrays): the
@@ -1021,11 +1241,13 @@ __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairA
 // Dense (all-pixel) phase D2 for widths that are not a multiple of 4: one pixel per thread on the
 // item decomposition of block_item_range (chunks of kThreads pixels), taps as REDs, per-pair constants
 // re-staged when a block moves on to its next pair.  The weight Adam runs as a separate pass.
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4,
-                   const float* __restrict__ bflow, float* weights, const PairAdjoint* __restrict__ adj,
-                   float* __restrict__ g_depth, float* __restrict__ g_weights, double* __restrict__ k4acc,
-                   float wsens, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
+template <class Lay>
+__device__ __forceinline__ void distribute_dense_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                                      const float* __restrict__ bflow, float* weights,
+                                                      const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
+                                                      float* __restrict__ g_weights, double* __restrict__ k4acc,
+                                                      float wsens, Lay lay, AdamFuse adam, int H, int W,
+                                                      int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   const int N = H * W;
@@ -1066,6 +1288,20 @@ k_distribute_dense(const float* __restrict__ depth, const float* __restrict__ k4
     i += ce - cb;
   }
   }
+}
+
+#define FM_DISTRIBUTE_DENSE_PARAMS                                                                            \
+  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
+      const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth, float* __restrict__ g_weights,        \
+      double* __restrict__ k4acc, float wsens
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute_dense(FM_DISTRIBUTE_DENSE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
+  distribute_dense_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
+}
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute_dense_ragged(FM_DISTRIBUTE_DENSE_PARAMS, RaggedPairs lay, AdamFuse adam, int H, int W, int BP,
+                          int rounds) {
+  distribute_dense_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
 }
 
 // Tile and halo of k_distribute_window (build-time knobs for tools/ab_libs.py).  With the defaults
@@ -1132,11 +1368,13 @@ namespace {
 // neighbouring windows overlap, and k_track_apply adds into the same gradient concurrently in
 // fm_overfit_step) and zeroed.  This replaces ~2.6 scattered 32-byte RED requests per pixel (bound by
 // the L2 atomic units) with ~0.7 coalesced ones.
-__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
-k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k4,
-                    const float* __restrict__ bflow, float* weights, const PairAdjoint* __restrict__ adj,
-                    float* __restrict__ g_depth, float* __restrict__ g_weights, double* __restrict__ k4acc,
-                    float wsens, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
+template <class Lay>
+__device__ __forceinline__ void distribute_window_body(const float* __restrict__ depth, const float* __restrict__ k4,
+                                                       const float* __restrict__ bflow, float* weights,
+                                                       const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
+                                                       float* __restrict__ g_weights, double* __restrict__ k4acc,
+                                                       float wsens, Lay lay, AdamFuse adam, int H,
+                                                       int W, int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   __shared__ PairGeom s_geom;
@@ -1245,6 +1483,17 @@ k_distribute_window(const float* __restrict__ depth, const float* __restrict__ k
   }
 }
 
+__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
+k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
+  distribute_window_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
+}
+__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
+k_distribute_window_ragged(FM_DISTRIBUTE_DENSE_PARAMS, RaggedPairs lay, AdamFuse adam, int H, int W, int BP,
+                           int rounds) {
+  distribute_window_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
+}
+#undef FM_DISTRIBUTE_DENSE_PARAMS
+
 #include "fm_tiled.cuh"
 
 __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
@@ -1255,6 +1504,21 @@ __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __
   double g[4] = {0, 0, 0, 0};
   if (include_flow) {
     flow_k4_grad(flowacc, t, F, g);
+    const double s = flow_scale ? (double)*flow_scale : 1.0;
+    for (int k = 0; k < 4; ++k) g[k] *= s;
+  }
+  for (int k = 0; k < 4; ++k) g_k4[(size_t)t * 4 + k] = (float)(g[k] + k4acc[(size_t)t * 4 + k]);
+}
+
+__global__ void k_k4_finalize_ragged(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                                     int include_flow, const float* __restrict__ flow_scale,
+                                     float* __restrict__ g_k4, int T, Videos v) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  double g[4] = {0, 0, 0, 0};
+  if (include_flow) {  // flow_k4_grad on video b's own frames
+    const int b = v.of_frame(t), f0 = v.first(b);
+    flow_k4_grad(flowacc + (size_t)f0 * kFlowAcc, t - f0, v.frames(b), g);
     const double s = flow_scale ? (double)*flow_scale : 1.0;
     for (int k = 0; k < 4; ++k) g[k] *= s;
   }
@@ -1415,14 +1679,18 @@ __device__ __forceinline__ Rigid rigid_from_smem(const float* src) {
   return r;
 }
 
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, int B, int F) {
+// RAGGED (k_pose_chain_ragged): block b chains video b of the packed layout from its own frame 0.
+template <bool RAGGED>
+__device__ __forceinline__ void pose_chain_body(const float* __restrict__ rt, float* __restrict__ ext, int F,
+                                                const Videos& v) {
   __shared__ float s_agg[12 * kChainThreads];
   const int b = blockIdx.x, t = threadIdx.x;
+  const int f0 = RAGGED ? v.first(b) : 0;
+  if (RAGGED) F = v.frames(b);
   const int P = F - 1;
   const int chunk = (P + kChainThreads - 1) / kChainThreads;
   const int lo = min(t * chunk, P), hi = min(lo + chunk, P);
-  const float* T = rt + (size_t)b * P * 12;
+  const float* T = RAGGED ? rt + (size_t)(f0 - b) * 12 : rt + (size_t)b * P * 12;
   Rigid agg = rigid_identity();
   for (int k = lo; k < hi; ++k) agg = rigid_mul(agg, rigid_load(T + (size_t)k * 12));
   rigid_to_smem(s_agg + t, agg);
@@ -1435,7 +1703,7 @@ k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, int B, int F
     __syncthreads();
   }
   Rigid run = t > 0 ? rigid_from_smem(s_agg + t - 1) : rigid_identity();  // exclusive prefix = P_lo
-  float* o = ext + (size_t)b * F * 16;
+  float* o = RAGGED ? ext + (size_t)f0 * 16 : ext + (size_t)b * F * 16;
   auto store = [o](int k, const Rigid& r) {
     float4* d = reinterpret_cast<float4*>(o + (size_t)k * 16);
     d[0] = make_float4(r.m[0], r.m[1], r.m[2], r.m[3]);
@@ -1450,23 +1718,35 @@ k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, int B, int F
   }
 }
 
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, int B, int F) {
+  pose_chain_body<false>(rt, ext, F, Videos{});
+}
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain_ragged(const float* __restrict__ rt, float* __restrict__ ext, Videos v) {
+  pose_chain_body<true>(rt, ext, 0, v);
+}
+
 // Adjoint of the chain.  With G_a = dL/dP_a (top 3 rows; the bottom row is constant):
 //   S_{F-1} = G_{F-1},  S_a = G_a + S_{a+1} T4_a^T,  dT_k = P_k^T S_{k+1} (3x4 part).
 // S_a = f_a(S_{a+1}) with the affine maps f_a(X) = G_a + X T4_a^T, whose composition
 // f_a o f_b (a < b) is the pair (T_a o T_b, G_a + G_b T4_a^T): a reverse (suffix) scan over the
 // elements a = 1 .. F-1, same block layout as the forward chain.
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext,
-                 const float* __restrict__ g_ext, float* __restrict__ g_rt, int B, int F) {
+template <bool RAGGED>
+__device__ __forceinline__ void pose_chain_bwd_body(const float* __restrict__ rt, const float* __restrict__ ext,
+                                                    const float* __restrict__ g_ext, float* __restrict__ g_rt, int F,
+                                                    const Videos& v) {
   __shared__ float s_t[12 * kChainThreads];
   __shared__ float s_b[12 * kChainThreads];
   const int b = blockIdx.x, t = threadIdx.x;
+  const int f0 = RAGGED ? v.first(b) : 0;
+  if (RAGGED) F = v.frames(b);
   const int n = F - 1;                       // elements j = a - 1 for a = 1 .. F-1
   const int chunk = (n + kChainThreads - 1) / kChainThreads;
   const int lo = min(t * chunk, n), hi = min(lo + chunk, n);
-  const float* T = rt + (size_t)b * n * 12;
-  const float* G = g_ext + (size_t)b * F * 16;
-  const float* Pm = ext + (size_t)b * F * 16;
+  const float* T = RAGGED ? rt + (size_t)(f0 - b) * 12 : rt + (size_t)b * n * 12;
+  const float* G = RAGGED ? g_ext + (size_t)f0 * 16 : g_ext + (size_t)b * F * 16;
+  const float* Pm = RAGGED ? ext + (size_t)f0 * 16 : ext + (size_t)b * F * 16;
   // element j: (T_a, G_a) with a = j + 1; the last one (a = F-1) has no T: identity
   auto elem_t = [T, n](int j) { return j + 1 < n + 0 ? rigid_load(T + (size_t)(j + 1) * 12) : rigid_identity(); };
   Rigid aggT = rigid_identity(), aggB;
@@ -1505,7 +1785,7 @@ k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext,
 #pragma unroll
     for (int i = 0; i < 12; ++i) S.m[i] = 0.f;
   }
-  float* out = g_rt + (size_t)b * n * 12;
+  float* out = RAGGED ? g_rt + (size_t)(f0 - b) * 12 : g_rt + (size_t)b * n * 12;
   for (int j = hi - 1; j >= lo; --j) {
     const Rigid tj = elem_t(j), gj = rigid_load(G + (size_t)(j + 1) * 16);
     const Rigid moved = mul_transposed(S, tj);
@@ -1523,6 +1803,17 @@ k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext,
     d[1] = make_float4(v[4], v[5], v[6], v[7]);
     d[2] = make_float4(v[8], v[9], v[10], v[11]);
   }
+}
+
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext,
+                 const float* __restrict__ g_ext, float* __restrict__ g_rt, int B, int F) {
+  pose_chain_bwd_body<false>(rt, ext, g_ext, g_rt, F, Videos{});
+}
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain_bwd_ragged(const float* __restrict__ rt, const float* __restrict__ ext,
+                        const float* __restrict__ g_ext, float* __restrict__ g_rt, Videos v) {
+  pose_chain_bwd_body<true>(rt, ext, g_ext, g_rt, 0, v);
 }
 
 // torch.optim.Adam (single-tensor, no amsgrad / weight decay), same operation order.
@@ -1566,6 +1857,26 @@ k_adam_frames(float* __restrict__ p, const float* __restrict__ g, float* __restr
   const float step_size = __ldg(consts), bc2_sqrt = __ldg(consts + 1);
   const int span = hi - lo, b = blockIdx.y / span, f = lo + (blockIdx.y - b * span);
   const size_t o = ((size_t)b * F + f) * frame_elems;
+  p += o; g += o; m += o; v += o;
+  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < frame_elems; i += (size_t)gridDim.x * kThreads) {
+    float pp = p[i], gg = g[i], mm = m[i], vv = v[i];
+    FM_ADAM1(pp, gg, mm, vv)
+    p[i] = pp; m[i] = mm; v[i] = vv;
+  }
+}
+
+// k_adam_frames for videos of different lengths: the rows lo <= r < min(hi, rows of video b) of every
+// video b, whose rows start at row_offset[b] - pairs * b and number row_offset[b + 1] - row_offset[b] - pairs
+// (row_offset = frame offsets; pairs = 0 for per-frame parameters, 1 for per-pair ones).
+__global__ void __launch_bounds__(kThreads)
+k_adam_frames_ragged(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                     size_t frame_elems, const int* __restrict__ row_offset, int pairs, int lo, int hi, float beta1,
+                     float beta2, float omb1, float omb2, float eps, const float* __restrict__ consts) {
+  const float step_size = __ldg(consts), bc2_sqrt = __ldg(consts + 1);
+  const int span = hi - lo, b = blockIdx.y / span, f = lo + (blockIdx.y - b * span);
+  const int r0 = __ldg(row_offset + b);
+  if (f >= __ldg(row_offset + b + 1) - r0 - pairs) return;
+  const size_t o = ((size_t)(r0 - pairs * b) + f) * frame_elems;
   p += o; g += o; m += o; v += o;
   for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < frame_elems; i += (size_t)gridDim.x * kThreads) {
     float pp = p[i], gg = g[i], mm = m[i], vv = v[i];
@@ -1760,8 +2071,14 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
 }
 
 // VIDEOS (the batched fused step): the segments of video b have start frames in [b F, (b + 1) F), F =
-// video_frames, and its loss sum / valid count go to sums[2 b], sums[2 b + 1].
-template <bool SHARED_K, bool VIDEOS>
+// video_frames, and its loss sum / valid count go to sums[2 b], sums[2 b + 1].  kRaggedVideos (videos of
+// different lengths): the video of a start frame is frame_video[start frame].
+constexpr int kRaggedVideos = 2;
+template <int VIDEOS>
+__device__ __forceinline__ int video_of_segment(int start_frame, int video_frames, const int* frame_video) {
+  return VIDEOS == kRaggedVideos ? __ldg(frame_video + start_frame) : start_frame / video_frames;
+}
+template <bool SHARED_K, int VIDEOS>
 __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, const float* __restrict__ k4,
                                                const float* __restrict__ ext, const int* __restrict__ seg,
                                                const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
@@ -1770,7 +2087,7 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
                                                double* __restrict__ trackacc, int* __restrict__ next_item,
                                                int num_items, int max_rows, int list_cap, int H, int W,
                                                TrackShard sh, int video_frames, float4* sm4, double* red,
-                                               int* s_wbase, int* s_item) {
+                                               int* s_wbase, int* s_item, const int* frame_video = nullptr) {
   float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
   constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
@@ -1968,7 +2285,8 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
       }
       __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
-    block_accumulate<2, kTrackThreads>(lc, VIDEOS ? sums + 2 * (si.start_frame / video_frames) : sums, red);
+    block_accumulate<2, kTrackThreads>(
+        lc, VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(si.start_frame, video_frames, frame_video) : sums, red);
     block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
     // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
     // with a barrier, so every slice is complete)
@@ -1999,12 +2317,17 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
 template <bool SHARED_K>
 __global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src(FM_TRACK_SRC_PARAMS) {
   FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, false>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item);
+  track_src_body<SHARED_K, 0>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item);
 }
 template <bool SHARED_K>
 __global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_videos(FM_TRACK_SRC_PARAMS, int video_frames) {
   FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, true>(FM_TRACK_SRC_ARGS, video_frames, sm4, red, s_wbase, s_item);
+  track_src_body<SHARED_K, 1>(FM_TRACK_SRC_ARGS, video_frames, sm4, red, s_wbase, s_item);
+}
+template <bool SHARED_K>
+__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_ragged(FM_TRACK_SRC_PARAMS, const int* frame_video) {
+  FM_TRACK_SRC_SHARED
+  track_src_body<SHARED_K, kRaggedVideos>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item, frame_video);
 }
 #undef FM_TRACK_SRC_SHARED
 #undef FM_TRACK_SRC_PARAMS
@@ -2028,20 +2351,21 @@ __global__ void k_track_video_loss(const double* __restrict__ sums, float loss_w
 
 // scale * (stored camera-space adjoint) -> the four depth taps of every source sample.  VIDEOS: the scale
 // of the segment's video (start frame / video_frames), see track_src_body.
-template <bool VIDEOS>
+template <int VIDEOS>
 __device__ __forceinline__ void track_apply_body(const float* __restrict__ k4, const int* __restrict__ seg,
                                                  const float* __restrict__ txy, const unsigned char* __restrict__ flag,
                                                  const float* __restrict__ dq, const double* __restrict__ sums,
                                                  float loss_weight, const float* __restrict__ go,
                                                  float* __restrict__ g_depth, int H, int W, TrackShard sh,
-                                                 int video_frames) {
+                                                 int video_frames, const int* frame_video = nullptr) {
   const SegInfo si = load_seg(seg, blockIdx.z);
   const int row = blockIdx.y;
   const int p = blockIdx.x * kThreads + threadIdx.x;
   if (row >= si.rows || p >= si.n || !sh.owns(si.start_frame + row)) return;
   const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p;
   if (!flag[sidx]) return;
-  const float scale = (float)track_scale(VIDEOS ? sums + 2 * (si.start_frame / video_frames) : sums, loss_weight, go);
+  const float scale = (float)track_scale(
+      VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(si.start_frame, video_frames, frame_video) : sums, loss_weight, go);
   const int frame = si.start_frame + row;
   const GridDims grid = make_grid(H, W);
   const Cam ks = make_cam(load_k4(k4, frame));
@@ -2062,7 +2386,7 @@ k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const f
               const unsigned char* __restrict__ flag, const float* __restrict__ dq,
               const double* __restrict__ sums, float loss_weight, const float* __restrict__ go,
               float* __restrict__ g_depth, int H, int W, TrackShard sh) {
-  track_apply_body<false>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh, 0);
+  track_apply_body<0>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh, 0);
 }
 
 __global__ void __launch_bounds__(kThreads)
@@ -2070,18 +2394,30 @@ k_track_apply_videos(const float* __restrict__ k4, const int* __restrict__ seg, 
                      const unsigned char* __restrict__ flag, const float* __restrict__ dq,
                      const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
                      TrackShard sh, int video_frames) {
-  track_apply_body<true>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, video_frames);
+  track_apply_body<1>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, video_frames);
 }
 
-// VIDEOS: frames f of B * video_frames, scaled by the sums of video f / video_frames.
-template <bool VIDEOS>
+__global__ void __launch_bounds__(kThreads)
+k_track_apply_ragged(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
+                     const unsigned char* __restrict__ flag, const float* __restrict__ dq,
+                     const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
+                     TrackShard sh, const int* __restrict__ frame_video) {
+  track_apply_body<kRaggedVideos>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, 0,
+                                  frame_video);
+}
+
+// VIDEOS: frames f of B * video_frames, scaled by the sums of video f / video_frames (kRaggedVideos:
+// of video frame_video[f]).
+template <int VIDEOS>
 __device__ __forceinline__ void track_finalize_body(const double* __restrict__ trackacc, const double* __restrict__ sums,
                                                     float loss_weight, const float* __restrict__ go,
                                                     const float* __restrict__ ext, float* __restrict__ g_ext,
-                                                    float* __restrict__ g_k4, int F, int video_frames) {
+                                                    float* __restrict__ g_k4, int F, int video_frames,
+                                                    const int* frame_video = nullptr) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
-  const double sc = track_scale(VIDEOS ? sums + 2 * (f / video_frames) : sums, loss_weight, go);
+  const double sc = track_scale(VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(f, video_frames, frame_video) : sums,
+                                loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
   for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
   const float* P = ext + (size_t)f * 16;
@@ -2101,13 +2437,19 @@ __global__ void k_track_finalize(const double* __restrict__ trackacc, const doub
                                  float loss_weight, const float* __restrict__ go,
                                  const float* __restrict__ ext, float* __restrict__ g_ext,
                                  float* __restrict__ g_k4, int F) {
-  track_finalize_body<false>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F, 0);
+  track_finalize_body<0>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F, 0);
 }
 
 __global__ void k_track_finalize_videos(const double* __restrict__ trackacc, const double* __restrict__ sums,
                                         float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
                                         float* __restrict__ g_k4, int BF, int video_frames) {
-  track_finalize_body<true>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, BF, video_frames);
+  track_finalize_body<1>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, BF, video_frames);
+}
+
+__global__ void k_track_finalize_ragged(const double* __restrict__ trackacc, const double* __restrict__ sums,
+                                        float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
+                                        float* __restrict__ g_k4, int T, const int* __restrict__ frame_video) {
+  track_finalize_body<kRaggedVideos>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, T, 0, frame_video);
 }
 
 // ================================================================== focal-length sweep
@@ -2194,13 +2536,14 @@ __global__ void k_sweep_aggregate(const PairAdjoint* __restrict__ adj, const flo
   }
 }
 
-template <bool BWD>
-__global__ void __launch_bounds__(kThreads)
-k_sweep(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
-        const float* __restrict__ bflow, const float* __restrict__ weights, float wsens,
-        const int64_t* __restrict__ indices, int num_indices, const float* __restrict__ g_err,
-        double* __restrict__ acc_out, float* __restrict__ g_depth, float* __restrict__ g_weights,
-        PairLayout lay, int H, int W) {
+#define FM_SWEEP_PARAMS                                                                                      \
+  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,               \
+      const float* __restrict__ bflow, const float* __restrict__ weights, float wsens,                       \
+      const int64_t* __restrict__ indices, int num_indices, const float* __restrict__ g_err,                 \
+      double* __restrict__ acc_out, float* __restrict__ g_depth, float* __restrict__ g_weights
+#define FM_SWEEP_ARGS depth, k4, rt, bflow, weights, wsens, indices, num_indices, g_err, acc_out, g_depth, g_weights
+template <bool BWD, class Lay>
+__device__ __forceinline__ void sweep_body(FM_SWEEP_PARAMS, const Lay& lay, int H, int W) {
   __shared__ double smem[12 * (kThreads / 32)];
   const int item = blockIdx.y;
   const int N = H * W;
@@ -2260,6 +2603,17 @@ k_sweep(const float* __restrict__ depth, const float* __restrict__ k4, const flo
   if (!BWD) block_accumulate<1>(acc, acc_out + (size_t)item * kSweepAcc, smem);
   else block_accumulate<12>(acc, acc_out + (size_t)item * kSweepAcc + 1, smem);
 }
+
+template <bool BWD>
+__global__ void __launch_bounds__(kThreads) k_sweep(FM_SWEEP_PARAMS, PairLayout lay, int H, int W) {
+  sweep_body<BWD>(FM_SWEEP_ARGS, lay, H, W);
+}
+template <bool BWD>
+__global__ void __launch_bounds__(kThreads) k_sweep_ragged(FM_SWEEP_PARAMS, RaggedSweep lay, int H, int W) {
+  sweep_body<BWD>(FM_SWEEP_ARGS, lay, H, W);
+}
+#undef FM_SWEEP_PARAMS
+#undef FM_SWEEP_ARGS
 
 __global__ void k_sweep_out(const double* __restrict__ acc, float* __restrict__ out, int items, int off,
                             int count) {
@@ -2573,15 +2927,19 @@ k_trajectory_ate(const float* __restrict__ gt, const float* __restrict__ pred, i
 // (capacity, B, 5) ring, with what k_trajectory_ate writes for one video (the same float64 sums in the
 // same order).  gt (B, F, 3); a video whose first position is NaN has no ground truth (ATE NaN);
 // gt_fxfy (B, 2) frame means of the ground-truth intrinsics (NaN: no ground truth).
-__global__ void __launch_bounds__(kAteThreads)
-k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, int F, MetricsRow row,
-                 const float* __restrict__ gt_fxfy) {
+// RAGGED (k_metrics_ragged): video b's frames start at frame f0 = frame_offset[b] and number its own F.
+template <bool RAGGED>
+__device__ __forceinline__ void metrics_videos_body(const float* __restrict__ gt, const float* __restrict__ pred,
+                                                    int F, MetricsRow row, const float* __restrict__ gt_fxfy,
+                                                    const Videos& vids) {
   __shared__ double s_red[kAteThreads / 32 * 9];
   const size_t b = blockIdx.x;
   float* r = row.log + ((size_t)((row.clock->step - 1u) % (unsigned)row.capacity) * gridDim.x + b) * 5;
-  const bool has_gt = gt && !isnan(gt[b * F * 3]);
+  const size_t f0 = RAGGED ? vids.first(b) : 0;
+  if (RAGGED) F = vids.frames(b);
+  const bool has_gt = gt && !isnan(gt[RAGGED ? f0 * 3 : b * F * 3]);
   if (threadIdx.x == 0) {
-    const float* k4 = row.k4 + b * F * 4;
+    const float* k4 = row.k4 + (RAGGED ? f0 * 4 : b * F * 4);
     double fx = 0.0, fy = 0.0;
     for (int f = 0; f < F; ++f) { fx += (double)k4[f * 4 + 0]; fy += (double)k4[f * 4 + 1]; }
     r[0] = row.loss[b];
@@ -2592,8 +2950,8 @@ k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, i
   }
   if (!has_gt) return;
   AtePoints x;
-  x.gt = gt + b * F * 3;
-  x.pred = pred + b * F * 16;
+  x.gt = gt + (RAGGED ? f0 * 3 : b * F * 3);
+  x.pred = pred + (RAGGED ? f0 * 16 : b * F * 16);
   x.gt_stride = 3;
   x.pred_stride = 16;
   x.pred_cstride = 4;
@@ -2602,6 +2960,17 @@ k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, i
   double v;
   trajectory_ate(x, threadIdx.x, kAteThreads, red, v, nullptr, nullptr);
   if (threadIdx.x == 0) r[4] = (float)v;
+}
+
+__global__ void __launch_bounds__(kAteThreads)
+k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, int F, MetricsRow row,
+                 const float* __restrict__ gt_fxfy) {
+  metrics_videos_body<false>(gt, pred, F, row, gt_fxfy, Videos{});
+}
+__global__ void __launch_bounds__(kAteThreads)
+k_metrics_ragged(const float* __restrict__ gt, const float* __restrict__ pred, MetricsRow row,
+                 const float* __restrict__ gt_fxfy, Videos v) {
+  metrics_videos_body<true>(gt, pred, 0, row, gt_fxfy, v);
 }
 
 // ================================================================== fused overfit step helpers
@@ -2617,15 +2986,25 @@ __global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restri
 }
 
 // k_k4_from_focal for B videos with one focal length each: frame t of the (B*F, 4) rows reads focal[t / F].
-__global__ void k_k4_from_focals(const float* __restrict__ focal, float* __restrict__ k4, int BF, int F, int H,
-                                 int W) {
+// (k_k4_from_focals_ragged: frame t reads the focal length of its video frame_video[t].)
+template <bool RAGGED>
+__device__ __forceinline__ void k4_from_focals_body(const float* __restrict__ focal, float* __restrict__ k4, int BF,
+                                                    int F, int H, int W, const Videos& v) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= BF) return;
-  const float scaled = focal[t / F] * sqrtf((float)H * (float)W);
+  const float scaled = focal[RAGGED ? v.of_frame(t) : t / F] * sqrtf((float)H * (float)W);
   k4[t * 4 + 0] = scaled / (float)W;
   k4[t * 4 + 1] = scaled / (float)H;
   k4[t * 4 + 2] = 0.5f;
   k4[t * 4 + 3] = 0.5f;
+}
+__global__ void k_k4_from_focals(const float* __restrict__ focal, float* __restrict__ k4, int BF, int F, int H,
+                                 int W) {
+  k4_from_focals_body<false>(focal, k4, BF, F, H, W, Videos{});
+}
+__global__ void k_k4_from_focals_ragged(const float* __restrict__ focal, float* __restrict__ k4, int T, int H, int W,
+                                        Videos v) {
+  k4_from_focals_body<true>(focal, k4, T, 0, H, W, v);
 }
 
 // d loss / d focal from the per-frame k4 gradients (flow-loss part + Procrustes part).
@@ -2666,6 +3045,13 @@ __global__ void k_focal_grad_videos(const double* __restrict__ k4acc, const doub
   const size_t f0 = (size_t)blockIdx.x * F;
   focal_grad_block(k4acc + f0 * 4, flowacc + f0 * kFlowAcc, extra_g_k4 ? extra_g_k4 + f0 * 4 : nullptr,
                    g_focal + blockIdx.x, 1, F, H, W, nullptr);
+}
+__global__ void k_focal_grad_ragged(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                                    const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int H, int W,
+                                    Videos v) {
+  const size_t f0 = v.first(blockIdx.x);
+  focal_grad_block(k4acc + f0 * 4, flowacc + f0 * kFlowAcc, extra_g_k4 ? extra_g_k4 + f0 * 4 : nullptr,
+                   g_focal + blockIdx.x, 1, v.frames(blockIdx.x), H, W, nullptr);
 }
 
 // ---------------------------------------------------------------- launch geometry
@@ -2773,6 +3159,34 @@ int launch_flow(const float* depth, const float* k4, const float* rt, const floa
   FM_CHECK_LAUNCH("k_flow_lean");
   k_flow_lean_convert<<<(BF + 63) / 64, 64, 0, s>>>(flowacc, rt, k4, focal ? 1 : 0, B, F, H, W);
   FM_CHECK_LAUNCH("k_flow_lean_convert");
+  return 0;
+}
+
+// The host's view of an fm_video_layout: the device tables and the counts.
+struct Ragged {
+  Videos v;
+  int B, T;  // videos, frames in all (T - B pairs)
+};
+
+// launch_flow with per-video normalisers for videos of different lengths (focal: one shared focal length
+// per video, else constant intrinsics).
+int launch_flow_ragged(const float* depth, const float* k4, const float* rt, const float* ff, const float* fb,
+                       const float* mf, const float* mb, const double* mask_sum, int mapping, float delta,
+                       float loss_weight, bool focal, float* g_depth, double* flowacc, const Ragged& r, int H, int W,
+                       cudaStream_t s) {
+  const int T = r.T;
+  const int vec = (W % 4 == 0) ? 4 : 1;
+  const int pg = persistent_grid(2, (long long)T * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
+  if (vec == 4) {
+    if (focal) k_flow_lean_ragged<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
+    else k_flow_lean_ragged<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
+  } else {
+    if (focal) k_flow_lean_ragged<1, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
+    else k_flow_lean_ragged<1, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
+  }
+  FM_CHECK_LAUNCH("k_flow_lean_ragged");
+  k_flow_lean_convert_ragged<<<(T + 63) / 64, 64, 0, s>>>(flowacc, rt, k4, focal ? 1 : 0, T, H, W, r.v);
+  FM_CHECK_LAUNCH("k_flow_lean_convert_ragged");
   return 0;
 }
 }  // namespace
@@ -2886,7 +3300,7 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 103; }
+int fm_version(void) { return 104; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -3071,6 +3485,84 @@ static int procrustes_bwd_impl(const float* depth, const float* k4, const float*
   return 0;
 }
 
+// procrustes_fwd_impl for videos of different lengths (no splat plan, no explicit PairLayout).
+static int procrustes_fwd_ragged(const float* depth, const float* k4, const float* backward_flow, const float* weights,
+                                 float wsens, const int64_t* indices, int num_indices, float* rt, void* ws,
+                                 const Ragged& r, int H, int W, cudaStream_t s, const float* moments_k4, bool solve) {
+  if (!depth || !k4 || !backward_flow || (!rt && solve) || !ws) return fail_msg("fm_procrustes_fwd: bad arguments");
+  if (indices && num_indices < 1) return fail_msg("fm_procrustes_fwd: empty index set");
+  const int BP = r.T - r.B;
+  Workspace w = carve_rows(ws, r.B, r.T, BP);
+  const RaggedPairs lay{r.v};
+  if (moments_k4) {  // fm_procrustes_moments_videos already ran with those intrinsics
+    if (indices) return fail_msg("fm_procrustes_fwd: precomputed moments serve the dense path");
+    if (!solve) return 0;
+    k_solve_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, moments_k4, k4);
+    FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve_ragged");
+    return 0;
+  }
+  cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
+  k_pair_shift_ragged<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift_ragged");
+  if (indices) {
+    dim3 grid(blocks_for_points(num_indices), BP);
+    k_moments_ragged<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, w.zshift, wsens, lay, H, W);
+  } else if (patch_shape_ok(H, W)) {
+    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
+    const int pg = persistent_grid(3, items);
+    k_moments_dense_ragged<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
+  } else if (W % 4 == 0) {
+    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
+    const int pg = persistent_grid(3, items);
+    k_moments_dense_ragged<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
+  } else {
+    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
+    const int pg = persistent_grid(3, items);
+    k_moments_dense_ragged<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items / 4, pg, true));
+  }
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_moments_ragged");
+  if (!solve) return 0;
+  k_solve_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, nullptr, nullptr);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve_ragged");
+  return 0;
+}
+
+// procrustes_bwd_impl of a whole step (flow loss included, unscaled) for videos of different lengths.
+static int procrustes_bwd_ragged(const float* depth, const float* k4, const float* backward_flow, const float* weights,
+                                 float wsens, const int64_t* indices, int num_indices, const float* g_rt,
+                                 float* g_depth, float* g_weights, float* g_k4, void* ws, const Ragged& r, int H, int W,
+                                 cudaStream_t s, const AdamFuse* adam) {
+  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws) return fail_msg("fm_procrustes_bwd: bad arguments");
+  const int BP = r.T - r.B;
+  Workspace w = carve_rows(ws, r.B, r.T, BP);
+  const RaggedPairs lay{r.v};
+  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)r.T * 4 * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
+  AdamFuse af;
+  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
+  float* weights_rw = const_cast<float*>(weights);
+  k_adjoint_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 1, nullptr, w.adj, BP, r.v);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint_ragged");
+  if (indices) {
+    dim3 grid(blocks_for_points(num_indices), BP);
+    k_distribute_ragged<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
+  } else if (W % 4 == 0) {
+    const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
+    const int pg = persistent_grid(FM_WIN_CTAS, items);
+    const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);
+    k_distribute_window_ragged<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
+  } else {
+    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
+    const int pg = persistent_grid(3, items);
+    k_distribute_dense_ragged<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
+  }
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute_ragged");
+  k_k4_finalize_ragged<<<(r.T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, 1, nullptr, g_k4, r.T, r.v);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize_ragged");
+  return 0;
+}
+
 int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward_flow,
                       const float* weights, const int64_t* indices, int num_indices,
                       const float* g_rt, int include_flow_loss, const float* flow_scale,
@@ -3189,6 +3681,31 @@ int fm_flow_loss_fwd_bwd(const float* depth, const float* k4, const float* rt,
   const int n = BF > BP ? BF : BP;
   k_flow_finalize<<<(n + 127) / 128, 128, 0, s>>>(w.flowacc, rt, loss, g_rt, g_k4, B, F);
   FM_CHECK_LAUNCH("fm_flow_loss_fwd_bwd: k_flow_finalize");
+  return 0;
+}
+
+// fm_video_layout -> Ragged; nonzero when the layout is unusable (B >= 1 videos of >= 2 frames each, the
+// per-video tables are the caller's: only their presence and the counts are checked here).
+static int ragged_of(const fm_video_layout* l, Ragged* r) {
+  if (!l || l->B < 1 || l->T < 2 * l->B || !l->frame_offset || !l->frame_video || !l->pair_video) return 1;
+  r->v.frame_offset = l->frame_offset;
+  r->v.frame_video = l->frame_video;
+  r->v.pair_video = l->pair_video;
+  r->B = l->B;
+  r->T = l->T;
+  return 0;
+}
+
+static int pose_chain_ragged(const float* rt, float* extrinsics, const Ragged& r, void* stream) {
+  k_pose_chain_ragged<<<r.B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, r.v);
+  FM_CHECK_LAUNCH("fm_pose_chain_videos");
+  return 0;
+}
+
+static int pose_chain_bwd_ragged(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
+                                 const Ragged& r, void* stream) {
+  k_pose_chain_bwd_ragged<<<r.B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, g_extrinsics, g_rt, r.v);
+  FM_CHECK_LAUNCH("fm_pose_chain_bwd_videos");
   return 0;
 }
 
@@ -3317,13 +3834,15 @@ size_t fm_track_reduce_bytes(int F) {
 
 // vsums != NULL (the batched fused step): the frames are B videos of F / B frames, and each video's loss
 // sum and valid count go to vsums[2 b], vsums[2 b + 1] (zeroed here) instead of the head of ws; `loss`
+// then receives B values.  frame_video != NULL as well: videos of different lengths, the video of a
+// segment's start frame from that table.
 // then receives B values.
 static int track_fwd_impl(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                           int num_segments, int max_rows, int max_points, const float* track_xy,
                           const unsigned char* track_vis, long long total_samples, int mapping, float delta,
                           float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
                           int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream,
-                          double* vsums = nullptr, int B = 1) {
+                          double* vsums = nullptr, int B = 1, const int* frame_video = nullptr) {
   if (!depth || !k4 || !extrinsics || !segments || !track_xy || !track_vis || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_fwd: bad arguments");
@@ -3354,13 +3873,22 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
     if (ea != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ea);
   }
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
-  if (vsums) {  // one focal length per video: shared intrinsics
+  if (vsums && frame_video) {
+    static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
+    k_track_src_ragged<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
+                                                               mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
+                                                               (int)items, max_rows, list_cap, H, W, sh, frame_video);
+    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_ragged");
+  } else if (vsums) {  // one focal length per video: shared intrinsics
     static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_videos<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
     k_track_src_videos<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
                                                                mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
                                                                (int)items, max_rows, list_cap, H, W, sh, F / B);
     FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_videos");
+  }
+  if (vsums) {
     if (loss) {
       k_track_video_loss<<<1, 32 * ((B + 31) / 32), 0, s>>>(vsums, loss_weight, loss, B);
       FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_video_loss");
@@ -3417,7 +3945,7 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
                           float loss_weight, const float* grad_out, float* g_depth, float* g_extrinsics,
                           float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
                           int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream,
-                          const double* vsums = nullptr, int B = 1) {
+                          const double* vsums = nullptr, int B = 1, const int* frame_video = nullptr) {
   if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !g_k4 || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_bwd: bad arguments");
@@ -3426,6 +3954,15 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
   TrackWs w = carve_track(ws, F, total_samples);
   dim3 grid((max_points + kThreads - 1) / kThreads, max_rows, num_segments);
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
+  if (vsums && frame_video) {
+    k_track_apply_ragged<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
+                                                             g_depth, H, W, sh, frame_video);
+    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply_ragged");
+    k_track_finalize_ragged<<<(F + 63) / 64, 64, 0, s>>>(w.acc, vsums, loss_weight, extrinsics, g_extrinsics, g_k4,
+                                                         F, frame_video);
+    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize_ragged");
+    return 0;
+  }
   if (vsums) {  // per-video scales (track_fwd_impl); grad_out is 1 in the batched step
     k_track_apply_videos<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
                                                              g_depth, H, W, sh, F / B);
@@ -3551,10 +4088,11 @@ PairLayout sweep_layout(int F, int H, int W, int cand) {
 }
 }  // namespace
 
-int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_sensitivity,
-                         const float* backward_flow, const int64_t* indices, int num_indices,
-                         const float* cand_k4, int num_candidates, float* err, float* rt, void* ws, int B,
-                         int F, int H, int W, void* stream) {
+// vids != NULL: videos of different lengths (each video's pair 0 through RaggedSweep; F is unused)
+static int sweep_fwd_impl(const float* depth, const float* weights, float weight_sensitivity,
+                          const float* backward_flow, const int64_t* indices, int num_indices,
+                          const float* cand_k4, int num_candidates, float* err, float* rt, void* ws, int B,
+                          int F, int H, int W, void* stream, const Videos* vids = nullptr) {
   if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 ||
       !err || !rt || !ws || bad_dims(B, F, H, W))
     return fail_msg("fm_softmin_sweep_fwd: bad arguments");
@@ -3571,12 +4109,18 @@ int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_
   k_sweep_base_k4<<<(B * 8 + 127) / 128, 128, 0, s>>>(cand_k4, base_k4, B, num_candidates);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_base_k4");
   float* base_zshift = w.zshift + items;  // one conditioning shift per batch element, for all candidates
-  k_pair_shift<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, lay1, H, W);
+  if (vids) k_pair_shift_ragged<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, RaggedSweep{*vids, 1}, H, W);
+  else k_pair_shift<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, lay1, H, W);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_pair_shift");
   {  // ONE moment pass (candidate 0); every candidate's moments are a rescaling of it
     dim3 grid(blocks_for_points(num_indices), B);
-    k_moments<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
-                                          base_moments, base_zshift, weight_sensitivity, lay1, H, W);
+    if (vids)
+      k_moments_ragged<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
+                                                   base_moments, base_zshift, weight_sensitivity, RaggedSweep{*vids, 1},
+                                                   H, W);
+    else
+      k_moments<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
+                                            base_moments, base_zshift, weight_sensitivity, lay1, H, W);
     FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_moments");
   }
   k_sweep_scale_solve<<<(items + 63) / 64, 64, 0, s>>>(base_moments, base_zshift, cand_k4, rt, w.state, B,
@@ -3585,20 +4129,33 @@ int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_
   e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
   dim3 grid(blocks_for_points(num_indices), items);
-  k_sweep<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                          indices, num_indices, nullptr, w.flowacc, nullptr, nullptr, lay,
-                                          H, W);
+  if (vids)
+    k_sweep_ragged<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
+                                                   indices, num_indices, nullptr, w.flowacc, nullptr, nullptr,
+                                                   RaggedSweep{*vids, num_candidates}, H, W);
+  else
+    k_sweep<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
+                                            indices, num_indices, nullptr, w.flowacc, nullptr, nullptr, lay,
+                                            H, W);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep");
   k_sweep_out<<<(items + 127) / 128, 128, 0, s>>>(w.flowacc, err, items, 0, 1);
   FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_out");
   return 0;
 }
 
-int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_sensitivity,
+int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_sensitivity,
                          const float* backward_flow, const int64_t* indices, int num_indices,
-                         const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
-                         float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
-                         void* stream) {
+                         const float* cand_k4, int num_candidates, float* err, float* rt, void* ws, int B,
+                         int F, int H, int W, void* stream) {
+  return sweep_fwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
+                        num_candidates, err, rt, ws, B, F, H, W, stream);
+}
+
+static int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensitivity,
+                          const float* backward_flow, const int64_t* indices, int num_indices,
+                          const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
+                          float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
+                          void* stream, const Videos* vids = nullptr) {
   if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 || !rt ||
       !g_err || !g_depth || !ws || bad_dims(B, F, H, W))
     return fail_msg("fm_softmin_sweep_bwd: bad arguments");
@@ -3615,9 +4172,14 @@ int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_
   e = cudaMemsetAsync(w.k4acc, 0, (size_t)(items + B) * 2 * 4 * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_softmin_sweep_bwd: memset", e);
   dim3 grid(blocks_for_points(num_indices), items);
-  k_sweep<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                         indices, num_indices, g_err, w.flowacc, g_depth, g_weights, lay, H,
-                                         W);
+  if (vids)
+    k_sweep_ragged<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
+                                                  indices, num_indices, g_err, w.flowacc, g_depth, g_weights,
+                                                  RaggedSweep{*vids, num_candidates}, H, W);
+  else
+    k_sweep<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
+                                           indices, num_indices, g_err, w.flowacc, g_depth, g_weights, lay, H,
+                                           W);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep");
   k_sweep_out<<<(items * 12 + 127) / 128, 128, 0, s>>>(w.flowacc, g_rt, items, 1, 12);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_out");
@@ -3629,11 +4191,25 @@ int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_
   AdamFuse af;
   memset(&af, 0, sizeof(af));
   dim3 grid1(blocks_for_points(num_indices), B);
-  k_distribute<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights), indices,
-                                            num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
-                                            weight_sensitivity, lay1, af, H, W);
+  if (vids)
+    k_distribute_ragged<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights),
+                                                     indices, num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
+                                                     weight_sensitivity, RaggedSweep{*vids, 1}, af, H, W);
+  else
+    k_distribute<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights), indices,
+                                              num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
+                                              weight_sensitivity, lay1, af, H, W);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_distribute");
   return 0;
+}
+
+int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_sensitivity,
+                         const float* backward_flow, const int64_t* indices, int num_indices,
+                         const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
+                         float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
+                         void* stream) {
+  return sweep_bwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
+                        num_candidates, rt, g_err, g_depth, g_weights, ws, B, F, H, W, stream);
 }
 
 int fm_softmin_focal(const float* err, const float* cand_focal, int num_candidates, int B, float* softmin,
@@ -3679,35 +4255,45 @@ static SideLane* side_lane(int which = 0) {
   return l.state == 1 ? &l : nullptr;
 }
 
-int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
+// rag != NULL (fm_overfit_step_videos): videos of different lengths packed along the frame axis; a->B and
+// a->F are then ignored, and B, T come from the layout.
+static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, void* stream) {
   if (!a || !a->depth || !a->fflow || !a->bflow || !a->fmask || !a->bmask || !a->mask_sum ||
-      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 || bad_dims(a->B > 1 ? a->B : 1, a->F, a->H, a->W))
+      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 ||
+      (rag ? bad_dims(rag->B, 2, a->H, a->W) : bad_dims(a->B > 1 ? a->B : 1, a->F, a->H, a->W)))
     return fail_msg("fm_overfit_step: bad arguments");
   // B independent videos of one shape: every per-video scalar is an array of B values
-  const int B = a->B > 1 ? a->B : 1;
-  if (B > 1 && (a->phase != FM_STEP_ALL || a->splat_plan))
+  const int B = rag ? rag->B : a->B > 1 ? a->B : 1;
+  const bool videos = B > 1 || rag;  // per-video normalisers, losses and focal lengths
+  if (videos && (a->phase != FM_STEP_ALL || a->splat_plan))
     return fail_msg("fm_overfit_step: B > 1 serves whole steps without a splat plan");
-  if (B > 1 && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
+  if (videos && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
     return fail_msg("fm_overfit_step: B > 1 does not fuse the logit update of a deferred step (pass step = 0)");
-  if (B > 1 && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step: B > 1 metrics need gt_fxfy");
+  if (videos && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step: B > 1 metrics need gt_fxfy");
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
   if (a->metrics_log && (a->phase != FM_STEP_ALL || !a->clock || !a->extrinsics || a->metrics_capacity < 1))
     return fail_msg("fm_overfit_step: metrics_log needs FM_STEP_ALL, a clock, extrinsics and metrics_capacity >= 1");
   cudaStream_t s = (cudaStream_t)stream;
-  const int F = a->F, H = a->H, W = a->W, BP = F - 1;
+  const int F = rag ? 0 : a->F, H = a->H, W = a->W, BP = F - 1;
   const size_t N = (size_t)H * W;
-  Workspace w = carve(a->ws, B, F);
+  // frames and pairs of all videos
+  const size_t TF = rag ? (size_t)rag->T : (size_t)B * F, TP = rag ? (size_t)(rag->T - B) : (size_t)B * BP;
+  const int* frame_video = rag ? rag->v.frame_video : nullptr;
+  Workspace w = rag ? carve_rows(a->ws, B, TF, TP) : carve(a->ws, B, F);
   int rc;
   cudaError_t e;
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
   // the splat plan of this video's backward flows serves the dense path (all-pixel Procrustes)
-  void* plan = (a->splat_plan && !a->indices && tiled_shape_ok(F, H, W)) ? a->splat_plan : nullptr;
+  void* plan = (!rag && a->splat_plan && !a->indices && tiled_shape_ok(F, H, W)) ? a->splat_plan : nullptr;
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
-    if (a->focal && B == 1) {
+    if (a->focal && rag) {
+      k_k4_from_focals_ragged<<<(rag->T + 63) / 64, 64, 0, s>>>(a->focal, k4, rag->T, H, W, rag->v);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals_ragged");
+    } else if (a->focal && B == 1) {
       k_k4_from_focal<<<(F + 63) / 64, 64, 0, s>>>(a->focal, k4, F, H, W);
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
     } else if (a->focal) {
@@ -3715,7 +4301,12 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
-    if ((rc = procrustes_fwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
+    if (rag) {
+      if ((rc = procrustes_fwd_ragged(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                                      a->num_indices, a->rt, a->ws, *rag, H, W, s,
+                                      a->indices ? nullptr : a->moments_k4, true)))
+        return rc;
+    } else if ((rc = procrustes_fwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
                                   a->indices, a->num_indices, a->rt, a->ws, B, F, H, W, stream, nullptr, plan,
                                   (a->indices || plan) ? nullptr : a->moments_k4)))
       return rc;
@@ -3728,13 +4319,20 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       if ((e = cudaStreamWaitEvent(fwd_lane->stream, fwd_lane->fork, 0)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
     }
     // LossFlow forward + direct gradients (loss_flow.py:31-70)
-    e = cudaMemsetAsync(w.flowacc, 0, (size_t)B * F * kFlowAcc * sizeof(double), s);
+    e = cudaMemsetAsync(w.flowacc, 0, TF * kFlowAcc * sizeof(double), s);
     if (e != cudaSuccess) return fail("fm_overfit_step: memset", e);
-    if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum,
+    if (rag) {
+      if ((rc = launch_flow_ragged(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum, a->mapping,
+                                   a->delta, a->flow_weight, a->focal != nullptr, a->g_depth, w.flowacc, *rag, H, W, s)))
+        return rc;
+    } else if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum,
                           a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, B, F,
                           H, W, s, /*per_video=*/B > 1)))
       return rc;
-    if (B == 1) {
+    if (rag) {
+      k_flow_video_loss_ragged<<<B, 128, 0, s>>>(w.flowacc, a->loss, rag->v);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss_ragged");
+    } else if (B == 1) {
       k_flow_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.flowacc, a->rt, a->loss, nullptr, nullptr, 1, F);
       FM_CHECK_LAUNCH("fm_overfit_step: k_flow_finalize");
     } else {
@@ -3746,13 +4344,15 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     if (a->tracks) {
       const fm_packed_tracks* t = a->tracks;
       void* ts = fwd_lane ? (void*)fwd_lane->stream : stream;
-      if ((rc = fm_pose_chain(a->rt, a->extrinsics, B, F, ts))) return rc;
+      if ((rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ts) : fm_pose_chain(a->rt, a->extrinsics, B, F, ts)))
+        return rc;
       // one focal length (or constant intrinsics) for all frames: only the summed K gradient is used.
-      // B > 1: the segments of video b start at frames b F + s, and its sums go to w.track_sums[b]
+      // B > 1: the segments of video b start at frames b F + s (ragged: frame_offset[b] + s), and its sums
+      // go to w.track_sums[b]
       if ((rc = track_fwd_impl(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
                                t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
-                               a->track_weight, a->track_loss, a->track_ws, B * F, H, W, 0, 0, B * F, 1, ts,
-                               B > 1 ? w.track_sums : nullptr, B)))
+                               a->track_weight, a->track_loss, a->track_ws, (int)TF, H, W, 0, 0, (int)TF, 1, ts,
+                               videos ? w.track_sums : nullptr, B, frame_video)))
         return rc;
       if (fwd_lane) {
         if ((e = cudaEventRecord(fwd_lane->join, fwd_lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -3773,7 +4373,9 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       ms = mlane->stream;
     }
     // the camera centres: the tracking loss chained the poses already, a flow-only step chains them here
-    if (!a->tracks && (rc = fm_pose_chain(a->rt, a->extrinsics, B, F, ms))) return rc;
+    if (!a->tracks &&
+        (rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ms) : fm_pose_chain(a->rt, a->extrinsics, B, F, ms)))
+      return rc;
     MetricsRow row;
     row.log = a->metrics_log;
     row.capacity = a->metrics_capacity;
@@ -3783,7 +4385,10 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     row.k4 = k4;
     row.gt_fx = a->gt_fx;
     row.gt_fy = a->gt_fy;
-    if (B == 1) {
+    if (rag) {
+      k_metrics_ragged<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, row, a->gt_fxfy, rag->v);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_ragged");
+    } else if (B == 1) {
       k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr,
                                                   nullptr, nullptr, row);
       FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
@@ -3799,7 +4404,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   const float* tscale = a->phase == FM_STEP_BACKWARD ? a->track_grad_scale : nullptr;
   if (fscale) {  // the direct flow-loss gradient in g_depth was computed for scale 1; scale it before
     // the tracking loss adds its own (differently scaled) part
-    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, (size_t)B * F * N);
+    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, TF * N);
     FM_CHECK_LAUNCH("fm_overfit_step: k_scale_inplace");
   }
   const float* g_rt = a->phase == FM_STEP_BACKWARD ? a->g_rt : nullptr;           // the caller's
@@ -3818,17 +4423,19 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     }
     if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
                              t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
-                             a->track_ws, B * F, H, W, 0, 0, B * F, s, apply_stream, B > 1 ? w.track_sums : nullptr,
-                             B)))
+                             a->track_ws, (int)TF, H, W, 0, 0, (int)TF, s, apply_stream,
+                             videos ? w.track_sums : nullptr, B, frame_video)))
       return rc;
     if (lane && (e = cudaEventRecord(lane->join, lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
-    if ((rc = fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, F, stream))) return rc;
+    if ((rc = rag ? pose_chain_bwd_ragged(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, *rag, stream)
+                  : fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, F, stream)))
+      return rc;
     g_rt = a->g_rt;
     track_g_k4 = a->track_g_k4;
   }
   // backward through Procrustes: adjoint constants, per-point distribution
   if (a->indices && a->g_weights) {  // subsampled Procrustes: sparse weight gradient, dense buffer
-    e = cudaMemsetAsync(a->g_weights, 0, (size_t)B * BP * N * sizeof(float), s);
+    e = cudaMemsetAsync(a->g_weights, 0, TP * N * sizeof(float), s);
     if (e != cudaSuccess) return fail("fm_overfit_step: memset g_weights", e);
   }
   AdamFuse af;
@@ -3836,7 +4443,7 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   const bool defer = a->defer_adam != 0;  // softmin stage: the sweep's backward still adds gradients
   // B > 1 with defer_adam = 1 would have to defer pair 0 of EVERY video (first_pair counts pairs of the
   // whole batch): that step leaves the logits to the caller instead
-  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(B > 1 && a->defer_adam == 1);
+  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(videos && a->defer_adam == 1);
   const StepClock* clock = (const StepClock*)a->clock;
   if (fuse_w) {  // the weight gradient is final inside k_distribute: update the logits there
     af.consts = clock ? &clock->step_size : nullptr;
@@ -3847,7 +4454,12 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
     af.step_size = (float)(a->lr / (1.0 - pow(a->beta1, (double)a->step)));
     af.bc2_sqrt = (float)sqrt(1.0 - pow(a->beta2, (double)a->step));
   }
-  if ((rc = procrustes_bwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
+  if (rag) {
+    if ((rc = procrustes_bwd_ragged(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                                    a->num_indices, g_rt, a->g_depth, a->g_weights, a->g_k4, a->ws, *rag, H, W, s,
+                                    fuse_w ? &af : nullptr)))
+      return rc;
+  } else if ((rc = procrustes_bwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
                                 a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
                                 a->g_k4, a->ws, B, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
                                 a->splat_overflow_max, /*depth_prescaled=*/fscale != nullptr)))
@@ -3859,13 +4471,16 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
       return clock ? fm_adam_step_clock(p, g, m, v, n, clock, focal_clock, a->beta1, a->beta2, a->eps, stream)
                    : fm_adam_step(p, g, m, v, n, a->lr, a->beta1, a->beta2, a->eps, step, stream);
     };
-    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, (size_t)B * F * N, a->step, 0))) return rc;
+    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, TF * N, a->step, 0))) return rc;
     if (a->weight_logits && !fuse_w &&
-        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, (size_t)B * BP * N, a->step, 0)))
+        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, TP * N, a->step, 0)))
       return rc;
   }
   if (a->focal) {  // d loss / d focal, then (update steps) its Adam
-    if (B == 1) {
+    if (rag) {
+      k_focal_grad_ragged<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, H, W, rag->v);
+      FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad_ragged");
+    } else if (B == 1) {
       k_focal_grad<<<1, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, 1, F, H, W, fscale);
       FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
     } else {  // whole steps only: no fscale
@@ -3884,6 +4499,86 @@ int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
   if (defer && a->step > 0 && a->weight_logits && !fuse_w) return fail_msg("fm_overfit_step: defer_adam needs the fused weight update");
   if (mlane && (e = cudaStreamWaitEvent(s, mlane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   return 0;
+}
+
+int fm_overfit_step(const fm_overfit_step_args* a, void* stream) { return overfit_step_impl(a, nullptr, stream); }
+
+int fm_overfit_step_videos(const fm_overfit_step_args* a, const fm_video_layout* layout, void* stream) {
+  Ragged r;
+  if (ragged_of(layout, &r)) return fail_msg("fm_overfit_step_videos: bad video layout");
+  return overfit_step_impl(a, &r, stream);
+}
+
+size_t fm_workspace_bytes_videos(int B, int T) {
+  if (B < 1 || T < 2 * B) return 0;
+  return carve_rows(nullptr, B, (size_t)T, (size_t)(T - B)).bytes;
+}
+
+int fm_procrustes_moments_videos(const float* depth, const float* k4, const float* backward_flow, const float* weights,
+                                 float weight_sensitivity, void* ws, const fm_video_layout* layout, int H, int W,
+                                 void* stream) {
+  Ragged r;
+  if (ragged_of(layout, &r) || bad_dims(1, 2, H, W)) return fail_msg("fm_procrustes_moments_videos: bad arguments");
+  return procrustes_fwd_ragged(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, r, H, W,
+                               (cudaStream_t)stream, nullptr, /*solve=*/false);
+}
+
+int fm_softmin_sweep_fwd_videos(const float* depth, const float* weights, float weight_sensitivity,
+                                const float* backward_flow, const int64_t* indices, int num_indices,
+                                const float* cand_k4, int num_candidates, float* err, float* rt, void* ws,
+                                const fm_video_layout* layout, int H, int W, void* stream) {
+  Ragged r;
+  if (ragged_of(layout, &r)) return fail_msg("fm_softmin_sweep_fwd_videos: bad video layout");
+  return sweep_fwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
+                        num_candidates, err, rt, ws, r.B, 2, H, W, stream, &r.v);
+}
+
+int fm_softmin_sweep_bwd_videos(const float* depth, const float* weights, float weight_sensitivity,
+                                const float* backward_flow, const int64_t* indices, int num_indices,
+                                const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
+                                float* g_depth, float* g_weights, void* ws, const fm_video_layout* layout, int H,
+                                int W, void* stream) {
+  Ragged r;
+  if (ragged_of(layout, &r)) return fail_msg("fm_softmin_sweep_bwd_videos: bad video layout");
+  return sweep_bwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
+                        num_candidates, rt, g_err, g_depth, g_weights, ws, r.B, 2, H, W, stream, &r.v);
+}
+
+int fm_adam_step_clock_frames_videos(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                                     size_t frame_elems, const fm_video_layout* layout, int pairs, int frame_lo,
+                                     int frame_hi, const void* clock, int focal_clock, double beta1_d, double beta2_d,
+                                     double eps_d, void* stream) {
+  Ragged r;
+  if (!param || !grad || !exp_avg || !exp_avg_sq || !clock || ragged_of(layout, &r) || frame_lo < 0 ||
+      (pairs != 0 && pairs != 1))
+    return fail_msg("fm_adam_step_clock_frames_videos: bad arguments");
+  if (frame_hi <= frame_lo || frame_elems == 0) return 0;
+  const long long rows = (long long)r.B * (frame_hi - frame_lo);
+  if (rows > 65535) return fail_msg("fm_adam_step_clock_frames_videos: too many frames");
+  size_t nx = (frame_elems + kThreads * 4 - 1) / (kThreads * 4);
+  if (nx < 1) nx = 1;
+  if (nx > 1024) nx = 1024;
+  const StepClock* c = (const StepClock*)clock;
+  k_adam_frames_ragged<<<dim3((unsigned)nx, (unsigned)rows), kThreads, 0, (cudaStream_t)stream>>>(
+      param, grad, exp_avg, exp_avg_sq, frame_elems, r.v.frame_offset, pairs, frame_lo, frame_hi, (float)beta1_d,
+      (float)beta2_d, (float)(1.0 - beta1_d), (float)(1.0 - beta2_d), (float)eps_d,
+      focal_clock ? &c->focal_step_size : &c->step_size);
+  FM_CHECK_LAUNCH("fm_adam_step_clock_frames_videos");
+  return 0;
+}
+
+int fm_pose_chain_videos(const float* rt, float* extrinsics, const fm_video_layout* layout, void* stream) {
+  Ragged r;
+  if (!rt || !extrinsics || ragged_of(layout, &r)) return fail_msg("fm_pose_chain_videos: bad arguments");
+  return pose_chain_ragged(rt, extrinsics, r, stream);
+}
+
+int fm_pose_chain_bwd_videos(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
+                             const fm_video_layout* layout, void* stream) {
+  Ragged r;
+  if (!rt || !extrinsics || !g_extrinsics || !g_rt || ragged_of(layout, &r))
+    return fail_msg("fm_pose_chain_bwd_videos: bad arguments");
+  return pose_chain_bwd_ragged(rt, extrinsics, g_extrinsics, g_rt, r, stream);
 }
 
 }  // extern "C"

@@ -415,10 +415,19 @@ class PackedTracks:
 
     Several videos (the batched fused step): `tracks` is a list of B such lists and `video_frames` the
     frame count F of every video; segment s of video b is packed with start frame b * F + s.start_frame,
-    so the segments of one video address its rows of the (B * F) frame arrays and never cross videos."""
+    so the segments of one video address its rows of the (B * F) frame arrays and never cross videos.
+    Videos of different lengths: `video_frames` is the list of their frame counts F_b, and segment s of
+    video b is packed with start frame fo_b + s.start_frame, fo_b = F_0 + ... + F_{b-1}."""
 
-    def __init__(self, tracks, device, video_frames: Optional[int] = None):
+    def __init__(self, tracks, device, video_frames=None):
         videos = [tracks] if video_frames is None else tracks
+        if isinstance(video_frames, (list, tuple)):
+            if len(video_frames) != len(videos):
+                raise ValueError("flowmap_b200: one frame count per video")
+            counts = [int(n) for n in video_frames]
+        else:
+            counts = None if video_frames is None else [int(video_frames)] * len(videos)
+        firsts = None if counts is None else [sum(counts[:b]) for b in range(len(counts))]
         segs, xy, vis, off = [], [], [], 0
         for b, video in enumerate(videos):
             for t in video:
@@ -427,10 +436,10 @@ class PackedTracks:
                     raise ValueError("flowmap_b200: tracking supports batch size 1 "
                                      "(flowmap/tracking/__init__.py:92-93)")
                 start = int(t.start_frame)
-                if video_frames is not None:
-                    if start < 0 or start + f > video_frames:
-                        raise ValueError(f"flowmap_b200: a track segment of video {b} leaves its {video_frames} frames")
-                    start += b * video_frames
+                if counts is not None:
+                    if start < 0 or start + f > counts[b]:
+                        raise ValueError(f"flowmap_b200: a track segment of video {b} leaves its {counts[b]} frames")
+                    start += firsts[b]
                 segs.append((off, f, n, start))
                 xy.append(t.xy[0].reshape(-1, 2))
                 vis.append(t.visibility[0].reshape(-1))

@@ -155,10 +155,22 @@ class FusedOverfitter(Overfitter):
     each step.  The parameters live in (B, ...) buffers; `models[b]` is video b's Model, whose
     parameters are views into them.  `tracks` is then a list of B segment lists (one per video; its
     tracking loss is normalised by its own valid count), and the metrics log holds (steps, B) values.
-    B > 1 does not serve the splat plan."""
+    B > 1 does not serve the splat plan.
+
+    Videos of different lengths (same H, W): `batch` a list of B one-video Batches, `flows` a list of their
+    Flows (1, F_b - 1, ...) and, with tracking, `tracks` a list of per-video segment lists.  The same B
+    independent overfits in one step (fm_overfit_step_videos); the parameters live in packed (T, H, W) /
+    (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs [fo_b - b, fo_b - b +
+    F_b - 1).  `models[b]` is a Model of F_b frames whose parameters are views into them.  training_step()
+    returns the (B,) totals and a list of the videos' relative poses; extrinsics(), intrinsics_k4() and
+    gradients() hand out per-video lists."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):
+        self._layout = None
+        if isinstance(batch, (list, tuple)):
+            self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
+            return
         b, f, _, h, w = batch.videos.shape
         if b > 1:
             if model is not None:
@@ -275,6 +287,163 @@ class FusedOverfitter(Overfitter):
         self._lib = lib()
         self._mlog = None  # per-step metrics ring (enable_metrics_log)
 
+    def _init_videos(self, cfg, batches, flows, tracks, device, use_splat_plan, model):
+        """The packed optimiser of videos of different lengths (see the class docstring)."""
+        from ._lib import OverfitStepArgs, PackedTracksC, VideoLayout, lib
+        import ctypes
+        if model is not None:
+            raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
+        if use_splat_plan:
+            raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
+        if not batches or not isinstance(flows, (list, tuple)) or len(flows) != len(batches):
+            raise ValueError("flowmap_b200: videos of different lengths need one Flows per Batch")
+        B = len(batches)
+        if cfg.use_tracking and (tracks is None or len(tracks) != B):
+            raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({B})")
+        frames = []
+        for i, bt in enumerate(batches):
+            nb, f, _, h, w = bt.videos.shape
+            if nb != 1:
+                raise ValueError(f"flowmap_b200: video {i} must be a one-video Batch")
+            if (h, w) != tuple(batches[0].videos.shape[-2:]):
+                raise ValueError("flowmap_b200: the videos of one step need the same H x W")
+            if f < 2:
+                raise ValueError(f"flowmap_b200: video {i} has {f} frame(s), a pair needs 2")
+            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+                t = getattr(flows[i], name)
+                if tuple(t.shape[:4]) != (1, f - 1, h, w):
+                    raise ValueError(f"flowmap_b200: flows[{i}].{name} must hold (1, F_b-1, H, W) = (1, {f - 1}, {h}, {w})")
+            frames.append(f)
+        h, w = batches[0].videos.shape[-2:]
+        dev = torch.device(device)
+        self.cfg, self.B, self.frames = cfg, B, frames
+        self.T, self.P = sum(frames), sum(frames) - B
+        self._first = [sum(frames[:i]) for i in range(B)]
+        self._hw = (h, w)
+        self.batches = [bt.to(device) for bt in batches]
+        self.batch = self.batches[0]
+        self.tracks = None if tracks is None else [[t.to(device) for t in v] for v in tracks]
+        self.global_step = self.optimizer_steps = self.focal_steps = 0
+        built = [build_model_and_losses(cfg, f, (h, w)) for f in frames]
+        self.models = [m.to(device) for m, _ in built]
+        self.model, self.losses, self.optimizer = self.models[0], built[0][1], None
+        # packed flows: the pairs of video b follow those of video b - 1
+        self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(dev), n)[0] for fl in flows]).contiguous()
+                             for n in ("forward", "backward", "forward_mask", "backward_mask")))
+        fo = torch.tensor(self._first + [self.T], dtype=torch.int32)
+        self._tables = (fo.to(dev),
+                        torch.repeat_interleave(torch.arange(B, dtype=torch.int32), torch.tensor(frames)).to(dev),
+                        torch.repeat_interleave(torch.arange(B, dtype=torch.int32), torch.tensor(frames) - 1).to(dev))
+        self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
+        self._layout_ref = ctypes.byref(self._layout)
+        self._use_plan, self._plan = False, None
+        self._softmin = cfg.intrinsics == "softmin"
+
+        def pack(params):
+            buf = torch.cat([p.data for p in params]).contiguous()
+            o = 0
+            for p in params:
+                p.data = buf[o:o + p.shape[0]]
+                o += p.shape[0]
+            return buf
+
+        def stack(params):
+            buf = torch.stack([p.data for p in params]).contiguous()
+            for i, p in enumerate(params):
+                p.data = buf[i]
+            return buf
+        self._depth = pack([m.backbone.depth for m in self.models])
+        self._wlog = pack([m.backbone.weights for m in self.models])
+        if not self._softmin:
+            self._focal = stack([m.intrinsics.focal_length for m in self.models])
+        elif cfg.regression_after is not None:
+            self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
+        else:
+            self._focal = torch.zeros(B, device=dev)
+        if self._softmin:
+            n = cfg.softmin_candidates
+            self._cand_f = self.model.intrinsics.focal_length_candidates.float().contiguous()
+            self._cand_k4 = ops.candidate_k4(self._cand_f, h, w, B)
+            self._sw_err, self._sw_sm, self._sw_gerr = (torch.empty(B, n, device=dev) for _ in range(3))
+            self._sw_rt = torch.empty(B * n, 3, 4, device=dev)
+            self._sw_focal = torch.zeros(B, device=dev)
+            self._sw_ws = torch.empty(lib().fm_softmin_workspace_bytes(B, n), dtype=torch.uint8, device=dev)
+            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(self.T, 4).contiguous()
+            self.window = []
+            self.injected_indices = None
+        z = lambda t: torch.zeros_like(t)  # noqa: E731
+        self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog), z(self._focal), z(self._focal)]
+        self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
+        self._g_focal = torch.zeros_like(self._focal)
+        self._k4, self._g_k4 = torch.empty(self.T, 4, device=dev), torch.empty(self.T, 4, device=dev)
+        self.rt = torch.empty(self.P, 3, 4, device=dev)
+        self._loss = torch.zeros(B, device=dev)
+        self._track_loss = torch.zeros_like(self._loss)
+        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
+        self._msum = self._video_mask_sums(self.flows)
+        self._indices = self.model.extrinsics.select_indices(h, w, dev) if not cfg.procrustes_randomize else None
+        a = OverfitStepArgs()
+        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        a.F, a.H, a.W, a.B = 0, h, w, B  # F: ignored by fm_overfit_step_videos
+        a.depth = P(self._depth)
+        a.weight_logits = P(self._wlog) if cfg.use_correspondence_weights else None
+        a.weight_sensitivity = cfg.weight_sensitivity
+        a.focal, a.k4 = P(self._focal), P(self._k4)
+        a.fflow, a.bflow = P(self.flows.forward), P(self.flows.backward)
+        a.fmask, a.bmask = P(self.flows.forward_mask), P(self.flows.backward_mask)
+        a.mask_sum = P(self._msum)
+        a.mapping, a.delta, a.flow_weight = ops.MAPPINGS[cfg.mapping], cfg.delta, cfg.flow_weight
+        (a.m_depth, a.v_depth, a.m_weights, a.v_weights, a.m_focal, a.v_focal) = [P(t) for t in self._state]
+        a.lr, a.beta1, a.beta2, a.eps = cfg.lr, 0.9, 0.999, 1e-8
+        a.g_depth, a.g_weights, a.g_focal, a.g_k4 = P(self._g_depth), P(self._g_w), P(self._g_focal), P(self._g_k4)
+        a.rt, a.loss, a.ws = P(self.rt), P(self._loss), P(self._ws)
+        self._clock = ops.StepClock(dev, cfg.lr)
+        self._side_stream = torch.cuda.Stream(device=dev)
+        a.clock = self._clock.ptr
+        self._total = torch.zeros_like(self._loss)
+        self._idx_buf = torch.empty(min(cfg.softmin_points, h * w), dtype=torch.int64, device=dev) \
+            if self._softmin else None
+        self.use_cuda_graph = False
+        self._graphs, self._eager_runs = {}, {}
+        self._set_plan_args(a)
+        self._packed = None
+        if cfg.use_tracking:
+            pk = ops.PackedTracks(self.tracks, dev, frames)
+            self._packed = pk
+            self._pk_c = PackedTracksC(P(pk.seg), P(pk.xy), P(pk.vis), pk.num_segments, pk.max_rows, pk.max_points,
+                                       pk.total)
+            self._ext = torch.empty(self.T, 4, 4, device=dev)
+            self._g_ext = torch.empty(self.T, 4, 4, device=dev)
+            self._g_rt = torch.empty(self.P, 3, 4, device=dev)
+            self._tg_k4 = torch.empty(self.T, 4, device=dev)
+            self._tws = torch.empty(lib().fm_track_workspace_bytes(self.T, pk.total), dtype=torch.uint8, device=dev)
+            a.track_weight = cfg.tracking_weight
+            a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
+            a.track_g_k4, a.track_loss, a.track_ws = P(self._tg_k4), P(self._track_loss), P(self._tws)
+        self._args, self._ctypes = a, ctypes
+        self._lib = lib()
+        self._mlog = None
+
+    def _dims(self):
+        """(B, F, H, W); with videos of different lengths F is the longest video's frame count."""
+        if self._layout is not None:
+            return self.B, max(self.frames), self._hw[0], self._hw[1]
+        b, f, _, h, w = self.batch.videos.shape
+        return b, f, h, w
+
+    def _per_video(self, t: Tensor, pairs: bool = False):
+        """Views of a packed (T, ...) / (T - B, ...) buffer, one per video."""
+        return [t[f0 - pairs * i:f0 - pairs * i + f - pairs] for i, (f0, f) in enumerate(zip(self._first, self.frames))]
+
+    def _call_step(self, what: str = "fm_overfit_step"):
+        from ._lib import check
+        st = torch.cuda.current_stream().cuda_stream
+        a = self._ctypes.byref(self._args)
+        if self._layout is not None:
+            check(self._lib.fm_overfit_step_videos(a, self._layout_ref, st), what)
+        else:
+            check(self._lib.fm_overfit_step(a, st), what)
+
     def _set_plan_args(self, a):
         pl = self._plan
         a.splat_plan = pl.ptr if pl is not None else None
@@ -283,7 +452,20 @@ class FusedOverfitter(Overfitter):
     def set_flows(self, flows: Flows, mask_sum: Optional[Tensor] = None):
         """Point the step at another device-resident Flows of the same shape (the next batch of a
         prefetching loader) without rebuilding parameters or optimiser state.  `mask_sum` is the
-        flow-loss normaliser (loss_flow.py:70) if the caller already has it."""
+        flow-loss normaliser (loss_flow.py:70) if the caller already has it.  Videos of different
+        lengths: a list of one Flows per video, copied into the packed buffers."""
+        if self._layout is not None:
+            if not isinstance(flows, (list, tuple)) or len(flows) != self.B:
+                raise ValueError(f"flowmap_b200: set_flows needs one Flows per video ({self.B})")
+            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+                dst = self._per_video(getattr(self.flows, name), pairs=True)
+                for i, fl in enumerate(flows):
+                    t = ops._canon(getattr(fl, name), name)
+                    if t.shape != (1, *dst[i].shape) or t.device != dst[i].device:
+                        raise ValueError(f"flowmap_b200: flows[{i}].{name} does not match the optimiser's shapes / device")
+                    dst[i].copy_(t[0])
+            self._msum.copy_(self._video_mask_sums(self.flows) if mask_sum is None else mask_sum)
+            return
         old = self.flows
         canon = {}
         for name in ("forward", "backward", "forward_mask", "backward_mask"):
@@ -308,11 +490,12 @@ class FusedOverfitter(Overfitter):
             return self._video_mask_sums(flows)
         return ops.mask_sum(flows.forward_mask, flows.backward_mask)
 
-    @staticmethod
-    def _video_mask_sums(flows: Flows) -> Tensor:
+    def _video_mask_sums(self, flows: Flows) -> Tensor:
         """(B,) float64: each video's own flow-loss normaliser."""
         fm, bm = flows.forward_mask, flows.backward_mask
-        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(fm.shape[0])])
+        if self._layout is not None:
+            fm, bm = self._per_video(fm, pairs=True), self._per_video(bm, pairs=True)
+        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(len(fm))])
 
     def _bind_batched_parameters(self):
         """B > 1: the videos' parameters move into (B, ...) buffers that the step updates in place; each
@@ -333,14 +516,21 @@ class FusedOverfitter(Overfitter):
         """Adam (step clock) on frames lo <= f < hi of every video of parameter i (0 depth, 1 weight logits)."""
         p, g = ((self._depth, self._g_depth), (self._wlog, self._g_w))[i]
         m, v = self._state[2 * i], self._state[2 * i + 1]
-        if self.B == 1:
+        if self._layout is not None:  # frames (pairs) lo <= r < min(hi, F_b (- 1)) of every video
+            from ._lib import check
+            with torch.cuda.device(p.device):
+                check(self._lib.fm_adam_step_clock_frames_videos(
+                    p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p[0].numel(), self._layout_ref, i, lo, hi,
+                    self._clock.ptr, 0, self._clock.betas[0], self._clock.betas[1], 1e-8,
+                    torch.cuda.current_stream().cuda_stream), "fm_adam_step_clock_frames_videos")
+        elif self.B == 1:
             ops.adam_step_clock(p[lo:hi], g[lo:hi], m[lo:hi], v[lo:hi], self._clock)
         else:
             ops.adam_step_clock_frames(p, g, m, v, lo, hi, self._clock)
 
     def _window_entry(self) -> Tensor:
         """The sweep's focal estimate for the hand-over window: a scalar, or (B,) for B videos."""
-        return self._sw_focal[0].clone() if self.B == 1 else self._sw_focal.clone()
+        return self._sw_focal[0].clone() if self.B == 1 and self._layout is None else self._sw_focal.clone()
 
     def _softmin_stage(self) -> bool:
         c = self.cfg
@@ -352,11 +542,12 @@ class FusedOverfitter(Overfitter):
         the step itself with that focal length, the sweep's backward, then Adam."""
         from ._lib import check
         c, a, L = self.cfg, self._args, self._lib
-        b, f, _, h, w = self.batch.videos.shape
+        b, f, h, w = self._dims()
         dev = self.rt.device
         st = torch.cuda.current_stream().cuda_stream
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         n = c.softmin_candidates
+        rag = self._layout is not None
         wl = P(self._wlog) if c.use_correspondence_weights else None
         sens = c.weight_sensitivity if c.use_correspondence_weights else 0.0
         # All-pixel Procrustes: the moment pass of the step does not have to wait for the focal length
@@ -367,8 +558,13 @@ class FusedOverfitter(Overfitter):
         with torch.cuda.device(dev):
             if early_moments:
                 self._side_stream.wait_stream(cur)
-                check(L.fm_procrustes_moments_batched(P(self._depth), P(self._k4_base), P(self.flows.backward), wl,
-                                                      sens, P(self._ws), b, f, h, w, st), "fm_procrustes_moments")
+                if rag:
+                    check(L.fm_procrustes_moments_videos(P(self._depth), P(self._k4_base), P(self.flows.backward), wl,
+                                                         sens, P(self._ws), self._layout_ref, h, w, st),
+                          "fm_procrustes_moments_videos")
+                else:
+                    check(L.fm_procrustes_moments_batched(P(self._depth), P(self._k4_base), P(self.flows.backward),
+                                                          wl, sens, P(self._ws), b, f, h, w, st), "fm_procrustes_moments")
             with torch.cuda.stream(self._side_stream if early_moments else cur):
                 sst = torch.cuda.current_stream().cuda_stream
                 idx = self.injected_indices
@@ -378,10 +574,16 @@ class FusedOverfitter(Overfitter):
                     else:
                         idx = ops.random_subset(h * w, min(c.softmin_points, h * w), dev)
                 idx = idx.contiguous()
-                check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                             idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                             P(self._sw_rt), P(self._sw_ws), b, f, h, w, sst),
-                      "fm_softmin_sweep_fwd")
+                if rag:
+                    check(L.fm_softmin_sweep_fwd_videos(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
+                                                        idx.numel(), P(self._cand_k4), n, P(self._sw_err),
+                                                        P(self._sw_rt), P(self._sw_ws), self._layout_ref, h, w, sst),
+                          "fm_softmin_sweep_fwd_videos")
+                else:
+                    check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
+                                                 idx.numel(), P(self._cand_k4), n, P(self._sw_err),
+                                                 P(self._sw_rt), P(self._sw_ws), b, f, h, w, sst),
+                          "fm_softmin_sweep_fwd")
                 check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, b, P(self._sw_sm),
                                          P(self._sw_focal), sst), "fm_softmin_focal")
             if early_moments:
@@ -390,12 +592,13 @@ class FusedOverfitter(Overfitter):
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
             # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
-            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and b == 1
+            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and b == 1 and \
+                not rag
             a.focal = P(self._sw_focal)
             a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
             a.defer_adam = 1 if fuse else 0
             try:
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step")
+                self._call_step()
             finally:
                 a.moments_k4 = None
             a.defer_adam = 0
@@ -411,11 +614,18 @@ class FusedOverfitter(Overfitter):
             check(L.fm_softmin_focal_bwd(P(self._sw_sm), P(self._cand_f), P(self._sw_focal),
                                          P(self._g_focal), n, b, P(self._sw_gerr), st),
                   "fm_softmin_focal_bwd")
-            check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                         idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
-                                         P(self._sw_gerr), P(self._g_depth),
-                                         P(self._g_w) if wl else None, P(self._sw_ws), b, f, h, w, st),
-                  "fm_softmin_sweep_bwd")
+            if rag:
+                check(L.fm_softmin_sweep_bwd_videos(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
+                                                    idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
+                                                    P(self._sw_gerr), P(self._g_depth), P(self._g_w) if wl else None,
+                                                    P(self._sw_ws), self._layout_ref, h, w, st),
+                      "fm_softmin_sweep_bwd_videos")
+            else:
+                check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
+                                             idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
+                                             P(self._sw_gerr), P(self._g_depth),
+                                             P(self._g_w) if wl else None, P(self._sw_ws), b, f, h, w, st),
+                      "fm_softmin_sweep_bwd")
         if update:
             self._adam_frames(0, 0, 2)
             if c.use_correspondence_weights:
@@ -436,6 +646,7 @@ class FusedOverfitter(Overfitter):
         candidate sweep first in the softmin stage).  Returns the weighted flow loss (device scalar,
         a buffer that the next call overwrites)."""
         from ._lib import check
+        self._refuse_videos("the split-step surface")
         c, a, L = self.cfg, self._args, self._lib
         _, f, _, h, w = self.batch.videos.shape
         dev = self.rt.device
@@ -485,6 +696,7 @@ class FusedOverfitter(Overfitter):
         """Chained poses + tracking loss of the step begun by forward_phase (loss_tracking.py:28-61).
         Returns the weighted tracking loss (device scalar buffer)."""
         from ._lib import check
+        self._refuse_videos("the split-step surface")
         c, a, L, pk = self.cfg, self._args, self._lib, self._packed
         _, f, _, h, w = self.batch.videos.shape
         P = lambda t: t.data_ptr()  # noqa: E731
@@ -503,6 +715,7 @@ class FusedOverfitter(Overfitter):
         backward].  flow_scale / track_scale: device float scalars d total / d loss (None = 1).
         Leaves the gradients in gradients()."""
         from ._lib import check
+        self._refuse_videos("the split-step surface")
         c, a, L = self.cfg, self._args, self._lib
         _, f, _, h, w = self.batch.videos.shape
         st = torch.cuda.current_stream().cuda_stream
@@ -528,6 +741,10 @@ class FusedOverfitter(Overfitter):
                                              P(self._g_w) if wl else None, P(self._sw_ws), 1, f, h, w, st),
                       "fm_softmin_sweep_bwd")
 
+    def _refuse_videos(self, what: str):
+        if self._layout is not None:
+            raise ValueError(f"flowmap_b200: {what} serves one video, not videos of different lengths")
+
     def _step_body(self, update: bool, track_on: bool, sweep: bool):
         """One step as a fixed launch sequence (no host-side step numbers: see ops.StepClock)."""
         from ._lib import check
@@ -545,9 +762,7 @@ class FusedOverfitter(Overfitter):
                 a.focal = self._focal.data_ptr()
                 a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
                 with torch.cuda.device(self.rt.device):
-                    check(self._lib.fm_overfit_step(self._ctypes.byref(a),
-                                                    torch.cuda.current_stream().cuda_stream),
-                          "fm_overfit_step")
+                    self._call_step()
         finally:
             a.metrics_log = None
         if track_on:
@@ -581,7 +796,7 @@ class FusedOverfitter(Overfitter):
         rt (B, F-1, 3, 4))."""
         c, a = self.cfg, self._args
         if c.procrustes_randomize:
-            _, _, _, h, w = self.batch.videos.shape
+            _, _, h, w = self._dims()
             self._indices = self.model.extrinsics.select_indices(h, w, self.rt.device)
         a.indices = None if self._indices is None else self._indices.data_ptr()
         a.num_indices = 0 if self._indices is None else self._indices.numel()
@@ -604,17 +819,28 @@ class FusedOverfitter(Overfitter):
             self.global_step += 1
             self.optimizer_steps += 1
             self.focal_steps += int(not sweep)
+        if self._layout is not None:
+            return self._total.clone(), self._per_video(self.rt, pairs=True)
         return self._total.clone(), self.rt
 
     def extrinsics(self) -> Tensor:
-        """Camera-to-world poses of the last step (projection.py:187-210)."""
+        """Camera-to-world poses of the last step (projection.py:187-210); a list of (F_b, 4, 4) for videos
+        of different lengths."""
+        if self._layout is not None:
+            return [ops.pose_chain(r[None])[0] for r in self._per_video(self.rt, pairs=True)]
         return ops.pose_chain(self.rt)
 
     def gradients(self):
+        if self._layout is not None:  # per-video views
+            return {"depth": self._per_video(self._g_depth), "weights": self._per_video(self._g_w, pairs=True),
+                    "focal": list(self._g_focal.unbind())}
         return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
 
     def intrinsics_k4(self) -> Tensor:
-        """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for B videos."""
+        """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for B videos; a list of (F_b, 4) for
+        videos of different lengths."""
+        if self._layout is not None:
+            return self._per_video(self._k4)
         return self._k4 if self.B == 1 else self._k4.view(self.B, -1, 4)
 
     METRIC_NAMES = ("train/loss/flow", "train/loss/tracking", "train/intrinsics/fx_error",
@@ -638,7 +864,19 @@ class FusedOverfitter(Overfitter):
         b, dev, B = self.batch, self.rt.device, self.B
         _, f, _, _, _ = b.videos.shape
         nan = float("nan")
-        if B == 1:
+        if self._layout is not None:  # each video's own Batch; the camera centres packed like the frames
+            gts, fxfy = [], []
+            for bt, fb in zip(self.batches, self.frames):
+                gts.append(torch.full((fb, 3), nan, device=dev) if bt.extrinsics is None else
+                           bt.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32))
+                k = None if bt.intrinsics is None else bt.intrinsics[0].double()
+                fxfy.append(torch.tensor([nan, nan], dtype=torch.float64) if k is None else
+                            torch.stack((k[:, 0, 0].mean(), k[:, 1, 1].mean())).cpu())
+            self._mlog_gt = torch.cat(gts).contiguous()
+            self._mlog_fxfy = torch.stack(fxfy).to(device=dev, dtype=torch.float32).contiguous()
+            fx = fy = nan
+            f = self.T
+        elif B == 1:
             self._mlog_gt = None if b.extrinsics is None else \
                 b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
             if b.intrinsics is None:
@@ -653,15 +891,17 @@ class FusedOverfitter(Overfitter):
                 torch.stack((b.intrinsics[:, :, 0, 0].double().mean(1), b.intrinsics[:, :, 1, 1].double().mean(1)), 1)
             self._mlog_fxfy = self._mlog_fxfy.to(device=dev, dtype=torch.float32).contiguous()
             fx = fy = nan
+        one = B == 1 and self._layout is None
         if getattr(self, "_ext", None) is None:  # flow-only steps chain the poses for the log
-            self._ext = torch.empty(B, f, 4, 4, device=dev)
-        self._mlog = torch.full((capacity, 5) if B == 1 else (capacity, B, 5), nan, device=dev)
+            self._ext = torch.empty(B, f, 4, 4, device=dev) if self._layout is None else \
+                torch.empty(self.T, 4, 4, device=dev)
+        self._mlog = torch.full((capacity, 5) if one else (capacity, B, 5), nan, device=dev)
         self._mlog_first = self.optimizer_steps
         a = self._args
         a.extrinsics = self._ext.data_ptr()
         a.gt_positions = None if self._mlog_gt is None else self._mlog_gt.data_ptr()
         a.gt_fx, a.gt_fy, a.metrics_capacity = fx, fy, capacity
-        a.gt_fxfy = None if B == 1 else self._mlog_fxfy.data_ptr()
+        a.gt_fxfy = None if one else self._mlog_fxfy.data_ptr()
         self._graphs.clear()  # captured steps were recorded without the log
         self._eager_runs.clear()
 
@@ -701,7 +941,7 @@ class ShardedFusedOverfitter(FusedOverfitter):
         from dataclasses import replace
         from . import parallel
         from ._lib import lib
-        if batch.videos.shape[0] != 1:
+        if isinstance(batch, (list, tuple)) or batch.videos.shape[0] != 1:
             raise ValueError("flowmap_b200: pair sharding optimises one video (batch size 1)")
         super().__init__(replace(cfg, use_tracking=False), batch, flows, None, device)
         self.cfg = cfg

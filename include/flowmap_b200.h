@@ -395,6 +395,54 @@ typedef struct {
  * parallel branches of the caller's graph. */
 int fm_overfit_step(const fm_overfit_step_args* args, void* stream);
 
+/* Videos of different lengths (same H, W), packed along the frame axis: video b owns the frames
+ * [frame_offset[b], frame_offset[b + 1]) of every per-frame buffer (T, ...) and the pairs
+ * [frame_offset[b] - b, frame_offset[b + 1] - b - 1) of every per-pair buffer (P, ...), P = T - B; no pair
+ * crosses two videos.  The three tables live in device memory and belong to the caller, who keeps them
+ * consistent (frame_offset[0] = 0, frame_offset[B] = T, every video >= 2 frames). */
+typedef struct {
+  int B;                    /* number of videos */
+  int T;                    /* frames of all videos */
+  const int* frame_offset;  /* (B + 1) first frame of every video, then T */
+  const int* frame_video;   /* (T) the video of every frame */
+  const int* pair_video;    /* (T - B) the video of every pair */
+} fm_video_layout;
+/* fm_overfit_step for videos of different lengths: args->B and args->F are ignored, every per-frame /
+ * per-pair buffer has the packed layout above, and the per-video scalars (focal, mask_sum, loss,
+ * track_loss, g_focal, m_focal, v_focal) hold B values, as with args->B > 1.  Video b gets what a
+ * one-video step on it gets; its poses chain from the identity at its own frame 0.  Tracks: the segments
+ * of video b carry start frames frame_offset[b] + s; track_ws is fm_track_workspace_bytes(T, total_samples).
+ * Metrics: gt_positions (T, 3), NaN first position of a video = no ground truth; the ring is
+ * (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).  Same restrictions as args->B > 1 (whole
+ * steps, no splat plan, no fused logit update in a deferred step). */
+int fm_overfit_step_videos(const fm_overfit_step_args* args, const fm_video_layout* layout, void* stream);
+size_t fm_workspace_bytes_videos(int B, int T);
+/* fm_procrustes_moments for packed videos of different lengths (see fm_overfit_step_args.moments_k4). */
+int fm_procrustes_moments_videos(const float* depth, const float* k4, const float* backward_flow,
+                                 const float* weights, float weight_sensitivity, void* ws,
+                                 const fm_video_layout* layout, int H, int W, void* stream);
+/* fm_softmin_sweep_fwd / _bwd on pair 0 of every video of a packed layout (cand_k4, err, rt, ws: as
+ * there with B = layout->B). */
+int fm_softmin_sweep_fwd_videos(const float* depth, const float* weights, float weight_sensitivity,
+                                const float* backward_flow, const int64_t* indices, int num_indices,
+                                const float* cand_k4, int num_candidates, float* err, float* rt, void* ws,
+                                const fm_video_layout* layout, int H, int W, void* stream);
+int fm_softmin_sweep_bwd_videos(const float* depth, const float* weights, float weight_sensitivity,
+                                const float* backward_flow, const int64_t* indices, int num_indices,
+                                const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
+                                float* g_depth, float* g_weights, void* ws, const fm_video_layout* layout,
+                                int H, int W, void* stream);
+/* fm_adam_step_clock_frames for a packed layout: the rows lo <= r < min(hi, rows of video b) of every
+ * video b, rows = its frames (pairs = 0: depth) or its pairs (pairs = 1: weight logits). */
+int fm_adam_step_clock_frames_videos(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                                     size_t frame_elems, const fm_video_layout* layout, int pairs, int frame_lo,
+                                     int frame_hi, const void* clock, int focal_clock, double beta1,
+                                     double beta2, double eps, void* stream);
+/* fm_pose_chain / fm_pose_chain_bwd for a packed layout: rt (T - B, 3, 4), extrinsics (T, 4, 4). */
+int fm_pose_chain_videos(const float* rt, float* extrinsics, const fm_video_layout* layout, void* stream);
+int fm_pose_chain_bwd_videos(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
+                             const fm_video_layout* layout, void* stream);
+
 /* Phase A alone (all pixels, one video): the 16 weighted moment sums of every frame pair into `ws`,
  * for intrinsics `k4` (F,4); `weights` are plain weights (weight_sensitivity == 0) or logits.  See
  * fm_overfit_step_args.moments_k4.  (Model.forward's first reduction, model.py:75-90 with
