@@ -78,9 +78,6 @@ SIGNATURES = {
     "fm_step_clock_tick": (c_int, [_P, c_double, c_double, c_double, ctypes.c_ulonglong, c_int, _P]),
     "fm_adam_step_clock": (c_int, [_P, _P, _P, _P, c_size_t, _P, c_int, c_double, c_double, c_double, _P]),
     "fm_random_subset_clock": (c_int, [_P, ctypes.c_longlong, c_int, _P, _P]),
-    "fm_procrustes_moments_batched": (c_int, [_P, _P, _P, _P, c_float, _P, c_int, c_int, c_int, c_int, _P]),
-    "fm_adam_step_clock_frames": (c_int, [_P, _P, _P, _P, c_size_t, c_int, c_int, c_int, c_int, _P, c_int,
-                                          c_double, c_double, c_double, _P]),
 }
 
 

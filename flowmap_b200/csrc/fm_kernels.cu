@@ -815,62 +815,10 @@ k_flow_lean(const float* __restrict__ depth, const float* __restrict__ k4, const
   }
 }
 
-// k_flow_lean for B independent videos (fm_overfit_step_args.B > 1): mask_sum holds one normaliser per
-// video and frame f of video b is scaled by its own (LossFlow instead normalises a batch by one sum).
-// A separate kernel, so that k_flow_lean keeps its code.
-template <int VEC, bool FOCAL, int MINB>
-__global__ void __launch_bounds__(kThreads, MINB)
-k_flow_lean_videos(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
-                   const float* __restrict__ fflow, const float* __restrict__ bflow,
-                   const float* __restrict__ fmask, const float* __restrict__ bmask,
-                   const double* __restrict__ mask_sum, int mapping, float delta, float loss_weight,
-                   float* __restrict__ g_depth, double* __restrict__ leanacc, int F, int H, int W, int BF) {
-  __shared__ double smem[kFlowLeanVals * (kThreads / 32)];
-  const int N = H * W;
-  constexpr int kChunk = kThreads * VEC;
-  const int chunks = (N + kChunk - 1) / kChunk;
-  const ItemRange range = block_item_range((long long)BF * chunks);
-  const RobustCfg rc = make_robust(mapping, delta, H, W);
-  const GridDims grid = make_grid(H, W);
-#pragma unroll 1
-  for (int it = range.i0; it < range.i1;) {
-    const int frame = it / chunks, cb = it - frame * chunks;
-    const int ce = (cb + (range.i1 - it) < chunks) ? cb + (range.i1 - it) : chunks;
-    const int bi = frame / F, i = frame - bi * F;
-    double den = mask_sum[bi];
-    if (den == 0.0) den = 1.0;  // loss_flow.py:70 "valid_sum or 1", per video
-    const float g = (float)((double)loss_weight / den);
-    const bool hasF = i < F - 1, hasB = i > 0;
-    FlowFrameLean f;
-    f.kk = make_cam(load_k4(k4, frame));
-    f.kn = make_cam(load_k4(k4, hasF ? frame + 1 : frame));
-    f.kp = make_cam(load_k4(k4, hasB ? frame - 1 : frame));
-    const int pairF = bi * (F - 1) + i, pairB = pairF - 1;
-    Rt tf, tb;
-    if (hasF) tf = load_rt(rt, pairF);
-    if (hasB) tb = load_rt(rt, pairB);
-    fill_lean(f, hasF ? &tf : nullptr, hasB ? &tb : nullptr);
-    const float* D = depth + (size_t)frame * N;
-    const float* ff = fflow + (size_t)(hasF ? pairF : 0) * N * 2;
-    const float* mf = fmask + (size_t)(hasF ? pairF : 0) * N;
-    const float* fb = bflow + (size_t)(hasB ? pairB : 0) * N * 2;
-    const float* mb = bmask + (size_t)(hasB ? pairB : 0) * N;
-    float* gd = g_depth + (size_t)frame * N;
-    float acc[kFlowLeanVals];
-#pragma unroll
-    for (int k = 0; k < kFlowLeanVals; ++k) acc[k] = 0.f;
-    if (hasF && hasB) flow_frame_body_lean<VEC, true, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
-    else if (hasF) flow_frame_body_lean<VEC, true, false, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
-    else flow_frame_body_lean<VEC, false, true, FOCAL>(f, D, ff, mf, fb, mb, gd, g, rc, grid, N, acc, cb, ce);
-    // lean slots live in the upper half of the frame's accumulator row until k_flow_lean_convert
-    block_accumulate<kFlowLeanVals>(acc, leanacc + (size_t)frame * kFlowAcc, smem);
-    it += ce - cb;
-  }
-}
-
-
-// k_flow_lean_videos for videos of different lengths: the frame's video from the tables of `v`.  Its own
-// copy of the kernel: as a body shared with k_flow_lean_videos, the table lookups changed that kernel's code.
+// k_flow_lean for several videos packed along the frame axis (fm_overfit_step_videos): the frame's video
+// from the tables of `v`, and mask_sum holds one normaliser per video, so frame f of video b is scaled by
+// its own (LossFlow instead normalises a batch by one sum).  A separate kernel, so that k_flow_lean keeps
+// its code.
 template <int VEC, bool FOCAL, int MINB>
 __global__ void __launch_bounds__(kThreads, MINB)
 k_flow_lean_ragged(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
@@ -1018,10 +966,12 @@ __global__ void k_flow_finalize(const double* __restrict__ flowacc, const float*
   }
 }
 
-// The batched fused step's flow losses: block b sums the F per-frame loss terms of video b into loss[b],
-// in the order in which k_flow_finalize's block 0 sums them for one video (launched with 128 threads).
-// (k_flow_video_loss_ragged: video b's frames start at frame_offset[b] and number its own F.)
-__device__ __forceinline__ void flow_video_loss_body(const double* __restrict__ acc, float* __restrict__ loss, int F) {
+// The packed fused step's flow losses: block b sums the F_b per-frame loss terms of video b (frames from
+// frame_offset[b]) into loss[b], in the order in which k_flow_finalize's block 0 sums them for one video
+// (launched with 128 threads).
+__global__ void k_flow_video_loss_ragged(const double* __restrict__ flowacc, float* __restrict__ loss, Videos v) {
+  const double* acc = flowacc + (size_t)v.first(blockIdx.x) * kFlowAcc;
+  const int F = v.frames(blockIdx.x);
   __shared__ double part[32];
   double s = 0.0;
   for (int k = threadIdx.x; k < F; k += blockDim.x) s += acc[(size_t)k * kFlowAcc];
@@ -1033,12 +983,6 @@ __device__ __forceinline__ void flow_video_loss_body(const double* __restrict__ 
     for (int w = 0; w < (int)((blockDim.x + 31) >> 5); ++w) tot += part[w];
     loss[blockIdx.x] = (float)tot;
   }
-}
-__global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __restrict__ loss, int F) {
-  flow_video_loss_body(flowacc + (size_t)blockIdx.x * F * kFlowAcc, loss, F);
-}
-__global__ void k_flow_video_loss_ragged(const double* __restrict__ flowacc, float* __restrict__ loss, Videos v) {
-  flow_video_loss_body(flowacc + (size_t)v.first(blockIdx.x) * kFlowAcc, loss, v.frames(blockIdx.x));
 }
 
 // ================================================================== phase D1: adjoint solve
@@ -1847,27 +1791,11 @@ k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m
   }
 }
 
-// k_adam on the frames lo <= f < hi of each video of F frames (frame_elems values per frame): the part of
-// a batched (B, F, ...) parameter whose gradient is final, without slice views.  blockIdx.y = one
-// (video, frame) row, so the index arithmetic stays out of the element loop.
-__global__ void __launch_bounds__(kThreads)
-k_adam_frames(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-              size_t frame_elems, int F, int lo, int hi, float beta1, float beta2, float omb1, float omb2,
-              float eps, const float* __restrict__ consts) {
-  const float step_size = __ldg(consts), bc2_sqrt = __ldg(consts + 1);
-  const int span = hi - lo, b = blockIdx.y / span, f = lo + (blockIdx.y - b * span);
-  const size_t o = ((size_t)b * F + f) * frame_elems;
-  p += o; g += o; m += o; v += o;
-  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < frame_elems; i += (size_t)gridDim.x * kThreads) {
-    float pp = p[i], gg = g[i], mm = m[i], vv = v[i];
-    FM_ADAM1(pp, gg, mm, vv)
-    p[i] = pp; m[i] = mm; v[i] = vv;
-  }
-}
-
-// k_adam_frames for videos of different lengths: the rows lo <= r < min(hi, rows of video b) of every
-// video b, whose rows start at row_offset[b] - pairs * b and number row_offset[b + 1] - row_offset[b] - pairs
-// (row_offset = frame offsets; pairs = 0 for per-frame parameters, 1 for per-pair ones).
+// k_adam on the rows lo <= r < min(hi, rows of video b) of every video b of a packed parameter
+// (frame_elems values per row): the part whose gradient is final, without slice views.  Video b's rows
+// start at row_offset[b] - pairs * b and number row_offset[b + 1] - row_offset[b] - pairs (row_offset =
+// frame offsets; pairs = 0 for per-frame parameters, 1 for per-pair ones).  blockIdx.y = one (video, row),
+// so the index arithmetic stays out of the element loop.
 __global__ void __launch_bounds__(kThreads)
 k_adam_frames_ragged(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                      size_t frame_elems, const int* __restrict__ row_offset, int pairs, int lo, int hi, float beta1,
@@ -2070,15 +1998,9 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
   return ((size_t)max_rows * (kTrackRec + (kTrackThreads / 32) * kTrackAcc) + (size_t)list_cap) * sizeof(float);
 }
 
-// VIDEOS (the batched fused step): the segments of video b have start frames in [b F, (b + 1) F), F =
-// video_frames, and its loss sum / valid count go to sums[2 b], sums[2 b + 1].  kRaggedVideos (videos of
-// different lengths): the video of a start frame is frame_video[start frame].
-constexpr int kRaggedVideos = 2;
-template <int VIDEOS>
-__device__ __forceinline__ int video_of_segment(int start_frame, int video_frames, const int* frame_video) {
-  return VIDEOS == kRaggedVideos ? __ldg(frame_video + start_frame) : start_frame / video_frames;
-}
-template <bool SHARED_K, int VIDEOS>
+// RAGGED (several videos packed along the frame axis, fm_overfit_step_videos): the video of a segment is
+// frame_video[its start frame], and that video's loss sum / valid count go to sums[2 b], sums[2 b + 1].
+template <bool SHARED_K, bool RAGGED>
 __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, const float* __restrict__ k4,
                                                const float* __restrict__ ext, const int* __restrict__ seg,
                                                const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
@@ -2086,8 +2008,8 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
                                                unsigned char* __restrict__ flag, float* __restrict__ dq_out,
                                                double* __restrict__ trackacc, int* __restrict__ next_item,
                                                int num_items, int max_rows, int list_cap, int H, int W,
-                                               TrackShard sh, int video_frames, float4* sm4, double* red,
-                                               int* s_wbase, int* s_item, const int* frame_video = nullptr) {
+                                               TrackShard sh, float4* sm4, double* red, int* s_wbase, int* s_item,
+                                               const int* frame_video = nullptr) {
   float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
   constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
@@ -2286,7 +2208,7 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
       __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
     block_accumulate<2, kTrackThreads>(
-        lc, VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(si.start_frame, video_frames, frame_video) : sums, red);
+        lc, RAGGED ? sums + 2 * __ldg(frame_video + si.start_frame) : sums, red);
     block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
     // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
     // with a barrier, so every slice is complete)
@@ -2317,17 +2239,12 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
 template <bool SHARED_K>
 __global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src(FM_TRACK_SRC_PARAMS) {
   FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, 0>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item);
-}
-template <bool SHARED_K>
-__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_videos(FM_TRACK_SRC_PARAMS, int video_frames) {
-  FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, 1>(FM_TRACK_SRC_ARGS, video_frames, sm4, red, s_wbase, s_item);
+  track_src_body<SHARED_K, false>(FM_TRACK_SRC_ARGS, sm4, red, s_wbase, s_item);
 }
 template <bool SHARED_K>
 __global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_ragged(FM_TRACK_SRC_PARAMS, const int* frame_video) {
   FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, kRaggedVideos>(FM_TRACK_SRC_ARGS, 0, sm4, red, s_wbase, s_item, frame_video);
+  track_src_body<SHARED_K, true>(FM_TRACK_SRC_ARGS, sm4, red, s_wbase, s_item, frame_video);
 }
 #undef FM_TRACK_SRC_SHARED
 #undef FM_TRACK_SRC_PARAMS
@@ -2343,29 +2260,28 @@ __global__ void k_track_loss(const double* __restrict__ sums, float loss_weight,
   *loss = (float)(track_scale(sums, loss_weight, nullptr) * sums[0]);
 }
 
-// The batched fused step's tracking losses: thread b reads video b's loss sum / valid count.
+// The packed fused step's tracking losses: thread b reads video b's loss sum / valid count.
 __global__ void k_track_video_loss(const double* __restrict__ sums, float loss_weight, float* __restrict__ loss, int B) {
   const int b = threadIdx.x;
   if (b < B) loss[b] = (float)(track_scale(sums + 2 * b, loss_weight, nullptr) * sums[2 * b]);
 }
 
-// scale * (stored camera-space adjoint) -> the four depth taps of every source sample.  VIDEOS: the scale
-// of the segment's video (start frame / video_frames), see track_src_body.
-template <int VIDEOS>
+// scale * (stored camera-space adjoint) -> the four depth taps of every source sample.  RAGGED: the scale
+// of the segment's video (frame_video[start frame]), see track_src_body.
+template <bool RAGGED>
 __device__ __forceinline__ void track_apply_body(const float* __restrict__ k4, const int* __restrict__ seg,
                                                  const float* __restrict__ txy, const unsigned char* __restrict__ flag,
                                                  const float* __restrict__ dq, const double* __restrict__ sums,
                                                  float loss_weight, const float* __restrict__ go,
                                                  float* __restrict__ g_depth, int H, int W, TrackShard sh,
-                                                 int video_frames, const int* frame_video = nullptr) {
+                                                 const int* frame_video = nullptr) {
   const SegInfo si = load_seg(seg, blockIdx.z);
   const int row = blockIdx.y;
   const int p = blockIdx.x * kThreads + threadIdx.x;
   if (row >= si.rows || p >= si.n || !sh.owns(si.start_frame + row)) return;
   const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p;
   if (!flag[sidx]) return;
-  const float scale = (float)track_scale(
-      VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(si.start_frame, video_frames, frame_video) : sums, loss_weight, go);
+  const float scale = (float)track_scale(RAGGED ? sums + 2 * __ldg(frame_video + si.start_frame) : sums, loss_weight, go);
   const int frame = si.start_frame + row;
   const GridDims grid = make_grid(H, W);
   const Cam ks = make_cam(load_k4(k4, frame));
@@ -2386,15 +2302,7 @@ k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const f
               const unsigned char* __restrict__ flag, const float* __restrict__ dq,
               const double* __restrict__ sums, float loss_weight, const float* __restrict__ go,
               float* __restrict__ g_depth, int H, int W, TrackShard sh) {
-  track_apply_body<0>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh, 0);
-}
-
-__global__ void __launch_bounds__(kThreads)
-k_track_apply_videos(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
-                     const unsigned char* __restrict__ flag, const float* __restrict__ dq,
-                     const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
-                     TrackShard sh, int video_frames) {
-  track_apply_body<1>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, video_frames);
+  track_apply_body<false>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh);
 }
 
 __global__ void __launch_bounds__(kThreads)
@@ -2402,22 +2310,18 @@ k_track_apply_ragged(const float* __restrict__ k4, const int* __restrict__ seg, 
                      const unsigned char* __restrict__ flag, const float* __restrict__ dq,
                      const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
                      TrackShard sh, const int* __restrict__ frame_video) {
-  track_apply_body<kRaggedVideos>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, 0,
-                                  frame_video);
+  track_apply_body<true>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, frame_video);
 }
 
-// VIDEOS: frames f of B * video_frames, scaled by the sums of video f / video_frames (kRaggedVideos:
-// of video frame_video[f]).
-template <int VIDEOS>
+// RAGGED: frame f scaled by the sums of its video frame_video[f].
+template <bool RAGGED>
 __device__ __forceinline__ void track_finalize_body(const double* __restrict__ trackacc, const double* __restrict__ sums,
                                                     float loss_weight, const float* __restrict__ go,
                                                     const float* __restrict__ ext, float* __restrict__ g_ext,
-                                                    float* __restrict__ g_k4, int F, int video_frames,
-                                                    const int* frame_video = nullptr) {
+                                                    float* __restrict__ g_k4, int F, const int* frame_video = nullptr) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
-  const double sc = track_scale(VIDEOS ? sums + 2 * video_of_segment<VIDEOS>(f, video_frames, frame_video) : sums,
-                                loss_weight, go);
+  const double sc = track_scale(RAGGED ? sums + 2 * __ldg(frame_video + f) : sums, loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
   for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
   const float* P = ext + (size_t)f * 16;
@@ -2437,19 +2341,13 @@ __global__ void k_track_finalize(const double* __restrict__ trackacc, const doub
                                  float loss_weight, const float* __restrict__ go,
                                  const float* __restrict__ ext, float* __restrict__ g_ext,
                                  float* __restrict__ g_k4, int F) {
-  track_finalize_body<0>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F, 0);
-}
-
-__global__ void k_track_finalize_videos(const double* __restrict__ trackacc, const double* __restrict__ sums,
-                                        float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
-                                        float* __restrict__ g_k4, int BF, int video_frames) {
-  track_finalize_body<1>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, BF, video_frames);
+  track_finalize_body<false>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F);
 }
 
 __global__ void k_track_finalize_ragged(const double* __restrict__ trackacc, const double* __restrict__ sums,
                                         float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
                                         float* __restrict__ g_k4, int T, const int* __restrict__ frame_video) {
-  track_finalize_body<kRaggedVideos>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, T, 0, frame_video);
+  track_finalize_body<true>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, T, frame_video);
 }
 
 // ================================================================== focal-length sweep
@@ -2923,23 +2821,22 @@ k_trajectory_ate(const float* __restrict__ gt, const float* __restrict__ pred, i
   }
 }
 
-// The batched fused step's metrics rows: block b writes video b of row (step - 1) % capacity of the
+// The packed fused step's metrics rows: block b writes video b of row (step - 1) % capacity of the
 // (capacity, B, 5) ring, with what k_trajectory_ate writes for one video (the same float64 sums in the
-// same order).  gt (B, F, 3); a video whose first position is NaN has no ground truth (ATE NaN);
-// gt_fxfy (B, 2) frame means of the ground-truth intrinsics (NaN: no ground truth).
-// RAGGED (k_metrics_ragged): video b's frames start at frame f0 = frame_offset[b] and number its own F.
-template <bool RAGGED>
-__device__ __forceinline__ void metrics_videos_body(const float* __restrict__ gt, const float* __restrict__ pred,
-                                                    int F, MetricsRow row, const float* __restrict__ gt_fxfy,
-                                                    const Videos& vids) {
+// same order).  Video b's frames start at frame f0 = frame_offset[b] and number its own F.  gt (T, 3); a
+// video whose first position is NaN has no ground truth (ATE NaN); gt_fxfy (B, 2) frame means of the
+// ground-truth intrinsics (NaN: no ground truth).
+__global__ void __launch_bounds__(kAteThreads)
+k_metrics_ragged(const float* __restrict__ gt, const float* __restrict__ pred, MetricsRow row,
+                 const float* __restrict__ gt_fxfy, Videos vids) {
   __shared__ double s_red[kAteThreads / 32 * 9];
   const size_t b = blockIdx.x;
   float* r = row.log + ((size_t)((row.clock->step - 1u) % (unsigned)row.capacity) * gridDim.x + b) * 5;
-  const size_t f0 = RAGGED ? vids.first(b) : 0;
-  if (RAGGED) F = vids.frames(b);
-  const bool has_gt = gt && !isnan(gt[RAGGED ? f0 * 3 : b * F * 3]);
+  const size_t f0 = vids.first(b);
+  const int F = vids.frames(b);
+  const bool has_gt = gt && !isnan(gt[f0 * 3]);
   if (threadIdx.x == 0) {
-    const float* k4 = row.k4 + (RAGGED ? f0 * 4 : b * F * 4);
+    const float* k4 = row.k4 + f0 * 4;
     double fx = 0.0, fy = 0.0;
     for (int f = 0; f < F; ++f) { fx += (double)k4[f * 4 + 0]; fy += (double)k4[f * 4 + 1]; }
     r[0] = row.loss[b];
@@ -2950,8 +2847,8 @@ __device__ __forceinline__ void metrics_videos_body(const float* __restrict__ gt
   }
   if (!has_gt) return;
   AtePoints x;
-  x.gt = gt + (RAGGED ? f0 * 3 : b * F * 3);
-  x.pred = pred + (RAGGED ? f0 * 16 : b * F * 16);
+  x.gt = gt + f0 * 3;
+  x.pred = pred + f0 * 16;
   x.gt_stride = 3;
   x.pred_stride = 16;
   x.pred_cstride = 4;
@@ -2960,17 +2857,6 @@ __device__ __forceinline__ void metrics_videos_body(const float* __restrict__ gt
   double v;
   trajectory_ate(x, threadIdx.x, kAteThreads, red, v, nullptr, nullptr);
   if (threadIdx.x == 0) r[4] = (float)v;
-}
-
-__global__ void __launch_bounds__(kAteThreads)
-k_metrics_videos(const float* __restrict__ gt, const float* __restrict__ pred, int F, MetricsRow row,
-                 const float* __restrict__ gt_fxfy) {
-  metrics_videos_body<false>(gt, pred, F, row, gt_fxfy, Videos{});
-}
-__global__ void __launch_bounds__(kAteThreads)
-k_metrics_ragged(const float* __restrict__ gt, const float* __restrict__ pred, MetricsRow row,
-                 const float* __restrict__ gt_fxfy, Videos v) {
-  metrics_videos_body<true>(gt, pred, 0, row, gt_fxfy, v);
 }
 
 // ================================================================== fused overfit step helpers
@@ -2985,26 +2871,17 @@ __global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restri
   k4[t * 4 + 3] = 0.5f;
 }
 
-// k_k4_from_focal for B videos with one focal length each: frame t of the (B*F, 4) rows reads focal[t / F].
-// (k_k4_from_focals_ragged: frame t reads the focal length of its video frame_video[t].)
-template <bool RAGGED>
-__device__ __forceinline__ void k4_from_focals_body(const float* __restrict__ focal, float* __restrict__ k4, int BF,
-                                                    int F, int H, int W, const Videos& v) {
+// k_k4_from_focal for packed videos with one focal length each: frame t of the (T, 4) rows reads the focal
+// length of its video frame_video[t].
+__global__ void k_k4_from_focals_ragged(const float* __restrict__ focal, float* __restrict__ k4, int T, int H, int W,
+                                        Videos v) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= BF) return;
-  const float scaled = focal[RAGGED ? v.of_frame(t) : t / F] * sqrtf((float)H * (float)W);
+  if (t >= T) return;
+  const float scaled = focal[v.of_frame(t)] * sqrtf((float)H * (float)W);
   k4[t * 4 + 0] = scaled / (float)W;
   k4[t * 4 + 1] = scaled / (float)H;
   k4[t * 4 + 2] = 0.5f;
   k4[t * 4 + 3] = 0.5f;
-}
-__global__ void k_k4_from_focals(const float* __restrict__ focal, float* __restrict__ k4, int BF, int F, int H,
-                                 int W) {
-  k4_from_focals_body<false>(focal, k4, BF, F, H, W, Videos{});
-}
-__global__ void k_k4_from_focals_ragged(const float* __restrict__ focal, float* __restrict__ k4, int T, int H, int W,
-                                        Videos v) {
-  k4_from_focals_body<true>(focal, k4, T, 0, H, W, v);
 }
 
 // d loss / d focal from the per-frame k4 gradients (flow-loss part + Procrustes part).
@@ -3037,15 +2914,8 @@ __global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __r
   focal_grad_block(k4acc, flowacc, extra_g_k4, g_focal, B, F, H, W, flow_scale);
 }
 
-// One focal length per video (the batched fused step): block b writes g_focal[b] from video b's frames,
+// One focal length per video (the packed fused step): block b writes g_focal[b] from video b's frames,
 // summed in the order k_focal_grad uses for one video.
-__global__ void k_focal_grad_videos(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                                    const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int F, int H,
-                                    int W) {
-  const size_t f0 = (size_t)blockIdx.x * F;
-  focal_grad_block(k4acc + f0 * 4, flowacc + f0 * kFlowAcc, extra_g_k4 ? extra_g_k4 + f0 * 4 : nullptr,
-                   g_focal + blockIdx.x, 1, F, H, W, nullptr);
-}
 __global__ void k_focal_grad_ragged(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
                                     const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int H, int W,
                                     Videos v) {
@@ -3128,8 +2998,7 @@ namespace {
 int launch_flow(const float* depth, const float* k4, const float* rt, const float* ff, const float* fb,
                 const float* mf, const float* mb, const double* mask_sum, int mapping, float delta,
                 float loss_weight, int intrinsics_mode, float* g_depth, double* flowacc, int B, int F,
-                int H, int W, cudaStream_t s, bool per_video = false) {
-  if (per_video && intrinsics_mode == 0) return fail_msg("launch_flow: per-video normalisers need shared intrinsics");
+                int H, int W, cudaStream_t s) {
   const int BF = B * F;
   const int vec = (W % 4 == 0) ? 4 : 1;
   dim3 grid(blocks_for(H * W, vec), BF);
@@ -3141,15 +3010,7 @@ int launch_flow(const float* depth, const float* k4, const float* rt, const floa
   }
   const bool focal = intrinsics_mode == 1;
   const int pg = persistent_grid(2, (long long)BF * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
-  if (per_video) {  // mask_sum holds B normalisers
-    if (vec == 4) {
-      if (focal) k_flow_lean_videos<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-      else k_flow_lean_videos<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-    } else {
-      if (focal) k_flow_lean_videos<1, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-      else k_flow_lean_videos<1, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-    }
-  } else if (vec == 4) {
+  if (vec == 4) {
     if (focal) k_flow_lean<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
     else k_flow_lean<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
   } else {
@@ -3300,7 +3161,7 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 104; }
+int fm_version(void) { return 105; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -3414,13 +3275,7 @@ int fm_procrustes_fwd(const float* depth, const float* k4, const float* backward
 int fm_procrustes_moments(const float* depth, const float* k4, const float* backward_flow,
                           const float* weights, float weight_sensitivity, void* ws, int F, int H, int W,
                           void* stream) {
-  return fm_procrustes_moments_batched(depth, k4, backward_flow, weights, weight_sensitivity, ws, 1, F, H, W, stream);
-}
-
-int fm_procrustes_moments_batched(const float* depth, const float* k4, const float* backward_flow,
-                                  const float* weights, float weight_sensitivity, void* ws, int B, int F, int H,
-                                  int W, void* stream) {
-  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, B, F,
+  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, 1, F,
                              H, W, stream, nullptr, nullptr, nullptr, /*solve=*/false);
 }
 
@@ -3760,25 +3615,6 @@ int fm_adam_step_clock(float* param, const float* grad, float* exp_avg, float* e
   return 0;
 }
 
-int fm_adam_step_clock_frames(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t frame_elems,
-                              int B, int F, int frame_lo, int frame_hi, const void* clock, int focal_clock,
-                              double beta1_d, double beta2_d, double eps_d, void* stream) {
-  if (!param || !grad || !exp_avg || !exp_avg_sq || !clock || B < 1 || F < 1 || frame_lo < 0 || frame_hi > F)
-    return fail_msg("fm_adam_step_clock_frames: bad arguments");
-  if (frame_hi <= frame_lo || frame_elems == 0) return 0;
-  const int rows = B * (frame_hi - frame_lo);
-  if (rows > 65535) return fail_msg("fm_adam_step_clock_frames: too many frames");
-  size_t nx = (frame_elems + kThreads * 4 - 1) / (kThreads * 4);
-  if (nx < 1) nx = 1;
-  if (nx > 1024) nx = 1024;
-  const StepClock* c = (const StepClock*)clock;
-  k_adam_frames<<<dim3((unsigned)nx, (unsigned)rows), kThreads, 0, (cudaStream_t)stream>>>(
-      param, grad, exp_avg, exp_avg_sq, frame_elems, F, frame_lo, frame_hi, (float)beta1_d, (float)beta2_d,
-      (float)(1.0 - beta1_d), (float)(1.0 - beta2_d), (float)eps_d, focal_clock ? &c->focal_step_size : &c->step_size);
-  FM_CHECK_LAUNCH("fm_adam_step_clock_frames");
-  return 0;
-}
-
 int fm_random_subset_clock(const void* clock, long long N, int n, int64_t* out, void* stream) {
   if (!clock || N < 1 || n < 1 || n > N || !out) return fail_msg("fm_random_subset_clock: bad arguments");
   k_random_subset<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(0ull, N, n, out, &((const StepClock*)clock)->seed);
@@ -3832,11 +3668,9 @@ size_t fm_track_reduce_bytes(int F) {
   return align_up(4 * sizeof(double), 256) + align_up((size_t)F * kTrackAcc * sizeof(double), 256);
 }
 
-// vsums != NULL (the batched fused step): the frames are B videos of F / B frames, and each video's loss
-// sum and valid count go to vsums[2 b], vsums[2 b + 1] (zeroed here) instead of the head of ws; `loss`
-// then receives B values.  frame_video != NULL as well: videos of different lengths, the video of a
-// segment's start frame from that table.
-// then receives B values.
+// vsums != NULL (the packed fused step): the frames are B videos packed along the frame axis, the video of
+// a segment's start frame is frame_video[that frame], and each video's loss sum and valid count go to
+// vsums[2 b], vsums[2 b + 1] (zeroed here) instead of the head of ws; `loss` then receives B values.
 static int track_fwd_impl(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                           int num_segments, int max_rows, int max_points, const float* track_xy,
                           const unsigned char* track_vis, long long total_samples, int mapping, float delta,
@@ -3873,22 +3707,13 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
     if (ea != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ea);
   }
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
-  if (vsums && frame_video) {
+  if (vsums) {  // one focal length per video: shared intrinsics
     static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
     k_track_src_ragged<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
                                                                mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
                                                                (int)items, max_rows, list_cap, H, W, sh, frame_video);
     FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_ragged");
-  } else if (vsums) {  // one focal length per video: shared intrinsics
-    static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_videos<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
-    k_track_src_videos<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
-                                                               mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
-                                                               (int)items, max_rows, list_cap, H, W, sh, F / B);
-    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_videos");
-  }
-  if (vsums) {
     if (loss) {
       k_track_video_loss<<<1, 32 * ((B + 31) / 32), 0, s>>>(vsums, loss_weight, loss, B);
       FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_video_loss");
@@ -3945,7 +3770,7 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
                           float loss_weight, const float* grad_out, float* g_depth, float* g_extrinsics,
                           float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
                           int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream,
-                          const double* vsums = nullptr, int B = 1, const int* frame_video = nullptr) {
+                          const double* vsums = nullptr, const int* frame_video = nullptr) {
   if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !g_k4 || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_bwd: bad arguments");
@@ -3954,22 +3779,13 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
   TrackWs w = carve_track(ws, F, total_samples);
   dim3 grid((max_points + kThreads - 1) / kThreads, max_rows, num_segments);
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
-  if (vsums && frame_video) {
+  if (vsums) {  // per-video scales (track_fwd_impl); grad_out is 1 in the packed step
     k_track_apply_ragged<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
                                                              g_depth, H, W, sh, frame_video);
     FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply_ragged");
     k_track_finalize_ragged<<<(F + 63) / 64, 64, 0, s>>>(w.acc, vsums, loss_weight, extrinsics, g_extrinsics, g_k4,
                                                          F, frame_video);
     FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize_ragged");
-    return 0;
-  }
-  if (vsums) {  // per-video scales (track_fwd_impl); grad_out is 1 in the batched step
-    k_track_apply_videos<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
-                                                             g_depth, H, W, sh, F / B);
-    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply_videos");
-    k_track_finalize_videos<<<(F + 63) / 64, 64, 0, s>>>(w.acc, vsums, loss_weight, extrinsics, g_extrinsics, g_k4,
-                                                         F, F / B);
-    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize_videos");
     return 0;
   }
   k_track_apply<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, w.sums, loss_weight,
@@ -4255,21 +4071,22 @@ static SideLane* side_lane(int which = 0) {
   return l.state == 1 ? &l : nullptr;
 }
 
-// rag != NULL (fm_overfit_step_videos): videos of different lengths packed along the frame axis; a->B and
-// a->F are then ignored, and B, T come from the layout.
+// rag == NULL: one video of a->F frames.  rag != NULL (fm_overfit_step_videos): B independent videos packed
+// along the frame axis; a->B and a->F are then ignored, B and T come from the layout, and every per-video
+// scalar is an array of B values.
 static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, void* stream) {
   if (!a || !a->depth || !a->fflow || !a->bflow || !a->fmask || !a->bmask || !a->mask_sum ||
       !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 ||
-      (rag ? bad_dims(rag->B, 2, a->H, a->W) : bad_dims(a->B > 1 ? a->B : 1, a->F, a->H, a->W)))
+      (rag ? bad_dims(rag->B, 2, a->H, a->W) : bad_dims(1, a->F, a->H, a->W)))
     return fail_msg("fm_overfit_step: bad arguments");
-  // B independent videos of one shape: every per-video scalar is an array of B values
-  const int B = rag ? rag->B : a->B > 1 ? a->B : 1;
-  const bool videos = B > 1 || rag;  // per-video normalisers, losses and focal lengths
-  if (videos && (a->phase != FM_STEP_ALL || a->splat_plan))
-    return fail_msg("fm_overfit_step: B > 1 serves whole steps without a splat plan");
-  if (videos && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
-    return fail_msg("fm_overfit_step: B > 1 does not fuse the logit update of a deferred step (pass step = 0)");
-  if (videos && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step: B > 1 metrics need gt_fxfy");
+  if (!rag && a->B > 1)
+    return fail_msg("fm_overfit_step: one video per call (B = 0 or 1); several videos go to fm_overfit_step_videos");
+  const int B = rag ? rag->B : 1;
+  if (rag && (a->phase != FM_STEP_ALL || a->splat_plan))
+    return fail_msg("fm_overfit_step_videos: serves whole steps without a splat plan");
+  if (rag && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
+    return fail_msg("fm_overfit_step_videos: does not fuse the logit update of a deferred step (pass step = 0)");
+  if (rag && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step_videos: metrics need gt_fxfy");
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
@@ -4279,7 +4096,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   const int F = rag ? 0 : a->F, H = a->H, W = a->W, BP = F - 1;
   const size_t N = (size_t)H * W;
   // frames and pairs of all videos
-  const size_t TF = rag ? (size_t)rag->T : (size_t)B * F, TP = rag ? (size_t)(rag->T - B) : (size_t)B * BP;
+  const size_t TF = rag ? (size_t)rag->T : (size_t)F, TP = rag ? (size_t)(rag->T - B) : (size_t)BP;
   const int* frame_video = rag ? rag->v.frame_video : nullptr;
   Workspace w = rag ? carve_rows(a->ws, B, TF, TP) : carve(a->ws, B, F);
   int rc;
@@ -4293,12 +4110,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     if (a->focal && rag) {
       k_k4_from_focals_ragged<<<(rag->T + 63) / 64, 64, 0, s>>>(a->focal, k4, rag->T, H, W, rag->v);
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals_ragged");
-    } else if (a->focal && B == 1) {
+    } else if (a->focal) {
       k_k4_from_focal<<<(F + 63) / 64, 64, 0, s>>>(a->focal, k4, F, H, W);
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
-    } else if (a->focal) {
-      k_k4_from_focals<<<(B * F + 63) / 64, 64, 0, s>>>(a->focal, k4, B * F, F, H, W);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
     if (rag) {
@@ -4307,7 +4121,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
                                       a->indices ? nullptr : a->moments_k4, true)))
         return rc;
     } else if ((rc = procrustes_fwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                  a->indices, a->num_indices, a->rt, a->ws, B, F, H, W, stream, nullptr, plan,
+                                  a->indices, a->num_indices, a->rt, a->ws, 1, F, H, W, stream, nullptr, plan,
                                   (a->indices || plan) ? nullptr : a->moments_k4)))
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
@@ -4326,33 +4140,30 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
                                    a->delta, a->flow_weight, a->focal != nullptr, a->g_depth, w.flowacc, *rag, H, W, s)))
         return rc;
     } else if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum,
-                          a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, B, F,
-                          H, W, s, /*per_video=*/B > 1)))
+                          a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, 1, F,
+                          H, W, s)))
       return rc;
     if (rag) {
       k_flow_video_loss_ragged<<<B, 128, 0, s>>>(w.flowacc, a->loss, rag->v);
       FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss_ragged");
-    } else if (B == 1) {
+    } else {
       k_flow_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.flowacc, a->rt, a->loss, nullptr, nullptr, 1, F);
       FM_CHECK_LAUNCH("fm_overfit_step: k_flow_finalize");
-    } else {
-      k_flow_video_loss<<<B, 128, 0, s>>>(w.flowacc, a->loss, F);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss");
     }
     // LossTracking (loss_tracking.py:28-61) on the chained poses: the forward sweep belongs to the
     // forward half of a split step, its scaling / scatter to the backward half
     if (a->tracks) {
       const fm_packed_tracks* t = a->tracks;
       void* ts = fwd_lane ? (void*)fwd_lane->stream : stream;
-      if ((rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ts) : fm_pose_chain(a->rt, a->extrinsics, B, F, ts)))
+      if ((rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ts) : fm_pose_chain(a->rt, a->extrinsics, 1, F, ts)))
         return rc;
       // one focal length (or constant intrinsics) for all frames: only the summed K gradient is used.
-      // B > 1: the segments of video b start at frames b F + s (ragged: frame_offset[b] + s), and its sums
-      // go to w.track_sums[b]
+      // Several videos: the segments of video b start at frames frame_offset[b] + s, and its sums go to
+      // w.track_sums[b]
       if ((rc = track_fwd_impl(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
                                t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
                                a->track_weight, a->track_loss, a->track_ws, (int)TF, H, W, 0, 0, (int)TF, 1, ts,
-                               videos ? w.track_sums : nullptr, B, frame_video)))
+                               rag ? w.track_sums : nullptr, B, frame_video)))
         return rc;
       if (fwd_lane) {
         if ((e = cudaEventRecord(fwd_lane->join, fwd_lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -4374,7 +4185,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     }
     // the camera centres: the tracking loss chained the poses already, a flow-only step chains them here
     if (!a->tracks &&
-        (rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ms) : fm_pose_chain(a->rt, a->extrinsics, B, F, ms)))
+        (rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ms) : fm_pose_chain(a->rt, a->extrinsics, 1, F, ms)))
       return rc;
     MetricsRow row;
     row.log = a->metrics_log;
@@ -4388,13 +4199,10 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     if (rag) {
       k_metrics_ragged<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, row, a->gt_fxfy, rag->v);
       FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_ragged");
-    } else if (B == 1) {
+    } else {
       k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr,
                                                   nullptr, nullptr, row);
       FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
-    } else {
-      k_metrics_videos<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, F, row, a->gt_fxfy);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_videos");
     }
     if (mlane && (e = cudaEventRecord(mlane->join, mlane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   }
@@ -4424,11 +4232,11 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
                              t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
                              a->track_ws, (int)TF, H, W, 0, 0, (int)TF, s, apply_stream,
-                             videos ? w.track_sums : nullptr, B, frame_video)))
+                             rag ? w.track_sums : nullptr, frame_video)))
       return rc;
     if (lane && (e = cudaEventRecord(lane->join, lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
     if ((rc = rag ? pose_chain_bwd_ragged(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, *rag, stream)
-                  : fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, F, stream)))
+                  : fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, 1, F, stream)))
       return rc;
     g_rt = a->g_rt;
     track_g_k4 = a->track_g_k4;
@@ -4441,9 +4249,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   AdamFuse af;
   memset(&af, 0, sizeof(af));
   const bool defer = a->defer_adam != 0;  // softmin stage: the sweep's backward still adds gradients
-  // B > 1 with defer_adam = 1 would have to defer pair 0 of EVERY video (first_pair counts pairs of the
-  // whole batch): that step leaves the logits to the caller instead
-  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(videos && a->defer_adam == 1);
+  // several videos with defer_adam = 1 would have to defer pair 0 of EVERY video (first_pair counts pairs
+  // of the whole batch): that step leaves the logits to the caller instead
+  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(rag && a->defer_adam == 1);
   const StepClock* clock = (const StepClock*)a->clock;
   if (fuse_w) {  // the weight gradient is final inside k_distribute: update the logits there
     af.consts = clock ? &clock->step_size : nullptr;
@@ -4461,7 +4269,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
       return rc;
   } else if ((rc = procrustes_bwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
                                 a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
-                                a->g_k4, a->ws, B, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
+                                a->g_k4, a->ws, 1, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
                                 a->splat_overflow_max, /*depth_prescaled=*/fscale != nullptr)))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -4480,12 +4288,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     if (rag) {
       k_focal_grad_ragged<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, H, W, rag->v);
       FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad_ragged");
-    } else if (B == 1) {
+    } else {
       k_focal_grad<<<1, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, 1, F, H, W, fscale);
       FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
-    } else {  // whole steps only: no fscale
-      k_focal_grad_videos<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, F, H, W);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad_videos");
     }
     if (a->step > 0 && !defer) {
       const int fstep = a->focal_step > 0 ? a->focal_step : a->step;

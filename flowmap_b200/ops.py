@@ -389,19 +389,6 @@ def adam_step_clock(param: Tensor, grad: Tensor, exp_avg: Tensor, exp_avg_sq: Te
               "fm_adam_step_clock")
 
 
-def adam_step_clock_frames(param: Tensor, grad: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, lo: int, hi: int,
-                           clock: StepClock, eps: float = 1e-8) -> None:
-    """adam_step_clock on the frames lo <= f < hi of every video of a (B, F, ...) parameter, in one launch."""
-    for t in (param, grad, exp_avg, exp_avg_sq):
-        if not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous() or t.shape != param.shape:
-            raise ValueError("flowmap_b200: adam_step needs contiguous CUDA float32 tensors of one shape")
-    b, f = param.shape[:2]
-    with torch.cuda.device(param.device):
-        check(lib().fm_adam_step_clock_frames(_ptr(param), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq),
-                                              param[0, 0].numel(), b, f, lo, hi, clock.ptr, 0, clock.betas[0],
-                                              clock.betas[1], eps, _stream()), "fm_adam_step_clock_frames")
-
-
 def random_subset_clock(clock: StepClock, num_items: int, out: Tensor) -> Tensor:
     """random_subset seeded by the current tick of `clock`, into the caller's int64 buffer."""
     with torch.cuda.device(out.device):
@@ -413,20 +400,18 @@ def random_subset_clock(clock: StepClock, num_items: int, out: Tensor) -> Tensor
 class PackedTracks:
     """All segments of a list[Tracks] in the flat layout fm_track_loss_* expects.
 
-    Several videos (the batched fused step): `tracks` is a list of B such lists and `video_frames` the
-    frame count F of every video; segment s of video b is packed with start frame b * F + s.start_frame,
-    so the segments of one video address its rows of the (B * F) frame arrays and never cross videos.
-    Videos of different lengths: `video_frames` is the list of their frame counts F_b, and segment s of
-    video b is packed with start frame fo_b + s.start_frame, fo_b = F_0 + ... + F_{b-1}."""
+    Several videos (the packed fused step): `tracks` is a list of B such lists and `video_frames` the list
+    of their frame counts F_b, or one count F for videos of one length; segment s of video b is packed
+    with start frame fo_b + s.start_frame, fo_b = F_0 + ... + F_{b-1}, so the segments of one video
+    address its rows of the packed frame arrays and never cross videos."""
 
     def __init__(self, tracks, device, video_frames=None):
         videos = [tracks] if video_frames is None else tracks
-        if isinstance(video_frames, (list, tuple)):
-            if len(video_frames) != len(videos):
-                raise ValueError("flowmap_b200: one frame count per video")
-            counts = [int(n) for n in video_frames]
-        else:
-            counts = None if video_frames is None else [int(video_frames)] * len(videos)
+        if isinstance(video_frames, int):
+            video_frames = [video_frames] * len(videos)
+        counts = None if video_frames is None else [int(n) for n in video_frames]
+        if counts is not None and len(counts) != len(videos):
+            raise ValueError("flowmap_b200: one frame count per video")
         firsts = None if counts is None else [sum(counts[:b]) for b in range(len(counts))]
         segs, xy, vis, off = [], [], [], 0
         for b, video in enumerate(videos):

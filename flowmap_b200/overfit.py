@@ -4,7 +4,7 @@ sum of losses -> backward -> Adam), without the Lightning/Hydra shell.
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, fields, replace
 from typing import Optional
 
 import torch
@@ -132,6 +132,14 @@ class Overfitter:
         return total.detach(), out
 
 
+_FLOW_NAMES = ("forward", "backward", "forward_mask", "backward_mask")
+
+
+def _video(x, i: int):
+    """Video i of a Batch or Flows of several videos, as a one-video instance of the same type (views)."""
+    return replace(x, **{f.name: getattr(x, f.name)[i:i + 1] for f in fields(x) if getattr(x, f.name) is not None})
+
+
 class FusedOverfitter(Overfitter):
     """Same optimisation as :class:`Overfitter` (explicit-depth backbone, Procrustes poses,
     regressed focal length, flow [+ tracking] loss, Adam) but each step is ONE C-ABI call,
@@ -145,151 +153,80 @@ class FusedOverfitter(Overfitter):
     parity-green but has been slower per backward than the default global-RED kernel
     (tools/ab_tiled.py compares the two), hence opt-in.
 
-    Several videos: `batch.videos` of shape (B, F, 3, H, W) with B > 1 (and Flows of shape
-    (B, F-1, ...)) runs B INDEPENDENT overfits in one step.  Video b gets what a one-video
-    FusedOverfitter on video b with the same cfg and step clock seed gets: its flow loss is normalised
-    by its own mask sum, and its gradients, Adam moments, focal length, softmin window and poses are its
-    own.  training_step() returns the (B,) per-video totals, whose sum is the objective.  This differs
-    on purpose from the reference's LossFlow at b > 1 (pretraining), which normalises a batch by ONE
-    pooled mask sum.  Shared by the batch: the Procrustes point subset and the softmin point sample of
-    each step.  The parameters live in (B, ...) buffers; `models[b]` is video b's Model, whose
-    parameters are views into them.  `tracks` is then a list of B segment lists (one per video; its
-    tracking loss is normalised by its own valid count), and the metrics log holds (steps, B) values.
-    B > 1 does not serve the splat plan.
+    Several videos run B INDEPENDENT overfits in one step (fm_overfit_step_videos).  Video b gets what a
+    one-video FusedOverfitter on video b with the same cfg and step clock seed gets: its flow loss is
+    normalised by its own mask sum, its tracking loss by its own valid count, and its gradients, Adam
+    moments, focal length, softmin window and poses are its own.  training_step() returns the (B,)
+    per-video totals, whose sum is the objective.  This differs on purpose from the reference's LossFlow
+    at b > 1 (pretraining), which normalises a batch by ONE pooled mask sum.  Shared by the batch: the
+    Procrustes point subset and the softmin point sample of each step.  The parameters live in packed
+    (T, H, W) / (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs
+    [fo_b - b, fo_b - b + F_b - 1); `models[b]` is video b's Model, whose parameters are views into them.
+    `tracks` is then a list of B segment lists, and the metrics log holds (steps, B) values.  Several
+    videos do not serve the splat plan, pair sharding or the split-step surface.  Two forms:
 
-    Videos of different lengths (same H, W): `batch` a list of B one-video Batches, `flows` a list of their
-    Flows (1, F_b - 1, ...) and, with tracking, `tracks` a list of per-video segment lists.  The same B
-    independent overfits in one step (fm_overfit_step_videos); the parameters live in packed (T, H, W) /
-    (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs [fo_b - b, fo_b - b +
-    F_b - 1).  `models[b]` is a Model of F_b frames whose parameters are views into them.  training_step()
-    returns the (B,) totals and a list of the videos' relative poses; extrinsics(), intrinsics_k4() and
-    gradients() hand out per-video lists."""
+    - `batch.videos` of shape (B, F, 3, H, W) with B > 1 and Flows of shape (B, F-1, ...): videos of one
+      length, whose packed buffers are the (B, F, ...) / (B, F-1, ...) tensors.  training_step(),
+      extrinsics(), intrinsics_k4() and gradients() hand out (B, F [- 1], ...) views, and set_flows takes
+      one (B, F-1, ...) Flows.
+    - `batch` a list of B one-video Batches of the same H, W, `flows` a list of their Flows (1, F_b - 1, ...):
+      videos of different lengths.  training_step() returns the (B,) totals and a list of the videos'
+      relative poses; extrinsics(), intrinsics_k4() and gradients() hand out per-video lists."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):
-        self._layout = None
+        self._layout, self._tensor_batch = None, False
         if isinstance(batch, (list, tuple)):
             self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
-            return
-        b, f, _, h, w = batch.videos.shape
-        if b > 1:
+        elif batch.videos.shape[0] > 1:
+            b, f = batch.videos.shape[:2]
             if model is not None:
                 raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
             if use_splat_plan:
                 raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
             if tracks is not None and len(tracks) != b:
                 raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({b})")
-            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+            for name in _FLOW_NAMES:
                 if tuple(getattr(flows, name).shape[:2]) != (b, f - 1):
                     raise ValueError(f"flowmap_b200: flows.{name} must hold (B, F-1) = ({b}, {f - 1}) pairs")
-        super().__init__(cfg, batch, flows, tracks if b == 1 else None, device, model=model)
-        from ._lib import OverfitStepArgs, PackedTracksC, lib
-        import ctypes
-        self.B = b
-        if b > 1 and tracks is not None:
-            self.tracks = [[t.to(device) for t in video] for video in tracks]
+            batch = batch.to(device)
+            self._init_videos(cfg, [_video(batch, i) for i in range(b)], [_video(flows, i) for i in range(b)],
+                              tracks, device, False, None)
+            self._tensor_batch, self.batch = True, batch
+        else:
+            self._init_one(cfg, batch, flows, tracks, device, use_splat_plan, model)
+        self._init_step(cfg)
+        if self._tensor_batch:  # the parameters as (B, F, ...) / (B, F-1, ...) views of the packed buffers
+            self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
+
+    def _init_one(self, cfg, batch, flows, tracks, device, use_splat_plan, model):
+        """The one-video optimiser: its parameters are the Model's own tensors."""
+        super().__init__(cfg, batch, flows, tracks, device, model=model)
+        _, f, _, h, w = batch.videos.shape
         # the kernels read raw pointers: canonical (contiguous float32) copies, kept alive here
         # (FlowPredictor.rescale_flow returns a permuted view, flow_predictor.py:40-49)
-        self.flows = Flows(*(ops._canon(getattr(self.flows, n), n)
-                             for n in ("forward", "backward", "forward_mask", "backward_mask")))
+        self.flows = Flows(*(ops._canon(getattr(self.flows, n), n) for n in _FLOW_NAMES))
         dev = self.flows.forward.device
+        self.B, self.frames, self.T, self._hw = 1, [f], f, (h, w)
+        self._lead = ((1, f), (1, f - 1), ())  # leading dims of the per-frame, per-pair and per-video buffers
+        self._track_frames = None
         self._use_plan = use_splat_plan and cfg.procrustes_points is None and not cfg.procrustes_randomize
         self._plan = ops.SplatPlan(self.flows.backward) if self._use_plan else None
-        self._softmin = cfg.intrinsics == "softmin"
         self.models = [self.model]
-        if b > 1:  # sets _depth, _wlog and (where it is a parameter) _focal
-            self.models += [build_model_and_losses(cfg, f, (h, w))[0].to(device) for _ in range(b - 1)]
-            self._bind_batched_parameters()
+        self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
+        intr = self.model.intrinsics
+        if cfg.intrinsics != "softmin":
+            self._focal = intr.focal_length.data
+        elif cfg.regression_after is not None:
+            self._focal = intr.intrinsics_regressed.focal_length.data
         else:
-            self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
-        if self._softmin:
-            intr = self.model.intrinsics
-            if b == 1:
-                self._focal = (intr.intrinsics_regressed.focal_length.data if cfg.regression_after
-                               is not None else torch.zeros((), device=dev))
-            elif cfg.regression_after is None:
-                self._focal = torch.zeros(b, device=dev)
-            n = cfg.softmin_candidates
-            self._cand_f = intr.focal_length_candidates.float().contiguous()
-            self._cand_k4 = ops.candidate_k4(self._cand_f, h, w, b)
-            self._sw_err = torch.empty(b, n, device=dev)
-            self._sw_sm = torch.empty(b, n, device=dev)
-            self._sw_gerr = torch.empty(b, n, device=dev)
-            self._sw_rt = torch.empty(b * n, 3, 4, device=dev)
-            self._sw_focal = torch.zeros(b, device=dev)
-            self._sw_ws = torch.empty(lib().fm_softmin_workspace_bytes(b, n), dtype=torch.uint8,
-                                      device=dev)
-            # candidate 0's intrinsics for every frame: what the early moment pass of a sweep step uses
-            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(b * f, 4).contiguous()
-            self.window = []
-            self.injected_indices = None
-        elif b == 1:
-            self._focal = self.model.intrinsics.focal_length.data
-        z = lambda t: torch.zeros_like(t)  # noqa: E731
-        self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog),
-                       z(self._focal), z(self._focal)]
-        self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
-        self._g_focal = torch.zeros_like(self._focal)
-        self._k4 = torch.empty(b * f, 4, device=dev)
-        self._g_k4 = torch.empty(b * f, 4, device=dev)
-        self.rt = torch.empty(b, f - 1, 3, 4, device=dev)
-        self._loss = torch.zeros(() if b == 1 else (b,), device=dev)
-        self._track_loss = torch.zeros_like(self._loss)
-        self._ws = ops.workspace(b, f, h, w, dev)
-        self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask) if b == 1 else \
-            self._video_mask_sums(self.flows)
-        self._indices = self.model.extrinsics.select_indices(h, w, dev) \
-            if not cfg.procrustes_randomize else None
-        a = OverfitStepArgs()
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        a.F, a.H, a.W, a.B = f, h, w, b
-        a.depth = P(self._depth)
-        a.weight_logits = P(self._wlog) if cfg.use_correspondence_weights else None
-        a.weight_sensitivity = cfg.weight_sensitivity
-        a.focal, a.k4 = P(self._focal), P(self._k4)
-        a.fflow, a.bflow = P(self.flows.forward), P(self.flows.backward)
-        a.fmask, a.bmask = P(self.flows.forward_mask), P(self.flows.backward_mask)
-        a.mask_sum = P(self._msum)
-        a.mapping, a.delta, a.flow_weight = ops.MAPPINGS[cfg.mapping], cfg.delta, cfg.flow_weight
-        (a.m_depth, a.v_depth, a.m_weights, a.v_weights, a.m_focal, a.v_focal) = \
-            [P(t) for t in self._state]
-        a.lr, a.beta1, a.beta2, a.eps = cfg.lr, 0.9, 0.999, 1e-8
-        a.g_depth, a.g_weights, a.g_focal, a.g_k4 = P(self._g_depth), P(self._g_w), \
-            P(self._g_focal), P(self._g_k4)
-        a.rt, a.loss, a.ws = P(self.rt), P(self._loss), P(self._ws)
-        # step-dependent scalars live in device memory: every step is the same launch sequence
-        self._clock = ops.StepClock(dev, cfg.lr)
-        self._side_stream = torch.cuda.Stream(device=dev)  # parallel branch of the step (see _step_softmin)
-        a.clock = self._clock.ptr
-        self._total = torch.zeros_like(self._loss)
-        self._idx_buf = torch.empty(min(cfg.softmin_points, h * w), dtype=torch.int64, device=dev) \
-            if self._softmin else None
-        self.use_cuda_graph = False  # opt-in: replay the update step as ONE CUDA graph launch
-        self._graphs, self._eager_runs = {}, {}
-        self._set_plan_args(a)
-        self._packed = None
-        if cfg.use_tracking:
-            assert self.tracks is not None
-            pk = ops.PackedTracks(self.tracks, dev, f if b > 1 else None)
-            self._packed = pk
-            self._pk_c = PackedTracksC(P(pk.seg), P(pk.xy), P(pk.vis), pk.num_segments,
-                                       pk.max_rows, pk.max_points, pk.total)
-            self._ext = torch.empty(b, f, 4, 4, device=dev)
-            self._g_ext = torch.empty(b, f, 4, 4, device=dev)
-            self._g_rt = torch.empty(b, f - 1, 3, 4, device=dev)
-            self._tg_k4 = torch.empty(b * f, 4, device=dev)
-            self._tws = torch.empty(lib().fm_track_workspace_bytes(b * f, pk.total), dtype=torch.uint8,
-                                    device=dev)
-            a.track_weight = cfg.tracking_weight
-            a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
-            a.track_g_k4, a.track_loss, a.track_ws = P(self._tg_k4), P(self._track_loss), P(self._tws)
-        self._args, self._ctypes = a, ctypes
-        self._lib = lib()
-        self._mlog = None  # per-step metrics ring (enable_metrics_log)
+            self._focal = torch.zeros((), device=dev)
+        self._ws = ops.workspace(1, f, h, w, dev)
+        self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
 
     def _init_videos(self, cfg, batches, flows, tracks, device, use_splat_plan, model):
-        """The packed optimiser of videos of different lengths (see the class docstring)."""
-        from ._lib import OverfitStepArgs, PackedTracksC, VideoLayout, lib
+        """The packed optimiser of several videos (see the class docstring)."""
+        from ._lib import VideoLayout, lib
         import ctypes
         if model is not None:
             raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
@@ -309,7 +246,7 @@ class FusedOverfitter(Overfitter):
                 raise ValueError("flowmap_b200: the videos of one step need the same H x W")
             if f < 2:
                 raise ValueError(f"flowmap_b200: video {i} has {f} frame(s), a pair needs 2")
-            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+            for name in _FLOW_NAMES:
                 t = getattr(flows[i], name)
                 if tuple(t.shape[:4]) != (1, f - 1, h, w):
                     raise ValueError(f"flowmap_b200: flows[{i}].{name} must hold (1, F_b-1, H, W) = (1, {f - 1}, {h}, {w})")
@@ -320,6 +257,8 @@ class FusedOverfitter(Overfitter):
         self.T, self.P = sum(frames), sum(frames) - B
         self._first = [sum(frames[:i]) for i in range(B)]
         self._hw = (h, w)
+        self._lead = ((self.T,), (self.P,), (B,))
+        self._track_frames = frames
         self.batches = [bt.to(device) for bt in batches]
         self.batch = self.batches[0]
         self.tracks = None if tracks is None else [[t.to(device) for t in v] for v in tracks]
@@ -329,7 +268,7 @@ class FusedOverfitter(Overfitter):
         self.model, self.losses, self.optimizer = self.models[0], built[0][1], None
         # packed flows: the pairs of video b follow those of video b - 1
         self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(dev), n)[0] for fl in flows]).contiguous()
-                             for n in ("forward", "backward", "forward_mask", "backward_mask")))
+                             for n in _FLOW_NAMES))
         fo = torch.tensor(self._first + [self.T], dtype=torch.int32)
         self._tables = (fo.to(dev),
                         torch.repeat_interleave(torch.arange(B, dtype=torch.int32), torch.tensor(frames)).to(dev),
@@ -337,7 +276,6 @@ class FusedOverfitter(Overfitter):
         self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
         self._layout_ref = ctypes.byref(self._layout)
         self._use_plan, self._plan = False, None
-        self._softmin = cfg.intrinsics == "softmin"
 
         def pack(params):
             buf = torch.cat([p.data for p in params]).contiguous()
@@ -354,12 +292,24 @@ class FusedOverfitter(Overfitter):
             return buf
         self._depth = pack([m.backbone.depth for m in self.models])
         self._wlog = pack([m.backbone.weights for m in self.models])
-        if not self._softmin:
+        if cfg.intrinsics != "softmin":
             self._focal = stack([m.intrinsics.focal_length for m in self.models])
         elif cfg.regression_after is not None:
             self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
         else:
             self._focal = torch.zeros(B, device=dev)
+        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
+        self._msum = self._video_mask_sums(self.flows)
+
+    def _init_step(self, cfg):
+        """What one video and packed videos wire alike: the softmin buffers, the Adam state, the gradient
+        and output buffers, the args struct, the step clock and the tracking buffers."""
+        from ._lib import OverfitStepArgs, PackedTracksC, lib
+        import ctypes
+        (h, w), B, T = self._hw, self.B, self.T
+        frame_dims, pair_dims, video_dims = self._lead
+        dev = self.flows.forward.device
+        self._softmin = cfg.intrinsics == "softmin"
         if self._softmin:
             n = cfg.softmin_candidates
             self._cand_f = self.model.intrinsics.focal_length_candidates.float().contiguous()
@@ -368,23 +318,22 @@ class FusedOverfitter(Overfitter):
             self._sw_rt = torch.empty(B * n, 3, 4, device=dev)
             self._sw_focal = torch.zeros(B, device=dev)
             self._sw_ws = torch.empty(lib().fm_softmin_workspace_bytes(B, n), dtype=torch.uint8, device=dev)
-            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(self.T, 4).contiguous()
+            # candidate 0's intrinsics for every frame: what the early moment pass of a sweep step uses
+            self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(T, 4).contiguous()
             self.window = []
             self.injected_indices = None
         z = lambda t: torch.zeros_like(t)  # noqa: E731
         self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog), z(self._focal), z(self._focal)]
         self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
         self._g_focal = torch.zeros_like(self._focal)
-        self._k4, self._g_k4 = torch.empty(self.T, 4, device=dev), torch.empty(self.T, 4, device=dev)
-        self.rt = torch.empty(self.P, 3, 4, device=dev)
-        self._loss = torch.zeros(B, device=dev)
+        self._k4, self._g_k4 = torch.empty(T, 4, device=dev), torch.empty(T, 4, device=dev)
+        self.rt = torch.empty(*pair_dims, 3, 4, device=dev)
+        self._loss = torch.zeros(video_dims, device=dev)
         self._track_loss = torch.zeros_like(self._loss)
-        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
-        self._msum = self._video_mask_sums(self.flows)
         self._indices = self.model.extrinsics.select_indices(h, w, dev) if not cfg.procrustes_randomize else None
         a = OverfitStepArgs()
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        a.F, a.H, a.W, a.B = 0, h, w, B  # F: ignored by fm_overfit_step_videos
+        a.F, a.H, a.W = T if self._layout is None else 0, h, w  # F: ignored by fm_overfit_step_videos
         a.depth = P(self._depth)
         a.weight_logits = P(self._wlog) if cfg.use_correspondence_weights else None
         a.weight_sensitivity = cfg.weight_sensitivity
@@ -397,42 +346,40 @@ class FusedOverfitter(Overfitter):
         a.lr, a.beta1, a.beta2, a.eps = cfg.lr, 0.9, 0.999, 1e-8
         a.g_depth, a.g_weights, a.g_focal, a.g_k4 = P(self._g_depth), P(self._g_w), P(self._g_focal), P(self._g_k4)
         a.rt, a.loss, a.ws = P(self.rt), P(self._loss), P(self._ws)
+        # step-dependent scalars live in device memory: every step is the same launch sequence
         self._clock = ops.StepClock(dev, cfg.lr)
-        self._side_stream = torch.cuda.Stream(device=dev)
+        self._side_stream = torch.cuda.Stream(device=dev)  # parallel branch of the step (see _step_softmin)
         a.clock = self._clock.ptr
         self._total = torch.zeros_like(self._loss)
         self._idx_buf = torch.empty(min(cfg.softmin_points, h * w), dtype=torch.int64, device=dev) \
             if self._softmin else None
-        self.use_cuda_graph = False
+        self.use_cuda_graph = False  # opt-in: replay the update step as ONE CUDA graph launch
         self._graphs, self._eager_runs = {}, {}
         self._set_plan_args(a)
         self._packed = None
         if cfg.use_tracking:
-            pk = ops.PackedTracks(self.tracks, dev, frames)
+            assert self.tracks is not None
+            pk = ops.PackedTracks(self.tracks, dev, self._track_frames)
             self._packed = pk
             self._pk_c = PackedTracksC(P(pk.seg), P(pk.xy), P(pk.vis), pk.num_segments, pk.max_rows, pk.max_points,
                                        pk.total)
-            self._ext = torch.empty(self.T, 4, 4, device=dev)
-            self._g_ext = torch.empty(self.T, 4, 4, device=dev)
-            self._g_rt = torch.empty(self.P, 3, 4, device=dev)
-            self._tg_k4 = torch.empty(self.T, 4, device=dev)
-            self._tws = torch.empty(lib().fm_track_workspace_bytes(self.T, pk.total), dtype=torch.uint8, device=dev)
+            self._ext = torch.empty(*frame_dims, 4, 4, device=dev)
+            self._g_ext = torch.empty(*frame_dims, 4, 4, device=dev)
+            self._g_rt = torch.empty(*pair_dims, 3, 4, device=dev)
+            self._tg_k4 = torch.empty(T, 4, device=dev)
+            self._tws = torch.empty(lib().fm_track_workspace_bytes(T, pk.total), dtype=torch.uint8, device=dev)
             a.track_weight = cfg.tracking_weight
             a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
             a.track_g_k4, a.track_loss, a.track_ws = P(self._tg_k4), P(self._track_loss), P(self._tws)
         self._args, self._ctypes = a, ctypes
         self._lib = lib()
-        self._mlog = None
-
-    def _dims(self):
-        """(B, F, H, W); with videos of different lengths F is the longest video's frame count."""
-        if self._layout is not None:
-            return self.B, max(self.frames), self._hw[0], self._hw[1]
-        b, f, _, h, w = self.batch.videos.shape
-        return b, f, h, w
+        self._mlog = None  # per-step metrics ring (enable_metrics_log)
 
     def _per_video(self, t: Tensor, pairs: bool = False):
-        """Views of a packed (T, ...) / (T - B, ...) buffer, one per video."""
+        """Views of a packed (T, ...) / (T - B, ...) buffer, one per video: a (B, F [- 1], ...) view for a
+        tensor batch, else a list."""
+        if self._tensor_batch:
+            return t.view(self.B, -1, *t.shape[1:])
         return [t[f0 - pairs * i:f0 - pairs * i + f - pairs] for i, (f0, f) in enumerate(zip(self._first, self.frames))]
 
     def _call_step(self, what: str = "fm_overfit_step"):
@@ -452,12 +399,15 @@ class FusedOverfitter(Overfitter):
     def set_flows(self, flows: Flows, mask_sum: Optional[Tensor] = None):
         """Point the step at another device-resident Flows of the same shape (the next batch of a
         prefetching loader) without rebuilding parameters or optimiser state.  `mask_sum` is the
-        flow-loss normaliser (loss_flow.py:70) if the caller already has it.  Videos of different
-        lengths: a list of one Flows per video, copied into the packed buffers."""
+        flow-loss normaliser (loss_flow.py:70) if the caller already has it.  Several videos: the new
+        flows are copied into the packed buffers, from one (B, F-1, ...) Flows for a tensor batch, else
+        from a list of one Flows per video."""
         if self._layout is not None:
+            if self._tensor_batch and isinstance(flows, Flows):
+                flows = [_video(flows, i) for i in range(flows.forward.shape[0])]
             if not isinstance(flows, (list, tuple)) or len(flows) != self.B:
                 raise ValueError(f"flowmap_b200: set_flows needs one Flows per video ({self.B})")
-            for name in ("forward", "backward", "forward_mask", "backward_mask"):
+            for name in _FLOW_NAMES:
                 dst = self._per_video(getattr(self.flows, name), pairs=True)
                 for i, fl in enumerate(flows):
                     t = ops._canon(getattr(fl, name), name)
@@ -468,7 +418,7 @@ class FusedOverfitter(Overfitter):
             return
         old = self.flows
         canon = {}
-        for name in ("forward", "backward", "forward_mask", "backward_mask"):
+        for name in _FLOW_NAMES:
             t = ops._canon(getattr(flows, name), name)
             if t.shape != getattr(old, name).shape or t.device != getattr(old, name).device:
                 raise ValueError(f"flowmap_b200: `{name}` does not match the optimiser's shapes / device")
@@ -486,51 +436,31 @@ class FusedOverfitter(Overfitter):
         self._eager_runs.clear()
 
     def _mask_sum(self, flows: Flows) -> Tensor:
-        if self.B > 1:
-            return self._video_mask_sums(flows)
         return ops.mask_sum(flows.forward_mask, flows.backward_mask)
 
     def _video_mask_sums(self, flows: Flows) -> Tensor:
         """(B,) float64: each video's own flow-loss normaliser."""
-        fm, bm = flows.forward_mask, flows.backward_mask
-        if self._layout is not None:
-            fm, bm = self._per_video(fm, pairs=True), self._per_video(bm, pairs=True)
-        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(len(fm))])
-
-    def _bind_batched_parameters(self):
-        """B > 1: the videos' parameters move into (B, ...) buffers that the step updates in place; each
-        video's Model keeps views of its rows, so state_dict() and the exports read them without a copy."""
-        def stack(params):
-            buf = torch.stack([p.data for p in params]).contiguous()
-            for i, p in enumerate(params):
-                p.data = buf[i]
-            return buf
-        self._depth = stack([m.backbone.depth for m in self.models])
-        self._wlog = stack([m.backbone.weights for m in self.models])
-        if self.cfg.intrinsics != "softmin":
-            self._focal = stack([m.intrinsics.focal_length for m in self.models])
-        elif self.cfg.regression_after is not None:
-            self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
+        fm, bm = self._per_video(flows.forward_mask, pairs=True), self._per_video(flows.backward_mask, pairs=True)
+        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(self.B)])
 
     def _adam_frames(self, i: int, lo: int, hi: int):
-        """Adam (step clock) on frames lo <= f < hi of every video of parameter i (0 depth, 1 weight logits)."""
+        """Adam (step clock) on frames lo <= f < hi of parameter i (0 depth, 1 weight logits); several videos:
+        on the frames (pairs) lo <= r < min(hi, F_b (- 1)) of every video."""
         p, g = ((self._depth, self._g_depth), (self._wlog, self._g_w))[i]
         m, v = self._state[2 * i], self._state[2 * i + 1]
-        if self._layout is not None:  # frames (pairs) lo <= r < min(hi, F_b (- 1)) of every video
-            from ._lib import check
-            with torch.cuda.device(p.device):
-                check(self._lib.fm_adam_step_clock_frames_videos(
-                    p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p[0].numel(), self._layout_ref, i, lo, hi,
-                    self._clock.ptr, 0, self._clock.betas[0], self._clock.betas[1], 1e-8,
-                    torch.cuda.current_stream().cuda_stream), "fm_adam_step_clock_frames_videos")
-        elif self.B == 1:
+        if self._layout is None:
             ops.adam_step_clock(p[lo:hi], g[lo:hi], m[lo:hi], v[lo:hi], self._clock)
-        else:
-            ops.adam_step_clock_frames(p, g, m, v, lo, hi, self._clock)
+            return
+        from ._lib import check
+        with torch.cuda.device(p.device):
+            check(self._lib.fm_adam_step_clock_frames_videos(
+                p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), g[0].numel(), self._layout_ref, i, lo, hi,
+                self._clock.ptr, 0, self._clock.betas[0], self._clock.betas[1], 1e-8,
+                torch.cuda.current_stream().cuda_stream), "fm_adam_step_clock_frames_videos")
 
     def _window_entry(self) -> Tensor:
-        """The sweep's focal estimate for the hand-over window: a scalar, or (B,) for B videos."""
-        return self._sw_focal[0].clone() if self.B == 1 and self._layout is None else self._sw_focal.clone()
+        """The sweep's focal estimate for the hand-over window: a scalar, or (B,) for several videos."""
+        return self._sw_focal[0].clone() if self._layout is None else self._sw_focal.clone()
 
     def _softmin_stage(self) -> bool:
         c = self.cfg
@@ -542,7 +472,7 @@ class FusedOverfitter(Overfitter):
         the step itself with that focal length, the sweep's backward, then Adam."""
         from ._lib import check
         c, a, L = self.cfg, self._args, self._lib
-        b, f, h, w = self._dims()
+        b, f, (h, w) = self.B, max(self.frames), self._hw
         dev = self.rt.device
         st = torch.cuda.current_stream().cuda_stream
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
@@ -563,8 +493,8 @@ class FusedOverfitter(Overfitter):
                                                          sens, P(self._ws), self._layout_ref, h, w, st),
                           "fm_procrustes_moments_videos")
                 else:
-                    check(L.fm_procrustes_moments_batched(P(self._depth), P(self._k4_base), P(self.flows.backward),
-                                                          wl, sens, P(self._ws), b, f, h, w, st), "fm_procrustes_moments")
+                    check(L.fm_procrustes_moments(P(self._depth), P(self._k4_base), P(self.flows.backward), wl, sens,
+                                                  P(self._ws), f, h, w, st), "fm_procrustes_moments")
             with torch.cuda.stream(self._side_stream if early_moments else cur):
                 sst = torch.cuda.current_stream().cuda_stream
                 idx = self.injected_indices
@@ -592,8 +522,7 @@ class FusedOverfitter(Overfitter):
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
             # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
-            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and b == 1 and \
-                not rag
+            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and not rag
             a.focal = P(self._sw_focal)
             a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
             a.defer_adam = 1 if fuse else 0
@@ -743,7 +672,7 @@ class FusedOverfitter(Overfitter):
 
     def _refuse_videos(self, what: str):
         if self._layout is not None:
-            raise ValueError(f"flowmap_b200: {what} serves one video, not videos of different lengths")
+            raise ValueError(f"flowmap_b200: {what} serves one video, not several")
 
     def _step_body(self, update: bool, track_on: bool, sweep: bool):
         """One step as a fixed launch sequence (no host-side step numbers: see ops.StepClock)."""
@@ -793,11 +722,10 @@ class FusedOverfitter(Overfitter):
 
     def training_step(self, update: bool = True):
         """Returns (total loss (device tensor: a scalar, or the (B,) per-video totals), relative poses
-        rt (B, F-1, 3, 4))."""
+        rt (B, F-1, 3, 4), or a list of (F_b - 1, 3, 4) for videos of different lengths)."""
         c, a = self.cfg, self._args
         if c.procrustes_randomize:
-            _, _, h, w = self._dims()
-            self._indices = self.model.extrinsics.select_indices(h, w, self.rt.device)
+            self._indices = self.model.extrinsics.select_indices(*self._hw, self.rt.device)
         a.indices = None if self._indices is None else self._indices.data_ptr()
         a.num_indices = 0 if self._indices is None else self._indices.numel()
         track_on = c.use_tracking and self.global_step >= c.tracking_enable_after
@@ -824,24 +752,22 @@ class FusedOverfitter(Overfitter):
         return self._total.clone(), self.rt
 
     def extrinsics(self) -> Tensor:
-        """Camera-to-world poses of the last step (projection.py:187-210); a list of (F_b, 4, 4) for videos
-        of different lengths."""
-        if self._layout is not None:
-            return [ops.pose_chain(r[None])[0] for r in self._per_video(self.rt, pairs=True)]
-        return ops.pose_chain(self.rt)
+        """Camera-to-world poses of the last step (projection.py:187-210): (B, F, 4, 4), or a list of
+        (F_b, 4, 4) for videos of different lengths."""
+        if self._layout is None or self._tensor_batch:
+            return ops.pose_chain(self.rt if self._layout is None else self._per_video(self.rt, pairs=True))
+        return [ops.pose_chain(r[None])[0] for r in self._per_video(self.rt, pairs=True)]
 
     def gradients(self):
-        if self._layout is not None:  # per-video views
-            return {"depth": self._per_video(self._g_depth), "weights": self._per_video(self._g_w, pairs=True),
-                    "focal": list(self._g_focal.unbind())}
-        return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
+        if self._layout is None:
+            return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
+        return {"depth": self._per_video(self._g_depth), "weights": self._per_video(self._g_w, pairs=True),
+                "focal": self._g_focal if self._tensor_batch else list(self._g_focal.unbind())}
 
     def intrinsics_k4(self) -> Tensor:
-        """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for B videos; a list of (F_b, 4) for
-        videos of different lengths."""
-        if self._layout is not None:
-            return self._per_video(self._k4)
-        return self._k4 if self.B == 1 else self._k4.view(self.B, -1, 4)
+        """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for a (B, F) tensor batch; a list of
+        (F_b, 4) for videos of different lengths."""
+        return self._k4 if self._layout is None else self._per_video(self._k4)
 
     METRIC_NAMES = ("train/loss/flow", "train/loss/tracking", "train/intrinsics/fx_error",
                     "train/intrinsics/fy_error", "metrics/ate")
@@ -862,9 +788,9 @@ class FusedOverfitter(Overfitter):
         if capacity < 1:
             raise ValueError("flowmap_b200: the metrics log needs a capacity >= 1")
         b, dev, B = self.batch, self.rt.device, self.B
-        _, f, _, _, _ = b.videos.shape
         nan = float("nan")
-        if self._layout is not None:  # each video's own Batch; the camera centres packed like the frames
+        one = self._layout is None
+        if not one:  # each video's own Batch; the camera centres packed like the frames
             gts, fxfy = [], []
             for bt, fb in zip(self.batches, self.frames):
                 gts.append(torch.full((fb, 3), nan, device=dev) if bt.extrinsics is None else
@@ -875,8 +801,7 @@ class FusedOverfitter(Overfitter):
             self._mlog_gt = torch.cat(gts).contiguous()
             self._mlog_fxfy = torch.stack(fxfy).to(device=dev, dtype=torch.float32).contiguous()
             fx = fy = nan
-            f = self.T
-        elif B == 1:
+        else:
             self._mlog_gt = None if b.extrinsics is None else \
                 b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
             if b.intrinsics is None:
@@ -884,17 +809,8 @@ class FusedOverfitter(Overfitter):
             else:
                 k = b.intrinsics[0].double()
                 fx, fy = float(k[:, 0, 0].mean()), float(k[:, 1, 1].mean())
-        else:  # per video; a video whose ground truth is NaN gets NaN columns
-            self._mlog_gt = None if b.extrinsics is None else \
-                b.extrinsics[:, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
-            self._mlog_fxfy = torch.full((B, 2), nan) if b.intrinsics is None else \
-                torch.stack((b.intrinsics[:, :, 0, 0].double().mean(1), b.intrinsics[:, :, 1, 1].double().mean(1)), 1)
-            self._mlog_fxfy = self._mlog_fxfy.to(device=dev, dtype=torch.float32).contiguous()
-            fx = fy = nan
-        one = B == 1 and self._layout is None
         if getattr(self, "_ext", None) is None:  # flow-only steps chain the poses for the log
-            self._ext = torch.empty(B, f, 4, 4, device=dev) if self._layout is None else \
-                torch.empty(self.T, 4, 4, device=dev)
+            self._ext = torch.empty(*self._lead[0], 4, 4, device=dev)
         self._mlog = torch.full((capacity, 5) if one else (capacity, B, 5), nan, device=dev)
         self._mlog_first = self.optimizer_steps
         a = self._args
@@ -938,7 +854,6 @@ class ShardedFusedOverfitter(FusedOverfitter):
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, plan, tracks=None, device="cuda",
                  group=None):
-        from dataclasses import replace
         from . import parallel
         from ._lib import lib
         if isinstance(batch, (list, tuple)) or batch.videos.shape[0] != 1:

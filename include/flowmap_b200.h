@@ -246,12 +246,6 @@ int fm_step_clock_tick(void* clock, double lr, double beta1, double beta2, unsig
 int fm_adam_step_clock(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t count,
                        const void* clock, int focal_clock, double beta1, double beta2, double eps, void* stream);
 int fm_random_subset_clock(const void* clock, long long N, int n, int64_t* out, void* stream);
-/* fm_adam_step_clock on the frames frame_lo <= f < frame_hi of each video of a (B, F, frame_elems)
- * parameter: one launch for the same frames of every video (the batched step's softmin stage, where the
- * sweep still adds to frames 0 / 1 of each video while the others are final). */
-int fm_adam_step_clock_frames(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, size_t frame_elems,
-                              int B, int F, int frame_lo, int frame_hi, const void* clock, int focal_clock,
-                              double beta1, double beta2, double eps, void* stream);
 
 /* intrinsics_softmin.py:84-131, the candidate sweep on the first frame pair.  For each of
  * the num_candidates intrinsics in cand_k4 (B*num_candidates, 2, 4: one k4 row per virtual
@@ -370,19 +364,11 @@ typedef struct {
   float gt_fx, gt_fy;            /* frame means of the normalised GT intrinsics, NaN: columns NaN */
   float* metrics_log;            /* (metrics_capacity, 5) ring, or NULL = off */
   int metrics_capacity;
-  /* Number of videos (0 or 1: one).  B > 1 optimises B independent videos of the same (F, H, W) in one
-     step: every per-frame / per-pair buffer above has the (B, F, ...) / (B, F-1, ...) layout, and focal,
-     mask_sum, loss, track_loss, g_focal, m_focal and v_focal hold B values.  Video b's flow loss is
-     normalised by its own mask_sum[b] and its tracking loss by its own valid count ("or 1" per video);
-     its gradients are those of a one-video step on video b.  (The reference's LossFlow normalises a batch
-     by ONE pooled mask sum; this is B overfit runs, not a pooled batch.)  Tracks: the segments of video b
-     carry start frames b * F + s (they never cross videos); track_ws is fm_track_workspace_bytes(B * F,
-     total_samples).  The metrics ring is (metrics_capacity, B, 5), gt_positions (B, F, 3) with a NaN
-     first position for a video without ground truth.  B > 1 needs phase FM_STEP_ALL and no splat plan,
-     and refuses defer_adam = 1 together with step > 0 and weight logits (the caller updates the logits
-     after the sweep's backward). */
+  /* 0 or 1; fm_overfit_step_videos ignores it.  fm_overfit_step optimises one video and refuses B > 1:
+     several videos go to fm_overfit_step_videos. */
   int B;
-  const float* gt_fxfy;          /* B > 1 with metrics_log: (B, 2) frame means of the GT intrinsics, NaN: none */
+  const float* gt_fxfy;          /* fm_overfit_step_videos with metrics_log: (B, 2) frame means of the GT
+                                    intrinsics, NaN: none */
 } fm_overfit_step_args;
 #define FM_STEP_ALL 0
 #define FM_STEP_FORWARD 1
@@ -395,7 +381,7 @@ typedef struct {
  * parallel branches of the caller's graph. */
 int fm_overfit_step(const fm_overfit_step_args* args, void* stream);
 
-/* Videos of different lengths (same H, W), packed along the frame axis: video b owns the frames
+/* Several videos (same H, W; equal or different lengths), packed along the frame axis: video b owns the frames
  * [frame_offset[b], frame_offset[b + 1]) of every per-frame buffer (T, ...) and the pairs
  * [frame_offset[b] - b, frame_offset[b + 1] - b - 1) of every per-pair buffer (P, ...), P = T - B; no pair
  * crosses two videos.  The three tables live in device memory and belong to the caller, who keeps them
@@ -407,17 +393,20 @@ typedef struct {
   const int* frame_video;   /* (T) the video of every frame */
   const int* pair_video;    /* (T - B) the video of every pair */
 } fm_video_layout;
-/* fm_overfit_step for videos of different lengths: args->B and args->F are ignored, every per-frame /
+/* fm_overfit_step for B independent videos in one step: args->B and args->F are ignored, every per-frame /
  * per-pair buffer has the packed layout above, and the per-video scalars (focal, mask_sum, loss,
- * track_loss, g_focal, m_focal, v_focal) hold B values, as with args->B > 1.  Video b gets what a
- * one-video step on it gets; its poses chain from the identity at its own frame 0.  Tracks: the segments
- * of video b carry start frames frame_offset[b] + s; track_ws is fm_track_workspace_bytes(T, total_samples).
- * Metrics: gt_positions (T, 3), NaN first position of a video = no ground truth; the ring is
- * (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).  Same restrictions as args->B > 1 (whole
- * steps, no splat plan, no fused logit update in a deferred step). */
+ * track_loss, g_focal, m_focal, v_focal) hold B values.  Video b gets what a one-video step on it gets:
+ * its flow loss is normalised by its own mask_sum[b] and its tracking loss by its own valid count ("or 1"
+ * per video), and its poses chain from the identity at its own frame 0.  (The reference's LossFlow
+ * normalises a batch by ONE pooled mask sum; this is B overfit runs, not a pooled batch.)  Tracks: the
+ * segments of video b carry start frames frame_offset[b] + s (they never cross videos); track_ws is
+ * fm_track_workspace_bytes(T, total_samples).  Metrics: gt_positions (T, 3), NaN first position of a
+ * video = no ground truth; the ring is (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).
+ * Needs phase FM_STEP_ALL and no splat plan, and refuses defer_adam = 1 together with step > 0 and weight
+ * logits (the caller updates the logits after the sweep's backward). */
 int fm_overfit_step_videos(const fm_overfit_step_args* args, const fm_video_layout* layout, void* stream);
 size_t fm_workspace_bytes_videos(int B, int T);
-/* fm_procrustes_moments for packed videos of different lengths (see fm_overfit_step_args.moments_k4). */
+/* fm_procrustes_moments for packed videos (see fm_overfit_step_args.moments_k4). */
 int fm_procrustes_moments_videos(const float* depth, const float* k4, const float* backward_flow,
                                  const float* weights, float weight_sensitivity, void* ws,
                                  const fm_video_layout* layout, int H, int W, void* stream);
@@ -432,8 +421,10 @@ int fm_softmin_sweep_bwd_videos(const float* depth, const float* weights, float 
                                 const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
                                 float* g_depth, float* g_weights, void* ws, const fm_video_layout* layout,
                                 int H, int W, void* stream);
-/* fm_adam_step_clock_frames for a packed layout: the rows lo <= r < min(hi, rows of video b) of every
- * video b, rows = its frames (pairs = 0: depth) or its pairs (pairs = 1: weight logits). */
+/* fm_adam_step_clock on the rows lo <= r < min(hi, rows of video b) of every video b of a packed layout,
+ * rows = its frames (pairs = 0: depth) or its pairs (pairs = 1: weight logits): one launch for the same
+ * rows of every video (the softmin stage, where the sweep still adds to frames 0 / 1 of each video while
+ * the others are final). */
 int fm_adam_step_clock_frames_videos(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
                                      size_t frame_elems, const fm_video_layout* layout, int pairs, int frame_lo,
                                      int frame_hi, const void* clock, int focal_clock, double beta1,
@@ -450,10 +441,6 @@ int fm_pose_chain_bwd_videos(const float* rt, const float* extrinsics, const flo
 int fm_procrustes_moments(const float* depth, const float* k4, const float* backward_flow,
                           const float* weights, float weight_sensitivity, void* ws, int F, int H, int W,
                           void* stream);
-/* The same for B videos (depth (B,F,H,W), k4 (B*F,4), ...): the moment pass of a B-video step. */
-int fm_procrustes_moments_batched(const float* depth, const float* k4, const float* backward_flow,
-                                  const float* weights, float weight_sensitivity, void* ws, int B, int F, int H,
-                                  int W, void* stream);
 
 /* ---- stages either side of the hot path (SURVEY 8(f) rank 4) ---------------------------- */
 
