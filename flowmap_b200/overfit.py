@@ -135,6 +135,15 @@ class Overfitter:
 _FLOW_NAMES = ("forward", "backward", "forward_mask", "backward_mask")
 
 
+def video_tables(frames, device):
+    """The device tables of an fm_video_layout for videos of `frames` frames packed along the frame axis:
+    the frame offsets (B + 1,), the video of every frame (T,) and of every pair (T - B,), int32."""
+    B, fr = len(frames), torch.tensor(frames)
+    fo = torch.tensor([sum(frames[:i]) for i in range(B + 1)], dtype=torch.int32)
+    return (fo.to(device), torch.repeat_interleave(torch.arange(B, dtype=torch.int32), fr).to(device),
+            torch.repeat_interleave(torch.arange(B, dtype=torch.int32), fr - 1).to(device))
+
+
 def _video(x, i: int):
     """Video i of a Batch or Flows of several videos, as a one-video instance of the same type (views)."""
     return replace(x, **{f.name: getattr(x, f.name)[i:i + 1] for f in fields(x) if getattr(x, f.name) is not None})
@@ -269,10 +278,7 @@ class FusedOverfitter(Overfitter):
         # packed flows: the pairs of video b follow those of video b - 1
         self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(dev), n)[0] for fl in flows]).contiguous()
                              for n in _FLOW_NAMES))
-        fo = torch.tensor(self._first + [self.T], dtype=torch.int32)
-        self._tables = (fo.to(dev),
-                        torch.repeat_interleave(torch.arange(B, dtype=torch.int32), torch.tensor(frames)).to(dev),
-                        torch.repeat_interleave(torch.arange(B, dtype=torch.int32), torch.tensor(frames) - 1).to(dev))
+        self._tables = video_tables(frames, dev)
         self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
         self._layout_ref = ctypes.byref(self._layout)
         self._use_plan, self._plan = False, None
