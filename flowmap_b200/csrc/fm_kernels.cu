@@ -384,12 +384,12 @@ __device__ __forceinline__ PairGeom pair_geom(const float* k4, const PairAddr& p
 
 // The conditioning shift of every moment pair (shift_sample / shift_from_sums in fm_pixel.cuh): one
 // block per pair, kShiftSamples gathers of the later frame's depth and the pair's weights.
-// Each Procrustes kernel below is a force-inlined body templated on its pair layout, instantiated as the
-// uniform kernel (PairLayout) and as a `_ragged` kernel of its own name (RaggedPairs / RaggedSweep).
+// Each Procrustes kernel below is templated on its pair layout: PairLayout for one video (and the
+// broadcast of the focal sweep), RaggedPairs / RaggedSweep for packed videos.
 template <class Lay>
-__device__ __forceinline__ void pair_shift_body(const float* __restrict__ depth, const float* __restrict__ weights,
-                                                float wsens, float* __restrict__ zshift, const Lay& lay, int H,
-                                                int W) {
+__global__ void __launch_bounds__(kThreads)
+k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
+             float* __restrict__ zshift, Lay lay, int H, int W) {
   __shared__ double smem[3][kThreads / 32];
   const int pair = blockIdx.x, N = H * W;
   const PairAddr pa = pair_addr(lay, pair, N);
@@ -416,24 +416,12 @@ __device__ __forceinline__ void pair_shift_body(const float* __restrict__ depth,
   }
 }
 
-__global__ void __launch_bounds__(kThreads)
-k_pair_shift(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
-             float* __restrict__ zshift, PairLayout lay, int H, int W) {
-  pair_shift_body(depth, weights, wsens, zshift, lay, H, W);
-}
-template <class Lay>
-__global__ void __launch_bounds__(kThreads)
-k_pair_shift_ragged(const float* __restrict__ depth, const float* __restrict__ weights, float wsens,
-                    float* __restrict__ zshift, Lay lay, int H, int W) {
-  pair_shift_body(depth, weights, wsens, zshift, lay, H, W);
-}
-
 template <int VEC, class Lay>
-__device__ __forceinline__ void moments_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                             const float* __restrict__ bflow, const float* __restrict__ weights,
-                                             const int64_t* __restrict__ indices, int num_indices,
-                                             double* __restrict__ moments, const float* __restrict__ zshift,
-                                             float wsens, const Lay& lay, int H, int W) {
+__global__ void __launch_bounds__(kThreads, 3)
+k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
+          const float* __restrict__ bflow, const float* __restrict__ weights,
+          const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
+          const float* __restrict__ zshift, float wsens, Lay lay, int H, int W) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int pair = blockIdx.y;
   const int N = H * W;
@@ -464,28 +452,12 @@ __device__ __forceinline__ void moments_body(const float* __restrict__ depth, co
   block_accumulate<kNumMoments>(acc, moments + (size_t)pair * kNumMoments, smem);
 }
 
-template <int VEC>
-__global__ void __launch_bounds__(kThreads, 3)
-k_moments(const float* __restrict__ depth, const float* __restrict__ k4,
-          const float* __restrict__ bflow, const float* __restrict__ weights,
-          const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
-          const float* __restrict__ zshift, float wsens, PairLayout lay, int H, int W) {
-  moments_body<VEC>(depth, k4, bflow, weights, indices, num_indices, moments, zshift, wsens, lay, H, W);
-}
-template <int VEC, class Lay>
-__global__ void __launch_bounds__(kThreads, 3)
-k_moments_ragged(const float* __restrict__ depth, const float* __restrict__ k4,
-                 const float* __restrict__ bflow, const float* __restrict__ weights,
-                 const int64_t* __restrict__ indices, int num_indices, double* __restrict__ moments,
-                 const float* __restrict__ zshift, float wsens, Lay lay, int H, int W) {
-  moments_body<VEC>(depth, k4, bflow, weights, indices, num_indices, moments, zshift, wsens, lay, H, W);
-}
-
 template <int VEC, int LX, class Lay>
-__device__ __forceinline__ void moments_dense_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                                   const float* __restrict__ bflow, const float* __restrict__ weights,
-                                                   double* __restrict__ moments, const float* __restrict__ zshift,
-                                                   float wsens, const Lay& lay, int H, int W, int BP, int rounds) {
+__global__ void __launch_bounds__(kThreads, 3)
+k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
+                const float* __restrict__ bflow, const float* __restrict__ weights,
+                double* __restrict__ moments, const float* __restrict__ zshift, float wsens, Lay lay,
+                int H, int W, int BP, int rounds) {
   __shared__ double smem[kNumMoments * (kThreads / 32)];
   const int N = H * W;
   constexpr int kChunk = kThreads * VEC;
@@ -549,33 +521,15 @@ __device__ __forceinline__ void moments_dense_body(const float* __restrict__ dep
   }
 }
 
-template <int VEC, int LX>
-__global__ void __launch_bounds__(kThreads, 3)
-k_moments_dense(const float* __restrict__ depth, const float* __restrict__ k4,
-                const float* __restrict__ bflow, const float* __restrict__ weights,
-                double* __restrict__ moments, const float* __restrict__ zshift, float wsens, PairLayout lay,
-                int H, int W, int BP, int rounds) {
-  moments_dense_body<VEC, LX>(depth, k4, bflow, weights, moments, zshift, wsens, lay, H, W, BP, rounds);
-}
-template <int VEC, int LX>
-__global__ void __launch_bounds__(kThreads, 3)
-k_moments_dense_ragged(const float* __restrict__ depth, const float* __restrict__ k4,
-                       const float* __restrict__ bflow, const float* __restrict__ weights,
-                       double* __restrict__ moments, const float* __restrict__ zshift, float wsens, RaggedPairs lay,
-                       int H, int W, int BP, int rounds) {
-  moments_dense_body<VEC, LX>(depth, k4, bflow, weights, moments, zshift, wsens, lay, H, W, BP, rounds);
-}
-
 // ================================================================== phase B: solve
 // moments_k4 != NULL: the sums were accumulated with the intrinsics moments_k4 (same principal points,
 // other focal lengths) before the step's own K was known.  Points scale per axis with the focal
 // ratio (p = S_b p', q = S_a q', S = diag(fx'/fx, fy'/fy, 1); the conditioning shift is along z), so
 // the 16 sums are rescaled exactly here -- and written back for later readers of the workspace.
 template <class Lay>
-__device__ __forceinline__ void solve_body(double* __restrict__ moments, const float* __restrict__ zshift,
-                                           float* __restrict__ rt, PairState* __restrict__ state, int BP,
-                                           const Lay& lay, int H, int W, const float* __restrict__ moments_k4,
-                                           const float* __restrict__ k4) {
+__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ zshift,
+                        float* __restrict__ rt, PairState* __restrict__ state, int BP, Lay lay,
+                        int H, int W, const float* __restrict__ moments_k4, const float* __restrict__ k4) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   const PairAddr pa = pair_addr(lay, pair, H * W);
@@ -599,18 +553,6 @@ __device__ __forceinline__ void solve_body(double* __restrict__ moments, const f
   procrustes_solve(m, shift, out, st);
   for (int k = 0; k < 12; ++k) rt[(size_t)pair * 12 + k] = out[k];
   state[pair] = st;
-}
-
-__global__ void k_solve(double* __restrict__ moments, const float* __restrict__ zshift,
-                        float* __restrict__ rt, PairState* __restrict__ state, int BP, PairLayout lay,
-                        int H, int W, const float* __restrict__ moments_k4 = nullptr,
-                        const float* __restrict__ k4 = nullptr) {
-  solve_body(moments, zshift, rt, state, BP, lay, H, W, moments_k4, k4);
-}
-__global__ void k_solve_ragged(double* __restrict__ moments, const float* __restrict__ zshift,
-                               float* __restrict__ rt, PairState* __restrict__ state, int BP, RaggedPairs lay,
-                               int H, int W, const float* __restrict__ moments_k4, const float* __restrict__ k4) {
-  solve_body(moments, zshift, rt, state, BP, lay, H, W, moments_k4, k4);
 }
 
 // ================================================================== phase C: flow loss
@@ -1050,12 +992,11 @@ struct AdamFuse {
 };
 
 template <int VEC, class Lay>
-__device__ __forceinline__ void distribute_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                                const float* __restrict__ bflow, float* weights,
-                                                const int64_t* __restrict__ indices, int num_indices,
-                                                const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
-                                                float* __restrict__ g_weights, double* __restrict__ k4acc,
-                                                float wsens, Lay lay, AdamFuse adam, int H, int W) {
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow,
+             float* weights, const int64_t* __restrict__ indices, int num_indices,
+             const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth, float* __restrict__ g_weights,
+             double* __restrict__ k4acc, float wsens, Lay lay, AdamFuse adam, int H, int W) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   const int pair = blockIdx.y;
@@ -1098,24 +1039,6 @@ __device__ __forceinline__ void distribute_body(const float* __restrict__ depth,
   // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
   block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
 }
-
-#define FM_DISTRIBUTE_PARAMS                                                                                  \
-  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
-      const int64_t* __restrict__ indices, int num_indices, const PairAdjoint* __restrict__ adj,               \
-      float* __restrict__ g_depth, float* __restrict__ g_weights, double* __restrict__ k4acc, float wsens
-template <int VEC>
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute(FM_DISTRIBUTE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W) {
-  distribute_body<VEC>(depth, k4, bflow, weights, indices, num_indices, adj, g_depth, g_weights, k4acc, wsens, lay,
-                       adam, H, W);
-}
-template <int VEC, class Lay>
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute_ragged(FM_DISTRIBUTE_PARAMS, Lay lay, AdamFuse adam, int H, int W) {
-  distribute_body<VEC>(depth, k4, bflow, weights, indices, num_indices, adj, g_depth, g_weights, k4acc, wsens, lay,
-                       adam, H, W);
-}
-#undef FM_DISTRIBUTE_PARAMS
 
 // Per-pixel work of the dense phase D2 for the VEC consecutive pixels of row r from column c0
 // (linear index base in the frame, wi = base + the pair's offset in the weight-shaped arrays): the
@@ -1185,13 +1108,13 @@ __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairA
 // Dense (all-pixel) phase D2 for widths that are not a multiple of 4: one pixel per thread on the
 // item decomposition of block_item_range (chunks of kThreads pixels), taps as REDs, per-pair constants
 // re-staged when a block moves on to its next pair.  The weight Adam runs as a separate pass.
+#define FM_DISTRIBUTE_DENSE_PARAMS                                                                            \
+  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
+      const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth, float* __restrict__ g_weights,        \
+      double* __restrict__ k4acc, float wsens
 template <class Lay>
-__device__ __forceinline__ void distribute_dense_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                                      const float* __restrict__ bflow, float* weights,
-                                                      const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
-                                                      float* __restrict__ g_weights, double* __restrict__ k4acc,
-                                                      float wsens, Lay lay, AdamFuse adam, int H, int W,
-                                                      int BP, int rounds) {
+__global__ void __launch_bounds__(kThreads, 3)
+k_distribute_dense(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, int W, int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   const int N = H * W;
@@ -1232,20 +1155,6 @@ __device__ __forceinline__ void distribute_dense_body(const float* __restrict__ 
     i += ce - cb;
   }
   }
-}
-
-#define FM_DISTRIBUTE_DENSE_PARAMS                                                                            \
-  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
-      const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth, float* __restrict__ g_weights,        \
-      double* __restrict__ k4acc, float wsens
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute_dense(FM_DISTRIBUTE_DENSE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
-  distribute_dense_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
-}
-__global__ void __launch_bounds__(kThreads, 3)
-k_distribute_dense_ragged(FM_DISTRIBUTE_DENSE_PARAMS, RaggedPairs lay, AdamFuse adam, int H, int W, int BP,
-                          int rounds) {
-  distribute_dense_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
 }
 
 // Tile and halo of k_distribute_window (build-time knobs for tools/ab_libs.py).  With the defaults
@@ -1313,12 +1222,8 @@ namespace {
 // fm_overfit_step) and zeroed.  This replaces ~2.6 scattered 32-byte RED requests per pixel (bound by
 // the L2 atomic units) with ~0.7 coalesced ones.
 template <class Lay>
-__device__ __forceinline__ void distribute_window_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                                       const float* __restrict__ bflow, float* weights,
-                                                       const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth,
-                                                       float* __restrict__ g_weights, double* __restrict__ k4acc,
-                                                       float wsens, Lay lay, AdamFuse adam, int H,
-                                                       int W, int BP, int rounds) {
+__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
+k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, int W, int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
   __shared__ PairAdjoint s_adj;
   __shared__ PairGeom s_geom;
@@ -1425,16 +1330,6 @@ __device__ __forceinline__ void distribute_window_body(const float* __restrict__
     i += te - tb;
   }
   }
-}
-
-__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
-k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, PairLayout lay, AdamFuse adam, int H, int W, int BP, int rounds) {
-  distribute_window_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
-}
-__global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
-k_distribute_window_ragged(FM_DISTRIBUTE_DENSE_PARAMS, RaggedPairs lay, AdamFuse adam, int H, int W, int BP,
-                           int rounds) {
-  distribute_window_body(depth, k4, bflow, weights, adj, g_depth, g_weights, k4acc, wsens, lay, adam, H, W, BP, rounds);
 }
 #undef FM_DISTRIBUTE_DENSE_PARAMS
 
@@ -2434,14 +2329,13 @@ __global__ void k_sweep_aggregate(const PairAdjoint* __restrict__ adj, const flo
   }
 }
 
-#define FM_SWEEP_PARAMS                                                                                      \
-  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,               \
-      const float* __restrict__ bflow, const float* __restrict__ weights, float wsens,                       \
-      const int64_t* __restrict__ indices, int num_indices, const float* __restrict__ g_err,                 \
-      double* __restrict__ acc_out, float* __restrict__ g_depth, float* __restrict__ g_weights
-#define FM_SWEEP_ARGS depth, k4, rt, bflow, weights, wsens, indices, num_indices, g_err, acc_out, g_depth, g_weights
 template <bool BWD, class Lay>
-__device__ __forceinline__ void sweep_body(FM_SWEEP_PARAMS, const Lay& lay, int H, int W) {
+__global__ void __launch_bounds__(kThreads)
+k_sweep(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ rt,
+        const float* __restrict__ bflow, const float* __restrict__ weights, float wsens,
+        const int64_t* __restrict__ indices, int num_indices, const float* __restrict__ g_err,
+        double* __restrict__ acc_out, float* __restrict__ g_depth, float* __restrict__ g_weights, Lay lay, int H,
+        int W) {
   __shared__ double smem[12 * (kThreads / 32)];
   const int item = blockIdx.y;
   const int N = H * W;
@@ -2501,17 +2395,6 @@ __device__ __forceinline__ void sweep_body(FM_SWEEP_PARAMS, const Lay& lay, int 
   if (!BWD) block_accumulate<1>(acc, acc_out + (size_t)item * kSweepAcc, smem);
   else block_accumulate<12>(acc, acc_out + (size_t)item * kSweepAcc + 1, smem);
 }
-
-template <bool BWD>
-__global__ void __launch_bounds__(kThreads) k_sweep(FM_SWEEP_PARAMS, PairLayout lay, int H, int W) {
-  sweep_body<BWD>(FM_SWEEP_ARGS, lay, H, W);
-}
-template <bool BWD>
-__global__ void __launch_bounds__(kThreads) k_sweep_ragged(FM_SWEEP_PARAMS, RaggedSweep lay, int H, int W) {
-  sweep_body<BWD>(FM_SWEEP_ARGS, lay, H, W);
-}
-#undef FM_SWEEP_PARAMS
-#undef FM_SWEEP_ARGS
 
 __global__ void k_sweep_out(const double* __restrict__ acc, float* __restrict__ out, int items, int off,
                             int count) {
@@ -3156,6 +3039,256 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
   }
   return 0;
 }
+
+// k_adjoint and k_k4_finalize find a pair's or a frame's video by dividing by F (one video, or a uniform
+// batch) or in the packed layout's tables; their parameter lists differ, so each layout has its launch.
+int launch_adjoint(const PairLayout& lay, const Workspace& w, const float* g_rt, int include_flow,
+                   const float* flow_scale, int BP, cudaStream_t s) {
+  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow, flow_scale, w.adj, BP, lay.F);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
+  return 0;
+}
+int launch_adjoint(const RaggedPairs& lay, const Workspace& w, const float* g_rt, int include_flow,
+                   const float* flow_scale, int BP, cudaStream_t s) {
+  k_adjoint_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow, flow_scale, w.adj, BP, lay.v);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint_ragged");
+  return 0;
+}
+int launch_k4_finalize(const PairLayout& lay, const Workspace& w, int include_flow, const float* flow_scale,
+                       float* g_k4, int T, cudaStream_t s) {
+  k_k4_finalize<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow, flow_scale, g_k4, T / lay.F, lay.F);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
+  return 0;
+}
+int launch_k4_finalize(const RaggedPairs& lay, const Workspace& w, int include_flow, const float* flow_scale,
+                       float* g_k4, int T, cudaStream_t s) {
+  k_k4_finalize_ragged<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow, flow_scale, g_k4, T, lay.v);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize_ragged");
+  return 0;
+}
+
+// The Procrustes forward of B videos with T frames (T - B pairs) in all, laid out as `lay`: dense_layout
+// for one video or a uniform batch, RaggedPairs for packed videos of different lengths.  Pair shift,
+// moments, then (solve) the poses.  moments_k4 != NULL: fm_procrustes_moments(_videos) already accumulated
+// the moments with those intrinsics, and only the solve runs.
+template <class Lay>
+int procrustes_fwd(const float* depth, const float* k4, const float* backward_flow, const float* weights, float wsens,
+                   const int64_t* indices, int num_indices, float* rt, void* ws, int B, int T, const Lay& lay, int H,
+                   int W, cudaStream_t s, const float* moments_k4, bool solve) {
+  if (!depth || !k4 || !backward_flow || (!rt && solve) || !ws || T < 2 * B || bad_dims(B, 2, H, W))
+    return fail_msg("fm_procrustes_fwd: bad arguments");
+  if (indices && num_indices < 1) return fail_msg("fm_procrustes_fwd: empty index set");
+  if (moments_k4 && indices) return fail_msg("fm_procrustes_fwd: precomputed moments serve the dense path");
+  const int BP = T - B;
+  Workspace w = carve_rows(ws, B, T, BP);
+  if (!moments_k4) {
+    cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
+    if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
+    k_pair_shift<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
+    FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift");
+    if (indices) {
+      dim3 grid(blocks_for_points(num_indices), BP);
+      k_moments<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, w.zshift, wsens, lay, H, W);
+    } else {
+      const int vec = W % 4 == 0 ? 4 : 1;  // patch_shape_ok implies W % 4 == 0
+      const long long items = (long long)BP * ((H * W + kThreads * vec - 1) / (kThreads * vec));
+      const int pg = persistent_grid(3, items);
+      const int rounds = procrustes_rounds(H, W, vec == 4 ? items : items / 4, pg, true);
+      if (patch_shape_ok(H, W))
+        k_moments_dense<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, rounds);
+      else if (vec == 4)
+        k_moments_dense<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, rounds);
+      else
+        k_moments_dense<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, rounds);
+    }
+    FM_CHECK_LAUNCH("fm_procrustes_fwd: k_moments");
+  }
+  if (!solve) return 0;
+  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, moments_k4, k4);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
+  return 0;
+}
+
+// The Procrustes backward in the layout of procrustes_fwd: d loss / d (depth, weights, K) from the pose
+// gradient g_rt and (include_flow_loss) the flow loss's, scaled by flow_scale.  The direct depth gradient
+// already in g_depth is scaled here too unless the caller did (depth_prescaled).
+template <class Lay>
+int procrustes_bwd(const float* depth, const float* k4, const float* backward_flow, const float* weights, float wsens,
+                   const int64_t* indices, int num_indices, const float* g_rt, int include_flow_loss,
+                   const float* flow_scale, float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int T,
+                   const Lay& lay, int H, int W, cudaStream_t s, const AdamFuse* adam, bool depth_prescaled) {
+  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || T < 2 * B || bad_dims(B, 2, H, W))
+    return fail_msg("fm_procrustes_bwd: bad arguments");
+  if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
+  const int BP = T - B;
+  Workspace w = carve_rows(ws, B, T, BP);
+  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)T * 4 * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
+  AdamFuse af;
+  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
+  float* weights_rw = const_cast<float*>(weights);
+  if (include_flow_loss && flow_scale && !depth_prescaled) {
+    // the direct depth gradient already sitting in g_depth was computed for scale 1
+    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)T * H * W);
+    FM_CHECK_LAUNCH("fm_procrustes_bwd: k_scale_inplace");
+  }
+  int rc = launch_adjoint(lay, w, g_rt, include_flow_loss, flow_scale, BP, s);
+  if (rc) return rc;
+  if (indices) {
+    dim3 grid(blocks_for_points(num_indices), BP);
+    k_distribute<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
+  } else if (W % 4 == 0) {
+    const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
+    const int pg = persistent_grid(FM_WIN_CTAS, items);
+    const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);  // rounds are sized in 1024-pixel chunks
+    k_distribute_window<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
+  } else {
+    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
+    const int pg = persistent_grid(3, items);
+    k_distribute_dense<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
+  }
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
+  return launch_k4_finalize(lay, w, include_flow_loss, flow_scale, g_k4, T, s);
+}
+
+// The splat plan's Procrustes forward and backward (fm_tiled.cuh): one video, all pixels, W % 4 == 0.
+int procrustes_fwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
+                           float wsens, void* plan, float* rt, void* ws, int F, int H, int W, cudaStream_t s) {
+  if (!depth || !k4 || !backward_flow || !rt || !ws || bad_dims(1, F, H, W))
+    return fail_msg("fm_procrustes_fwd: bad arguments");
+  if (!tiled_shape_ok(F, H, W))
+    return fail_msg("fm_procrustes_fwd: the splat plan serves the dense single-video path with W % 4 == 0");
+  const int BP = F - 1;
+  const PairLayout lay = dense_layout(F, H, W);
+  Workspace w = carve(ws, 1, F);
+  cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
+  k_pair_shift<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift");
+  const int rc = launch_moments_tiled(depth, k4, backward_flow, weights, wsens, tiled::plan_carve(plan, F, H, W),
+                                      w.moments, w.zshift, F, H, W, s);
+  if (rc) return rc;
+  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, nullptr, nullptr);
+  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
+  return 0;
+}
+
+// The caller scales the direct depth gradient in g_depth: flow_scale only scales the flow loss's pose and
+// K gradients here.
+int procrustes_bwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
+                           float wsens, void* plan, unsigned plan_ovf_max, const float* g_rt, int include_flow_loss,
+                           const float* flow_scale, float* g_depth, float* g_weights, float* g_k4, void* ws, int F,
+                           int H, int W, cudaStream_t s, const AdamFuse* adam) {
+  if (!tiled_shape_ok(F, H, W))
+    return fail_msg("fm_procrustes_bwd: the splat plan serves the dense single-video path with W % 4 == 0");
+  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || bad_dims(1, F, H, W))
+    return fail_msg("fm_procrustes_bwd: bad arguments");
+  if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
+  const int BP = F - 1;
+  Workspace w = carve(ws, 1, F);
+  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)F * 4 * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
+  AdamFuse af;
+  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
+  // one focal length shared by all frames (or constant intrinsics): the Procrustes part of the
+  // intrinsics gradient comes from the moment sums, the pixel kernel carries no K accumulators
+  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP, F,
+                                          w.moments, k4, w.k4acc);
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
+  const int rc = launch_backward_tiled(depth, k4, backward_flow, const_cast<float*>(weights), wsens,
+                                       tiled::plan_carve(plan, F, H, W), plan_ovf_max, w.adj, g_depth, g_weights, af,
+                                       F, H, W, s);
+  if (rc) return rc;
+  return launch_k4_finalize(dense_layout(F, H, W), w, include_flow_loss, flow_scale, g_k4, F, s);
+}
+
+PairLayout sweep_layout(int F, int H, int W, int cand) {
+  PairLayout l = dense_layout(F, H, W);  // strides of the REAL tensors
+  l.F = 2;                               // the sweep only sees frames 0 and 1 (pair 0)
+  l.cand = cand;
+  return l;
+}
+
+// The focal-length sweep on pair 0 of each of B videos: `lay` holds num_candidates virtual items per video,
+// `lay1` one (sweep_layout for one video or a uniform batch, RaggedSweep for packed videos).
+template <class Lay>
+int sweep_fwd_impl(const float* depth, const float* weights, float weight_sensitivity, const float* backward_flow,
+                   const int64_t* indices, int num_indices, const float* cand_k4, int num_candidates, float* err,
+                   float* rt, void* ws, int B, int F, int H, int W, void* stream, const Lay& lay, const Lay& lay1) {
+  if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 ||
+      !err || !rt || !ws || bad_dims(B, F, H, W))
+    return fail_msg("fm_softmin_sweep_fwd: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int items = B * num_candidates;
+  Workspace w = carve(ws, items + B, 2);
+  float* scratch = (float*)((char*)ws + align_up(w.bytes, 256));
+  float* base_k4 = scratch + (size_t)items * 12 + (size_t)items * 8;  // after g_rt and g_k4 of the bwd
+  double* base_moments = w.moments + (size_t)items * kNumMoments;
+  cudaError_t e = cudaMemsetAsync(base_moments, 0, (size_t)B * kNumMoments * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
+  k_sweep_base_k4<<<(B * 8 + 127) / 128, 128, 0, s>>>(cand_k4, base_k4, B, num_candidates);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_base_k4");
+  float* base_zshift = w.zshift + items;  // one conditioning shift per batch element, for all candidates
+  k_pair_shift<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, lay1, H, W);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_pair_shift");
+  {  // ONE moment pass (candidate 0); every candidate's moments are a rescaling of it
+    dim3 grid(blocks_for_points(num_indices), B);
+    k_moments<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
+                                          base_moments, base_zshift, weight_sensitivity, lay1, H, W);
+    FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_moments");
+  }
+  k_sweep_scale_solve<<<(items + 63) / 64, 64, 0, s>>>(base_moments, base_zshift, cand_k4, rt, w.state, B,
+                                                      num_candidates);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_scale_solve");
+  e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
+  dim3 grid(blocks_for_points(num_indices), items);
+  k_sweep<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity, indices,
+                                          num_indices, nullptr, w.flowacc, nullptr, nullptr, lay, H, W);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep");
+  k_sweep_out<<<(items + 127) / 128, 128, 0, s>>>(w.flowacc, err, items, 0, 1);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_out");
+  return 0;
+}
+
+template <class Lay>
+int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensitivity, const float* backward_flow,
+                   const int64_t* indices, int num_indices, const float* cand_k4, int num_candidates, const float* rt,
+                   const float* g_err, float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
+                   void* stream, const Lay& lay, const Lay& lay1) {
+  if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 || !rt ||
+      !g_err || !g_depth || !ws || bad_dims(B, F, H, W))
+    return fail_msg("fm_softmin_sweep_bwd: bad arguments");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int items = B * num_candidates;
+  Workspace w = carve(ws, items + B, 2);
+  float* scratch = (float*)((char*)ws + align_up(w.bytes, 256));
+  float* g_rt = scratch;
+  float* base_k4 = scratch + (size_t)items * 12 + (size_t)items * 8;
+  cudaError_t e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_softmin_sweep_bwd: memset", e);
+  e = cudaMemsetAsync(w.k4acc, 0, (size_t)(items + B) * 2 * 4 * sizeof(double), s);
+  if (e != cudaSuccess) return fail("fm_softmin_sweep_bwd: memset", e);
+  dim3 grid(blocks_for_points(num_indices), items);
+  k_sweep<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity, indices,
+                                         num_indices, g_err, w.flowacc, g_depth, g_weights, lay, H, W);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep");
+  k_sweep_out<<<(items * 12 + 127) / 128, 128, 0, s>>>(w.flowacc, g_rt, items, 1, 12);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_out");
+  // per-candidate adjoint constants, collapsed into one per batch element, then ONE distribution pass
+  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, 2);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_adjoint");
+  k_sweep_aggregate<<<B, 32, 0, s>>>(w.adj, cand_k4, w.adj + items, B, num_candidates);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_aggregate");
+  AdamFuse af;
+  memset(&af, 0, sizeof(af));
+  dim3 grid1(blocks_for_points(num_indices), B);
+  k_distribute<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights), indices,
+                                            num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
+                                            weight_sensitivity, lay1, af, H, W);
+  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_distribute");
+  return 0;
+}
 }  // namespace
 
 // =================================================================== C ABI
@@ -3213,209 +3346,18 @@ int fm_reproject(const float* xyz, const float* rt, const float* k4, float* xy, 
   return 0;
 }
 
-static int procrustes_fwd_impl(const float* depth, const float* k4, const float* backward_flow,
-                               const float* weights, float wsens, const int64_t* indices,
-                               int num_indices, float* rt, void* ws, int B, int F, int H, int W,
-                               void* stream, const PairLayout* layout = nullptr, void* plan = nullptr,
-                               const float* moments_k4 = nullptr, bool solve = true) {
-  const PairLayout lay = layout ? *layout : dense_layout(F, H, W);
-  if (!depth || !k4 || !backward_flow || (!rt && solve) || !ws || bad_dims(B, F, H, W))
-    return fail_msg("fm_procrustes_fwd: bad arguments");
-  if (plan && (B != 1 || indices || layout || !tiled_shape_ok(F, H, W)))
-    return fail_msg("fm_procrustes_fwd: the splat plan serves the dense single-video path with W % 4 == 0");
-  if (indices && num_indices < 1) return fail_msg("fm_procrustes_fwd: empty index set");
-  cudaStream_t s = (cudaStream_t)stream;
-  Workspace w = carve(ws, B, F);
-  const int BP = B * (F - 1);
-  if (moments_k4) {  // fm_procrustes_moments already ran with those intrinsics
-    if (plan || indices || layout) return fail_msg("fm_procrustes_fwd: precomputed moments serve the dense path");
-    if (!solve) return 0;
-    k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, moments_k4, k4);
-    FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
-    return 0;
-  }
-  cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
-  k_pair_shift<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift");
-  if (plan) {
-    const tiled::Plan pl = tiled::plan_carve(plan, F, H, W);
-    const int rc = launch_moments_tiled(depth, k4, backward_flow, weights, wsens, pl, w.moments, w.zshift, F, H, W, s);
-    if (rc) return rc;
-  } else if (indices) {
-    dim3 grid(blocks_for_points(num_indices), BP);
-    k_moments<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, w.zshift, wsens, lay, H, W);
-  } else if (patch_shape_ok(H, W)) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_moments_dense<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
-  } else if (W % 4 == 0) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_moments_dense<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
-  } else {
-    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
-    const int pg = persistent_grid(3, items);
-    k_moments_dense<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items / 4, pg, true));
-  }
-  if (!plan) FM_CHECK_LAUNCH("fm_procrustes_fwd: k_moments");
-  if (!solve) return 0;
-  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
-  return 0;
-}
-
 int fm_procrustes_fwd(const float* depth, const float* k4, const float* backward_flow,
                       const float* weights, const int64_t* indices, int num_indices, float* rt,
                       void* ws, int B, int F, int H, int W, void* stream) {
-  return procrustes_fwd_impl(depth, k4, backward_flow, weights, 0.f, indices, num_indices, rt, ws, B, F,
-                             H, W, stream);
+  return procrustes_fwd(depth, k4, backward_flow, weights, 0.f, indices, num_indices, rt, ws, B, B * F,
+                        dense_layout(F, H, W), H, W, (cudaStream_t)stream, nullptr, /*solve=*/true);
 }
 
 int fm_procrustes_moments(const float* depth, const float* k4, const float* backward_flow,
                           const float* weights, float weight_sensitivity, void* ws, int F, int H, int W,
                           void* stream) {
-  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, 1, F,
-                             H, W, stream, nullptr, nullptr, nullptr, /*solve=*/false);
-}
-
-static int procrustes_bwd_impl(const float* depth, const float* k4, const float* backward_flow,
-                               const float* weights, float wsens, const int64_t* indices,
-                               int num_indices, const float* g_rt, int include_flow_loss,
-                               const float* flow_scale, float* g_depth, float* g_weights, float* g_k4,
-                               void* ws, int B, int F, int H, int W, void* stream,
-                               const PairLayout* layout = nullptr, const AdamFuse* adam = nullptr,
-                               void* plan = nullptr, unsigned plan_ovf_max = 0u, bool depth_prescaled = false) {
-  const PairLayout lay = layout ? *layout : dense_layout(F, H, W);
-  if (plan && (B != 1 || indices || layout || !tiled_shape_ok(F, H, W)))
-    return fail_msg("fm_procrustes_bwd: the splat plan serves the dense single-video path with W % 4 == 0");
-  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || bad_dims(B, F, H, W))
-    return fail_msg("fm_procrustes_bwd: bad arguments");
-  if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
-  cudaStream_t s = (cudaStream_t)stream;
-  Workspace w = carve(ws, B, F);
-  const int BP = B * (F - 1), BF = B * F;
-  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)BF * 4 * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
-  AdamFuse af;
-  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
-  float* weights_rw = const_cast<float*>(weights);
-  if (include_flow_loss && flow_scale && !depth_prescaled) {
-    // the direct depth gradient already sitting in g_depth was computed for scale 1
-    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)BF * H * W);
-    FM_CHECK_LAUNCH("fm_procrustes_bwd: k_scale_inplace");
-  }
-  if (plan) {
-    // one focal length shared by all frames (or constant intrinsics): the Procrustes part of the
-    // intrinsics gradient comes from the moment sums, the pixel kernel carries no K accumulators
-    k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP, F,
-                                            w.moments, k4, w.k4acc);
-    FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
-    const tiled::Plan pl = tiled::plan_carve(plan, F, H, W);
-    const int rc = launch_backward_tiled(depth, k4, backward_flow, weights_rw, wsens, pl, plan_ovf_max, w.adj, g_depth,
-                                         g_weights, af, F, H, W, s);
-    if (rc) return rc;
-    k_k4_finalize<<<(BF + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, B, F);
-    FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
-    return 0;
-  }
-  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP, F);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
-  if (indices) {
-    dim3 grid(blocks_for_points(num_indices), BP);
-    k_distribute<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
-  } else if (W % 4 == 0) {
-    const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
-    const int pg = persistent_grid(FM_WIN_CTAS, items);
-    const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);  // rounds are sized in 1024-pixel chunks
-    k_distribute_window<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
-  } else {
-    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
-    const int pg = persistent_grid(3, items);
-    k_distribute_dense<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
-  }
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
-  k_k4_finalize<<<(BF + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, B, F);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
-  return 0;
-}
-
-// procrustes_fwd_impl for videos of different lengths (no splat plan, no explicit PairLayout).
-static int procrustes_fwd_ragged(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                                 float wsens, const int64_t* indices, int num_indices, float* rt, void* ws,
-                                 const Ragged& r, int H, int W, cudaStream_t s, const float* moments_k4, bool solve) {
-  if (!depth || !k4 || !backward_flow || (!rt && solve) || !ws) return fail_msg("fm_procrustes_fwd: bad arguments");
-  if (indices && num_indices < 1) return fail_msg("fm_procrustes_fwd: empty index set");
-  const int BP = r.T - r.B;
-  Workspace w = carve_rows(ws, r.B, r.T, BP);
-  const RaggedPairs lay{r.v};
-  if (moments_k4) {  // fm_procrustes_moments_videos already ran with those intrinsics
-    if (indices) return fail_msg("fm_procrustes_fwd: precomputed moments serve the dense path");
-    if (!solve) return 0;
-    k_solve_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, moments_k4, k4);
-    FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve_ragged");
-    return 0;
-  }
-  cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
-  k_pair_shift_ragged<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift_ragged");
-  if (indices) {
-    dim3 grid(blocks_for_points(num_indices), BP);
-    k_moments_ragged<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights, indices, num_indices, w.moments, w.zshift, wsens, lay, H, W);
-  } else if (patch_shape_ok(H, W)) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_moments_dense_ragged<4, kPatchLanes><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
-  } else if (W % 4 == 0) {
-    const long long items = (long long)BP * ((H * W + kThreads * 4 - 1) / (kThreads * 4));
-    const int pg = persistent_grid(3, items);
-    k_moments_dense_ragged<4, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items, pg, true));
-  } else {
-    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
-    const int pg = persistent_grid(3, items);
-    k_moments_dense_ragged<1, 0><<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights, w.moments, w.zshift, wsens, lay, H, W, BP, procrustes_rounds(H, W, items / 4, pg, true));
-  }
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_moments_ragged");
-  if (!solve) return 0;
-  k_solve_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, nullptr, nullptr);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve_ragged");
-  return 0;
-}
-
-// procrustes_bwd_impl of a whole step (flow loss included, unscaled) for videos of different lengths.
-static int procrustes_bwd_ragged(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                                 float wsens, const int64_t* indices, int num_indices, const float* g_rt,
-                                 float* g_depth, float* g_weights, float* g_k4, void* ws, const Ragged& r, int H, int W,
-                                 cudaStream_t s, const AdamFuse* adam) {
-  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws) return fail_msg("fm_procrustes_bwd: bad arguments");
-  const int BP = r.T - r.B;
-  Workspace w = carve_rows(ws, r.B, r.T, BP);
-  const RaggedPairs lay{r.v};
-  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)r.T * 4 * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
-  AdamFuse af;
-  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
-  float* weights_rw = const_cast<float*>(weights);
-  k_adjoint_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 1, nullptr, w.adj, BP, r.v);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint_ragged");
-  if (indices) {
-    dim3 grid(blocks_for_points(num_indices), BP);
-    k_distribute_ragged<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
-  } else if (W % 4 == 0) {
-    const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
-    const int pg = persistent_grid(FM_WIN_CTAS, items);
-    const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);
-    k_distribute_window_ragged<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
-  } else {
-    const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
-    const int pg = persistent_grid(3, items);
-    k_distribute_dense_ragged<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
-  }
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute_ragged");
-  k_k4_finalize_ragged<<<(r.T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, 1, nullptr, g_k4, r.T, r.v);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize_ragged");
-  return 0;
+  return procrustes_fwd(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, 1, F,
+                        dense_layout(F, H, W), H, W, (cudaStream_t)stream, nullptr, /*solve=*/false);
 }
 
 int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward_flow,
@@ -3423,9 +3365,9 @@ int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward
                       const float* g_rt, int include_flow_loss, const float* flow_scale,
                       float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int F, int H,
                       int W, void* stream) {
-  return procrustes_bwd_impl(depth, k4, backward_flow, weights, 0.f, indices, num_indices, g_rt,
-                             include_flow_loss, flow_scale, g_depth, g_weights, g_k4, ws, B, F, H, W,
-                             stream);
+  return procrustes_bwd(depth, k4, backward_flow, weights, 0.f, indices, num_indices, g_rt, include_flow_loss,
+                        flow_scale, g_depth, g_weights, g_k4, ws, B, B * F, dense_layout(F, H, W), H, W,
+                        (cudaStream_t)stream, nullptr, /*depth_prescaled=*/false);
 }
 
 size_t fm_splat_plan_bytes(int F, int H, int W) {
@@ -3486,8 +3428,8 @@ int fm_procrustes_fwd_planned(const float* depth, const float* k4, const float* 
                               float weight_sensitivity, void* plan, float* rt, void* ws, int F, int H, int W,
                               void* stream) {
   if (!plan) return fail_msg("fm_procrustes_fwd_planned: plan missing");
-  return procrustes_fwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, rt, ws, 1, F, H, W,
-                             stream, nullptr, plan);
+  return procrustes_fwd_planned(depth, k4, backward_flow, weights, weight_sensitivity, plan, rt, ws, F, H, W,
+                                (cudaStream_t)stream);
 }
 
 int fm_procrustes_bwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
@@ -3495,9 +3437,9 @@ int fm_procrustes_bwd_planned(const float* depth, const float* k4, const float* 
                               int include_flow_loss, float* g_depth, float* g_weights, float* g_k4, void* ws, int F,
                               int H, int W, void* stream) {
   if (!plan) return fail_msg("fm_procrustes_bwd_planned: plan missing");
-  return procrustes_bwd_impl(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, g_rt, include_flow_loss,
-                             nullptr, g_depth, g_weights, g_k4, ws, 1, F, H, W, stream, nullptr, nullptr, plan,
-                             plan_overflow_max);
+  return procrustes_bwd_planned(depth, k4, backward_flow, weights, weight_sensitivity, plan, plan_overflow_max, g_rt,
+                                include_flow_loss, nullptr, g_depth, g_weights, g_k4, ws, F, H, W,
+                                (cudaStream_t)stream, nullptr);
 }
 
 int fm_mask_sum(const float* forward_mask, const float* backward_mask, double* out, size_t count, void* stream) {
@@ -3895,128 +3837,13 @@ size_t fm_softmin_workspace_bytes(int B, int num_candidates) {
          align_up((items * 12 + (items + B) * 8) * sizeof(float), 256);
 }
 
-namespace {
-PairLayout sweep_layout(int F, int H, int W, int cand) {
-  PairLayout l = dense_layout(F, H, W);  // strides of the REAL tensors
-  l.F = 2;                               // the sweep only sees frames 0 and 1 (pair 0)
-  l.cand = cand;
-  return l;
-}
-}  // namespace
-
-// vids != NULL: videos of different lengths (each video's pair 0 through RaggedSweep; F is unused)
-static int sweep_fwd_impl(const float* depth, const float* weights, float weight_sensitivity,
-                          const float* backward_flow, const int64_t* indices, int num_indices,
-                          const float* cand_k4, int num_candidates, float* err, float* rt, void* ws, int B,
-                          int F, int H, int W, void* stream, const Videos* vids = nullptr) {
-  if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 ||
-      !err || !rt || !ws || bad_dims(B, F, H, W))
-    return fail_msg("fm_softmin_sweep_fwd: bad arguments");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int items = B * num_candidates;
-  const PairLayout lay = sweep_layout(F, H, W, num_candidates);
-  const PairLayout lay1 = sweep_layout(F, H, W, 1);
-  Workspace w = carve(ws, items + B, 2);
-  float* scratch = (float*)((char*)ws + align_up(w.bytes, 256));
-  float* base_k4 = scratch + (size_t)items * 12 + (size_t)items * 8;  // after g_rt and g_k4 of the bwd
-  double* base_moments = w.moments + (size_t)items * kNumMoments;
-  cudaError_t e = cudaMemsetAsync(base_moments, 0, (size_t)B * kNumMoments * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
-  k_sweep_base_k4<<<(B * 8 + 127) / 128, 128, 0, s>>>(cand_k4, base_k4, B, num_candidates);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_base_k4");
-  float* base_zshift = w.zshift + items;  // one conditioning shift per batch element, for all candidates
-  if (vids) k_pair_shift_ragged<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, RaggedSweep{*vids, 1}, H, W);
-  else k_pair_shift<<<B, kThreads, 0, s>>>(depth, weights, weight_sensitivity, base_zshift, lay1, H, W);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_pair_shift");
-  {  // ONE moment pass (candidate 0); every candidate's moments are a rescaling of it
-    dim3 grid(blocks_for_points(num_indices), B);
-    if (vids)
-      k_moments_ragged<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
-                                                   base_moments, base_zshift, weight_sensitivity, RaggedSweep{*vids, 1},
-                                                   H, W);
-    else
-      k_moments<1><<<grid, kThreads, 0, s>>>(depth, base_k4, backward_flow, weights, indices, num_indices,
-                                            base_moments, base_zshift, weight_sensitivity, lay1, H, W);
-    FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_moments");
-  }
-  k_sweep_scale_solve<<<(items + 63) / 64, 64, 0, s>>>(base_moments, base_zshift, cand_k4, rt, w.state, B,
-                                                      num_candidates);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_scale_solve");
-  e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_softmin_sweep_fwd: memset", e);
-  dim3 grid(blocks_for_points(num_indices), items);
-  if (vids)
-    k_sweep_ragged<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                                   indices, num_indices, nullptr, w.flowacc, nullptr, nullptr,
-                                                   RaggedSweep{*vids, num_candidates}, H, W);
-  else
-    k_sweep<false><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                            indices, num_indices, nullptr, w.flowacc, nullptr, nullptr, lay,
-                                            H, W);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep");
-  k_sweep_out<<<(items + 127) / 128, 128, 0, s>>>(w.flowacc, err, items, 0, 1);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_fwd: k_sweep_out");
-  return 0;
-}
-
 int fm_softmin_sweep_fwd(const float* depth, const float* weights, float weight_sensitivity,
                          const float* backward_flow, const int64_t* indices, int num_indices,
                          const float* cand_k4, int num_candidates, float* err, float* rt, void* ws, int B,
                          int F, int H, int W, void* stream) {
   return sweep_fwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
-                        num_candidates, err, rt, ws, B, F, H, W, stream);
-}
-
-static int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensitivity,
-                          const float* backward_flow, const int64_t* indices, int num_indices,
-                          const float* cand_k4, int num_candidates, const float* rt, const float* g_err,
-                          float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
-                          void* stream, const Videos* vids = nullptr) {
-  if (!depth || !backward_flow || !indices || num_indices < 1 || !cand_k4 || num_candidates < 1 || !rt ||
-      !g_err || !g_depth || !ws || bad_dims(B, F, H, W))
-    return fail_msg("fm_softmin_sweep_bwd: bad arguments");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int items = B * num_candidates;
-  const PairLayout lay = sweep_layout(F, H, W, num_candidates);
-  const PairLayout lay1 = sweep_layout(F, H, W, 1);
-  Workspace w = carve(ws, items + B, 2);
-  float* scratch = (float*)((char*)ws + align_up(w.bytes, 256));
-  float* g_rt = scratch;
-  float* base_k4 = scratch + (size_t)items * 12 + (size_t)items * 8;
-  cudaError_t e = cudaMemsetAsync(w.flowacc, 0, (size_t)items * kSweepAcc * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_softmin_sweep_bwd: memset", e);
-  e = cudaMemsetAsync(w.k4acc, 0, (size_t)(items + B) * 2 * 4 * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_softmin_sweep_bwd: memset", e);
-  dim3 grid(blocks_for_points(num_indices), items);
-  if (vids)
-    k_sweep_ragged<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                                  indices, num_indices, g_err, w.flowacc, g_depth, g_weights,
-                                                  RaggedSweep{*vids, num_candidates}, H, W);
-  else
-    k_sweep<true><<<grid, kThreads, 0, s>>>(depth, cand_k4, rt, backward_flow, weights, weight_sensitivity,
-                                           indices, num_indices, g_err, w.flowacc, g_depth, g_weights, lay, H,
-                                           W);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep");
-  k_sweep_out<<<(items * 12 + 127) / 128, 128, 0, s>>>(w.flowacc, g_rt, items, 1, 12);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_out");
-  // per-candidate adjoint constants, collapsed into one per batch element, then ONE distribution pass
-  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, 2);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_adjoint");
-  k_sweep_aggregate<<<B, 32, 0, s>>>(w.adj, cand_k4, w.adj + items, B, num_candidates);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_aggregate");
-  AdamFuse af;
-  memset(&af, 0, sizeof(af));
-  dim3 grid1(blocks_for_points(num_indices), B);
-  if (vids)
-    k_distribute_ragged<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights),
-                                                     indices, num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
-                                                     weight_sensitivity, RaggedSweep{*vids, 1}, af, H, W);
-  else
-    k_distribute<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights), indices,
-                                              num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
-                                              weight_sensitivity, lay1, af, H, W);
-  FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_distribute");
-  return 0;
+                        num_candidates, err, rt, ws, B, F, H, W, stream, sweep_layout(F, H, W, num_candidates),
+                        sweep_layout(F, H, W, 1));
 }
 
 int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_sensitivity,
@@ -4025,7 +3852,8 @@ int fm_softmin_sweep_bwd(const float* depth, const float* weights, float weight_
                          float* g_depth, float* g_weights, void* ws, int B, int F, int H, int W,
                          void* stream) {
   return sweep_bwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
-                        num_candidates, rt, g_err, g_depth, g_weights, ws, B, F, H, W, stream);
+                        num_candidates, rt, g_err, g_depth, g_weights, ws, B, F, H, W, stream,
+                        sweep_layout(F, H, W, num_candidates), sweep_layout(F, H, W, 1));
 }
 
 int fm_softmin_focal(const float* err, const float* cand_focal, int num_candidates, int B, float* softmin,
@@ -4104,6 +3932,8 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
   // the splat plan of this video's backward flows serves the dense path (all-pixel Procrustes)
   void* plan = (!rag && a->splat_plan && !a->indices && tiled_shape_ok(F, H, W)) ? a->splat_plan : nullptr;
+  // runs a Procrustes launcher on the pairs of the packed videos or of the one video
+  auto on_pairs = [&](auto launch) { return rag ? launch(RaggedPairs{rag->v}) : launch(dense_layout(F, H, W)); };
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
@@ -4115,14 +3945,13 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
-    if (rag) {
-      if ((rc = procrustes_fwd_ragged(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
-                                      a->num_indices, a->rt, a->ws, *rag, H, W, s,
-                                      a->indices ? nullptr : a->moments_k4, true)))
-        return rc;
-    } else if ((rc = procrustes_fwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                  a->indices, a->num_indices, a->rt, a->ws, 1, F, H, W, stream, nullptr, plan,
-                                  (a->indices || plan) ? nullptr : a->moments_k4)))
+    if ((rc = plan ? procrustes_fwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
+                                            a->rt, a->ws, F, H, W, s)
+                   : on_pairs([&](const auto& lay) {
+                       return procrustes_fwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
+                                             a->indices, a->num_indices, a->rt, a->ws, B, (int)TF, lay, H, W, s,
+                                             a->indices ? nullptr : a->moments_k4, /*solve=*/true);
+                     })))
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
     // two branches of the step (the tracking sweep is issue-bound, the flow kernel waits on memory:
@@ -4262,15 +4091,16 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     af.step_size = (float)(a->lr / (1.0 - pow(a->beta1, (double)a->step)));
     af.bc2_sqrt = (float)sqrt(1.0 - pow(a->beta2, (double)a->step));
   }
-  if (rag) {
-    if ((rc = procrustes_bwd_ragged(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
-                                    a->num_indices, g_rt, a->g_depth, a->g_weights, a->g_k4, a->ws, *rag, H, W, s,
-                                    fuse_w ? &af : nullptr)))
-      return rc;
-  } else if ((rc = procrustes_bwd_impl(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
-                                a->g_k4, a->ws, 1, F, H, W, stream, nullptr, fuse_w ? &af : nullptr, plan,
-                                a->splat_overflow_max, /*depth_prescaled=*/fscale != nullptr)))
+  // g_depth was scaled by fscale above
+  if ((rc = plan ? procrustes_bwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
+                                          a->splat_overflow_max, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4,
+                                          a->ws, F, H, W, s, fuse_w ? &af : nullptr)
+                 : on_pairs([&](const auto& lay) {
+                     return procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
+                                           a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
+                                           a->g_k4, a->ws, B, (int)TF, lay, H, W, s, fuse_w ? &af : nullptr,
+                                           /*depth_prescaled=*/true);
+                   })))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   // Adam (model_wrapper_overfit.py:104-105)
@@ -4324,8 +4154,8 @@ int fm_procrustes_moments_videos(const float* depth, const float* k4, const floa
                                  void* stream) {
   Ragged r;
   if (ragged_of(layout, &r) || bad_dims(1, 2, H, W)) return fail_msg("fm_procrustes_moments_videos: bad arguments");
-  return procrustes_fwd_ragged(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, r, H, W,
-                               (cudaStream_t)stream, nullptr, /*solve=*/false);
+  return procrustes_fwd(depth, k4, backward_flow, weights, weight_sensitivity, nullptr, 0, nullptr, ws, r.B, r.T,
+                        RaggedPairs{r.v}, H, W, (cudaStream_t)stream, nullptr, /*solve=*/false);
 }
 
 int fm_softmin_sweep_fwd_videos(const float* depth, const float* weights, float weight_sensitivity,
@@ -4335,7 +4165,8 @@ int fm_softmin_sweep_fwd_videos(const float* depth, const float* weights, float 
   Ragged r;
   if (ragged_of(layout, &r)) return fail_msg("fm_softmin_sweep_fwd_videos: bad video layout");
   return sweep_fwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
-                        num_candidates, err, rt, ws, r.B, 2, H, W, stream, &r.v);
+                        num_candidates, err, rt, ws, r.B, 2, H, W, stream, RaggedSweep{r.v, num_candidates},
+                        RaggedSweep{r.v, 1});
 }
 
 int fm_softmin_sweep_bwd_videos(const float* depth, const float* weights, float weight_sensitivity,
@@ -4346,7 +4177,8 @@ int fm_softmin_sweep_bwd_videos(const float* depth, const float* weights, float 
   Ragged r;
   if (ragged_of(layout, &r)) return fail_msg("fm_softmin_sweep_bwd_videos: bad video layout");
   return sweep_bwd_impl(depth, weights, weight_sensitivity, backward_flow, indices, num_indices, cand_k4,
-                        num_candidates, rt, g_err, g_depth, g_weights, ws, r.B, 2, H, W, stream, &r.v);
+                        num_candidates, rt, g_err, g_depth, g_weights, ws, r.B, 2, H, W, stream,
+                        RaggedSweep{r.v, num_candidates}, RaggedSweep{r.v, 1});
 }
 
 int fm_adam_step_clock_frames_videos(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,

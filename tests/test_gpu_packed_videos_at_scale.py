@@ -1,5 +1,5 @@
-"""The packed multi-video step (FusedOverfitter on a list of videos: fm_overfit_step_videos and its `_ragged`
-kernels) at the shapes where its persistent grids cross pairs and videos.
+"""The packed multi-video step (FusedOverfitter on a list of videos: fm_overfit_step_videos and its kernels on
+the packed layout) at the shapes where its persistent grids cross pairs and videos.
 
 A persistent ragged kernel hands every block a contiguous range of items (pixel chunks or window tiles of
 one pair or frame).  Where a range runs into the next pair, the block restages that pair's constants
@@ -74,9 +74,9 @@ def _walk(units, per_unit, grid, rounds, video):
 
 
 def launch_geometry(frames, h, w, sms, l2_bytes=L2_BYTES):
-    """{kernel: (rounds, multi, cross)} of the persistent launches of procrustes_fwd_ragged
-    (k_moments_dense_ragged), launch_flow_ragged (k_flow_lean_ragged) and procrustes_bwd_ragged
-    (k_distribute_window_ragged for W % 4 == 0, else k_distribute_dense_ragged) in fm_kernels.cu:
+    """{kernel: (rounds, multi, cross)} of the persistent launches of procrustes_fwd<RaggedPairs>
+    (k_moments_dense<..., RaggedPairs>), launch_flow_ragged (k_flow_lean_ragged) and procrustes_bwd<RaggedPairs>
+    (k_distribute_window<RaggedPairs> for W % 4 == 0, else k_distribute_dense<RaggedPairs>) in fm_kernels.cu:
     256-thread chunks of 4 pixels (W % 4 == 0) or 1, 64 x 32 window tiles, 3 / 2 / 3 blocks per SM."""
     pair_video = [b for b, f in enumerate(frames) for _ in range(f - 1)]
     frame_video = [b for b, f in enumerate(frames) for _ in range(f)]
