@@ -1718,7 +1718,7 @@ k_adam_frames_ragged(float* __restrict__ p, const float* __restrict__ g, float* 
 // gradient scale is only known after a full pass.  Everything is therefore accumulated
 // unscaled in ONE sweep over the (source, target, point) triples and scaled at the end:
 //   k_track_src     work item = (segment, source row, half of its points): bilinear-sample xyz at the track
-//                   location, lift to world space, loop over the segment's target rows:
+//                   location, lift to world axes about the source camera, loop over the segment's target rows:
 //                   loss sum + valid count, the unscaled camera-space adjoint of the sampled
 //                   point (stored per sample), source-frame K / pose-twist sums in registers,
 //                   target-frame K / pose-twist sums by a recursive-halving warp reduction per
@@ -1749,22 +1749,29 @@ __device__ __forceinline__ SegInfo load_seg(const int* seg, int s) {
 // Per-frame record: R (9, row-major, camera-to-world), t (3), c = -R^T t (3), fx fy cx cy ifx ify,
 // 3 pad -- kTrackRec floats, 16-byte aligned, so that a warp reads a record with six broadcast
 // 16-byte shared-memory loads (TrackRec).
+// The records are staged per work item with the world origin moved to the item's source camera
+// (source_frame): t = t_frame - t_source and c = -R^T t, both in double.  The twists take lever arms
+// X - t, which do not depend on the origin, and the source points lift to R_s q, so no float32
+// quantity carries the camera's distance from frame 0 (|t| of tens against depths of a few units)
+// and cancels it again.
 __device__ __forceinline__ void load_segment_frames(float* sm, const float* ext, const float* k4,
-                                                    const SegInfo& si) {
+                                                    const SegInfo& si, int source_frame) {
+  const float* Ps = ext + (size_t)source_frame * 16;
   for (int row = threadIdx.x; row < si.rows; row += blockDim.x) {
     const float* P = ext + (size_t)(si.start_frame + row) * 16;
     float* o = sm + row * kTrackRec;
     float v[kTrackRec];
     float* R = v;
-    float* t = v + 9;
+    double t[3];
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       R[i * 3 + 0] = __ldg(P + i * 4 + 0); R[i * 3 + 1] = __ldg(P + i * 4 + 1); R[i * 3 + 2] = __ldg(P + i * 4 + 2);
-      t[i] = __ldg(P + i * 4 + 3);
+      t[i] = (double)__ldg(P + i * 4 + 3) - (double)__ldg(Ps + i * 4 + 3);
+      v[9 + i] = (float)t[i];
     }
 #pragma unroll
     for (int i = 0; i < 3; ++i)
-      v[12 + i] = -(R[0 * 3 + i] * t[0] + R[1 * 3 + i] * t[1] + R[2 * 3 + i] * t[2]);
+      v[12 + i] = (float)-((double)R[0 * 3 + i] * t[0] + (double)R[1 * 3 + i] * t[1] + (double)R[2 * 3 + i] * t[2]);
     const float4 k = __ldg(reinterpret_cast<const float4*>(k4) + si.start_frame + row);
     v[15] = k.x; v[16] = k.y; v[17] = k.z; v[18] = k.w; v[19] = 1.0f / k.x; v[20] = 1.0f / k.y;
     v[21] = v[22] = v[23] = 0.f;
@@ -1926,7 +1933,7 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
     const SegInfo si = load_seg(seg, srow / max_rows);
     const int row = srow % max_rows;
     if (row >= si.rows || !sh.owns(si.start_frame + row)) continue;
-    load_segment_frames(sm, ext, k4, si);
+    load_segment_frames(sm, ext, k4, si, si.start_frame + row);
     float* tgt = s_tgt + (size_t)warp * si.rows * kTrackAcc;
     for (int i = lane; i < si.rows * kTrackAcc; i += 32) tgt[i] = 0.f;
     __syncwarp();
@@ -1977,7 +1984,7 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
       const int npass = (total + kTrackPass - 1) / kTrackPass;
       for (int ps = warp; ps < npass; ps += NW) {  // warp-uniform: the shuffles below need all 32 lanes
         const int pb = ps * kTrackPass + lane;
-        // lift the pass's source points to world space
+        // lift the pass's source points to world axes, origin at the source camera (load_segment_frames)
         float Xw[kTrackPPT][3];
         int ix[kTrackPPT];  // sample offset within the segment: row ft of point p is p + ft * n
         {

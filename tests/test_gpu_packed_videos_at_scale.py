@@ -159,6 +159,11 @@ ORACLE_CASES = {
     "two-360x640-regressed": ("two-360x640", ("scene", "scale_small"), {}),
 }
 _FLOW_NAMES = ("forward", "backward", "forward_mask", "backward_mask")
+# Regimes whose 41-row segments the float32 oracle cannot place: its own position error (on the 200- and
+# 1000-deep pixels, and under the divergent `zoom` flow) sets a guard band that clears more than 1 % of their
+# samples on the LLFF cases -- `horizon` 1.4 % (all pixels) to 22 % (1000 Procrustes points), `zoom` 3 %,
+# `centre_far` 5.3 % (1000 points).  They keep 9 rows.
+SHORT_SEGMENT_KINDS = ("horizon", "zoom", "centre_far")
 
 
 def _regime_video(kind, f, h, w, seed, focal_scale):
@@ -175,10 +180,9 @@ def _regime_video(kind, f, h, w, seed, focal_scale):
     assert bool(torch.isfinite(depth).all()), (kind, f, seed)
     if ext is not None:
         tracks = O.scene_tracks(depth[0], ext, focal, [(0, f), (2, 3), (f - 2, 2)], n_points=600, seed=seed)
-    else:
-        # segments of 9 rows: with the reference's 41 (radius 20), uniform random tracks under the coherent
-        # `shift` motion of a 42-frame video put one frame's depth gradient 20x past the float32 oracle's error
-        tracks = O.synthetic_tracks(f, n_points=300, interval=5, radius=4, seed=seed, dtype=torch.float64)
+    else:  # the reference's segments, 41 rows, guarded by the tests (_guard_video); 9 rows in SHORT_SEGMENT_KINDS
+        tracks = O.synthetic_tracks(f, n_points=300, interval=5, radius=4 if kind in SHORT_SEGMENT_KINDS else 20,
+                                    seed=seed, dtype=torch.float64)
     depth, focal = start_point(depth, focal, seed=seed + 1)
     return dict(kind=kind, depth=depth[0], wparam=wparam[0], flows=fl, focal=focal * focal_scale, tracks=tracks,
                 depth_regime=kind in O.DEPTH_REGIMES)
@@ -209,15 +213,44 @@ def _packed_optimiser(cfg, videos):
     return o
 
 
-def _oracle(v, kw, dt, steps=1, **step_kw):
-    """OverfitOracle on video v alone in dtype dt: the oracle and its first `steps` training steps."""
+def _oracle_model(v, kw, dt):
+    """OverfitOracle on video v alone in dtype dt, at v's start point, and v's flows in dt."""
     from oracle import flowmap_oracle as O
     f, h, w = v["depth"].shape
     st = O.OverfitOracle(O.OverfitConfig(initial_focal=v["focal"], **kw), f, h, w, dtype=dt)
     with torch.no_grad():
         st.depth.copy_(v["depth"].to(dt))
         st.weights.copy_(v["wparam"].to(dt))
-    flows = O.Flows(*(getattr(v["flows"], n).to(dt) for n in _FLOW_NAMES))
+    return st, O.Flows(*(getattr(v["flows"], n).to(dt) for n in _FLOW_NAMES))
+
+
+def _guard_video(v, kw, **forward_kw):
+    """v with its tracks guarded by track_travel_checks.clear_track_kinks at the poses and intrinsics of step 0 of
+    its float64 oracle, the band from the float32 oracle's position error.  Under a long coherent motion the
+    41-row segments cross the [0,1)^2 border ~1e5 times, and a target within rounding of it is valid in one
+    precision and not in the other: a whole saturated Huber term at four depth taps of one frame."""
+    import track_travel_checks as T
+    from oracle import flowmap_oracle as O
+    if v["kind"] in SHORT_SEGMENT_KINDS:
+        return v  # 9-row segments, as before the guard: the float32 oracle's band there is the problem
+    triples = {}
+    for dt in (torch.float64, torch.float32):
+        st, flows = _oracle_model(v, kw, dt)
+        with torch.no_grad():
+            m = st.forward(flows, 0, **forward_kw)
+            triples[dt] = T.track_triples(m.surfaces, m.extrinsics, m.intrinsics,
+                                          [O.Tracks(t.xy.to(dt), t.visibility, t.start_frame) for t in v["tracks"]])
+    band = T.position_band(triples[torch.float64], triples[torch.float32], v["tracks"])
+    tracks, cleared = T.clear_track_kinks(v["tracks"], triples[torch.float64], band)
+    samples = sum(int(t.visibility.sum()) for t in v["tracks"])
+    assert cleared <= 0.01 * samples, (v["kind"], "guard cleared", cleared, samples)
+    return dict(v, tracks=tracks)
+
+
+def _oracle(v, kw, dt, steps=1, **step_kw):
+    """OverfitOracle on video v alone in dtype dt: the oracle and its first `steps` training steps."""
+    from oracle import flowmap_oracle as O
+    st, flows = _oracle_model(v, kw, dt)
     tracks = [O.Tracks(t.xy.to(dt), t.visibility, t.start_frame) for t in v["tracks"]] \
         if kw.get("use_tracking") else None
     out = []
@@ -280,8 +313,12 @@ def test_packed_step_vs_float64_oracle_per_video(case):
     geometry_case, kinds, extra = ORACLE_CASES[case]
     if "procrustes_points" not in extra:
         _device_geometry(geometry_case)
-    videos = _regime_videos(geometry_case, kinds)
+    from oracle import flowmap_oracle as O
     kw = dict(intrinsics="regressed", use_tracking=True, tracking_enable_after=0, **extra)
+    h, w = GEOMETRY[geometry_case][1:3]
+    idx = None if "procrustes_points" not in extra else \
+        O.procrustes_indices(h, w, extra["procrustes_points"], False, device="cuda").cpu()
+    videos = [_guard_video(v, kw, procrustes_idx=idx) for v in _regime_videos(geometry_case, kinds)]
     o = _packed_optimiser(OverfitCfg(**kw), videos)
     pts = None if o._indices is None else o._indices.cpu()  # the oracle gets the device's point set
     total, _ = o.training_step(update=False)
@@ -301,11 +338,11 @@ def test_packed_softmin_stage_vs_float64_oracle_per_video():
     ragged sweep's forward and backward, and the per-video frame Adam."""
     from flowmap_b200.overfit import OverfitCfg
     _device_geometry("llff-176x224")
-    videos = _regime_videos("llff-176x224", KINDS)
-    h, w = videos[0]["depth"].shape[-2:]
+    h, w = GEOMETRY["llff-176x224"][1:3]
     kw = dict(intrinsics="softmin", regression_after=None, use_tracking=True, tracking_enable_after=0)
-    o = _packed_optimiser(OverfitCfg(**kw), videos)
     sweep_idx = torch.randperm(h * w, generator=torch.Generator().manual_seed(35))[:8192].cuda()
+    videos = [_guard_video(v, kw, softmin_indices=sweep_idx.cpu()) for v in _regime_videos("llff-176x224", KINDS)]
+    o = _packed_optimiser(OverfitCfg(**kw), videos)
     o.injected_indices = sweep_idx
     label = "packed softmin llff-176x224"
     total, _ = o.training_step(update=False)

@@ -811,6 +811,13 @@ def test_pose_chain_scan_vs_sequential_float64(b, f):
     assert rel_l2(rt.grad.cpu(), T.grad[..., :3, :]) <= 1e-5
 
 
+def twist(rot, g):
+    """Left-perturbation twist (F, 6) of an ambient pose gradient g (1, F, 4, 4) at rotations rot (F, 3, 3):
+    omega = sum_c R_c x G_c, v = G_t."""
+    om = torch.linalg.cross(rot.transpose(-1, -2), g[0, :, :3, :3].transpose(-1, -2), dim=-1).sum(dim=-2)
+    return torch.cat((om, g[0, :, :3, 3]), dim=-1)
+
+
 def test_tracking_per_frame_intrinsics_gradient_and_shared_mode():
     """Tracking loss with PER-FRAME intrinsics (different k4 rows): d loss / d k4 per frame against the
     float64 oracle (general kernel variant); and the shared-intrinsics variant must give the same
@@ -857,16 +864,11 @@ def test_tracking_per_frame_intrinsics_gradient_and_shared_mode():
         out[shared] = (float(loss), d.grad.cpu(), e.grad.cpu(), k.grad.cpu())
     g_focal_frames = focal.grad  # per-frame d loss / d focal_i
     rot = ext.detach()[0, :, :3, :3]
-
-    def twist(g):  # left-perturbation twist of an ambient pose gradient: omega = sum_c R_c x G_c, v = G_t
-        om = torch.linalg.cross(rot.transpose(-1, -2), g[0, :, :3, :3].transpose(-1, -2), dim=-1).sum(dim=-2)
-        return torch.cat((om, g[0, :, :3, 3]), dim=-1)
-
     for shared in (False, True):
         loss, gd, ge, gk = out[shared]
         assert abs(loss - float(ref)) <= 1e-4 * abs(float(ref))
         assert rel_l2(gd, depth.grad) <= 2e-4
-        assert rel_l2(twist(ge.double()), twist(ext.grad)) <= 2e-4   # only the tangent part is defined
+        assert rel_l2(twist(rot, ge.double()), twist(rot, ext.grad)) <= 2e-4   # only the tangent part is defined
     per_frame = out[False][3][0, :, 0].double() * s / w + out[False][3][0, :, 1].double() * s / h
     assert rel_l2(per_frame, g_focal_frames) <= 2e-4
     total = lambda gk: float((gk[0, :, 0].double() * s / w + gk[0, :, 1].double() * s / h).sum())  # noqa: E731
