@@ -99,9 +99,17 @@ Workspace carve(void* base, int B, int F) { return carve_rows(base, B, (size_t)B
 // Videos of different lengths packed along the frame axis (fm_video_layout): video b owns the frames
 // [frame_offset[b], frame_offset[b + 1]) of the (T, ...) buffers and the pairs [frame_offset[b] - b,
 // frame_offset[b + 1] - b - 1) of the (P, ...) ones, P = T - B.  Pair p of video b joins frames p + b and
-// p + b + 1, so no pair crosses two videos.  The ragged kernels find a frame's or a pair's video in these
-// tables where their uniform siblings divide by F or F - 1.
+// p + b + 1, so no pair crosses two videos.  The per-frame and per-video kernels are templated on the video
+// layout: Videos, or Uniform below, and find a frame's or a pair's video through these accessors.
+// Scale: how a layout's kernels take d total / d loss.  Packed videos run only whole steps, so their loss
+// gradients are never scaled (NoScale); one video also runs split phases, which pass it as a device scalar.
+struct NoScale {
+  __host__ __device__ NoScale(const float*) {}
+};
+__device__ __forceinline__ double scale_of(const float* s) { return s ? (double)*s : 1.0; }
+__device__ __forceinline__ double scale_of(NoScale) { return 1.0; }
 struct Videos {
+  using Scale = NoScale;
   const int* frame_offset;  // [B + 1]
   const int* frame_video;   // [T]
   const int* pair_video;    // [P]
@@ -109,6 +117,16 @@ struct Videos {
   __device__ __forceinline__ int of_pair(int p) const { return __ldg(pair_video + p); }
   __device__ __forceinline__ int first(int b) const { return __ldg(frame_offset + b); }
   __device__ __forceinline__ int frames(int b) const { return __ldg(frame_offset + b + 1) - __ldg(frame_offset + b); }
+};
+// B videos of F frames each in the (B F, ...) and (B (F - 1), ...) buffers: one video (B = 1) and the
+// standalone (B, F) entry points.  Pair p of video b joins frames p + b and p + b + 1, as in Videos.
+struct Uniform {
+  using Scale = const float* __restrict__;
+  int F;
+  __device__ __forceinline__ int of_frame(int t) const { return t / F; }
+  __device__ __forceinline__ int of_pair(int p) const { return p / (F - 1); }
+  __device__ __forceinline__ int first(int b) const { return b * F; }
+  __device__ __forceinline__ int frames(int) const { return F; }
 };
 
 // ---------------------------------------------------------------- small device helpers
@@ -812,18 +830,17 @@ k_flow_lean_ragged(const float* __restrict__ depth, const float* __restrict__ k4
 }
 
 // Rewrites each frame's lean accumulators (slots 0-13) into the standard layout in place.
-template <bool RAGGED>
-__device__ __forceinline__ void flow_lean_convert_body(double* __restrict__ flowacc, const float* __restrict__ rt,
-                                                       const float* __restrict__ k4, int focal_mode, int BF, int F,
-                                                       int H, int W, const Videos& v) {
+template <class Lay>
+__global__ void k_flow_lean_convert(double* __restrict__ flowacc, const float* __restrict__ rt,
+                                    const float* __restrict__ k4, int focal_mode, int T, int H, int W, Lay lay) {
   const int frame = blockIdx.x * blockDim.x + threadIdx.x;
-  if (frame >= BF) return;
-  const int bi = RAGGED ? v.of_frame(frame) : frame / F, i = RAGGED ? frame - v.first(bi) : frame - bi * F;
+  if (frame >= T) return;
+  const int bi = lay.of_frame(frame), i = frame - lay.first(bi);
   double lean[kFlowLeanVals], out[kFlowVals];
   double* row = flowacc + (size_t)frame * kFlowAcc;
   for (int k = 0; k < kFlowLeanVals; ++k) lean[k] = row[k];
-  const int pairF = RAGGED ? frame - bi : bi * (F - 1) + i;
-  const float* rtF = i < (RAGGED ? v.frames(bi) : F) - 1 ? rt + (size_t)pairF * 12 : nullptr;
+  const int pairF = frame - bi;
+  const float* rtF = i < lay.frames(bi) - 1 ? rt + (size_t)pairF * 12 : nullptr;
   const float* rtB = i > 0 ? rt + (size_t)(pairF - 1) * 12 : nullptr;
   const double s = sqrt((double)H * (double)W);
   const double focal = (double)k4[(size_t)frame * 4] * (double)W / s;
@@ -831,21 +848,12 @@ __device__ __forceinline__ void flow_lean_convert_body(double* __restrict__ flow
   for (int k = 0; k < kFlowVals; ++k) row[k] = out[k];
 }
 
-__global__ void k_flow_lean_convert(double* __restrict__ flowacc, const float* __restrict__ rt,
-                                    const float* __restrict__ k4, int focal_mode, int B, int F, int H, int W) {
-  flow_lean_convert_body<false>(flowacc, rt, k4, focal_mode, B * F, F, H, W, Videos{});
-}
-__global__ void k_flow_lean_convert_ragged(double* __restrict__ flowacc, const float* __restrict__ rt,
-                                           const float* __restrict__ k4, int focal_mode, int T, int H, int W,
-                                           Videos v) {
-  flow_lean_convert_body<true>(flowacc, rt, k4, focal_mode, T, 0, H, W, v);
-}
-
-// Assemble dL/d[R|t] of pair p (float64, 12 values) from the per-frame accumulators.
+// Assemble dL/d[R|t] of pair p (float64, 12 values) from the per-frame accumulators.  The pair's earlier
+// frame is p + (its video).
+template <class Lay>
 __device__ inline void flow_pose_grad(const double* flowacc, const PairState* st, const float* rt,
-                                      int pair, int F, double* g) {
-  const int bi = pair / (F - 1), i = pair - bi * (F - 1);
-  const int a = bi * F + i;
+                                      int pair, const Lay& lay, double* g) {
+  const int a = pair + lay.of_pair(pair);
   const double* fa = flowacc + (size_t)a * kFlowAcc;        // forward term lives on frame a
   const double* fb = flowacc + (size_t)(a + 1) * kFlowAcc;  // backward term on frame b
   double R[9];
@@ -854,18 +862,6 @@ __device__ inline void flow_pose_grad(const double* flowacc, const PairState* st
   for (int r = 0; r < 3; ++r) {
     for (int c = 0; c < 3; ++c) g[r * 4 + c] = fa[1 + r * 3 + c] + fb[13 + r * 3 + c];
     g[r * 4 + 3] = fb[22 + r] - (R[r * 3 + 0] * fa[10] + R[r * 3 + 1] * fa[11] + R[r * 3 + 2] * fa[12]);
-  }
-}
-// flow_pose_grad for videos of different lengths: pair p's earlier frame is p + (its video).
-__device__ inline void flow_pose_grad_ragged(const double* flowacc, const PairState* st, int pair, const Videos& v,
-                                             double* g) {
-  const int a = pair + v.of_pair(pair);
-  const double* fa = flowacc + (size_t)a * kFlowAcc;
-  const double* fb = fa + kFlowAcc;
-  for (int r = 0; r < 3; ++r) {
-    for (int c = 0; c < 3; ++c) g[r * 4 + c] = fa[1 + r * 3 + c] + fb[13 + r * 3 + c];
-    g[r * 4 + 3] = fb[22 + r] - (st[pair].R[r * 3 + 0] * fa[10] + st[pair].R[r * 3 + 1] * fa[11] +
-                                 st[pair].R[r * 3 + 2] * fa[12]);
   }
 }
 
@@ -885,7 +881,7 @@ __global__ void k_flow_finalize(const double* __restrict__ flowacc, const float*
   const int BP = B * (F - 1), BF = B * F;
   if (t < BP && g_rt) {
     double g[12];
-    flow_pose_grad(flowacc, nullptr, rt, t, F, g);
+    flow_pose_grad(flowacc, nullptr, rt, t, Uniform{F}, g);
     for (int k = 0; k < 12; ++k) g_rt[(size_t)t * 12 + k] = (float)g[k];
   }
   if (t < BF && g_k4) {
@@ -908,12 +904,12 @@ __global__ void k_flow_finalize(const double* __restrict__ flowacc, const float*
   }
 }
 
-// The packed fused step's flow losses: block b sums the F_b per-frame loss terms of video b (frames from
-// frame_offset[b]) into loss[b], in the order in which k_flow_finalize's block 0 sums them for one video
-// (launched with 128 threads).
-__global__ void k_flow_video_loss_ragged(const double* __restrict__ flowacc, float* __restrict__ loss, Videos v) {
-  const double* acc = flowacc + (size_t)v.first(blockIdx.x) * kFlowAcc;
-  const int F = v.frames(blockIdx.x);
+// The fused step's flow losses: block b sums the F_b per-frame loss terms of video b into loss[b], in the
+// order in which k_flow_finalize's block 0 sums them for one video (launched with 128 threads).
+template <class Lay>
+__global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __restrict__ loss, Lay lay) {
+  const double* acc = flowacc + (size_t)lay.first(blockIdx.x) * kFlowAcc;
+  const int F = lay.frames(blockIdx.x);
   __shared__ double part[32];
   double s = 0.0;
   for (int k = threadIdx.x; k < F; k += blockDim.x) s += acc[(size_t)k * kFlowAcc];
@@ -932,17 +928,18 @@ __global__ void k_flow_video_loss_ragged(const double* __restrict__ flowacc, flo
 // of d loss / d focal is taken from the moment sums (fm_procrustes.cuh) and booked as the
 // equivalent d/dfx of the pair's earlier frame in k4acc -- the per-pixel kernels carry no
 // intrinsics accumulators at all.
+template <class Lay>
 __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* __restrict__ state,
                           const float* __restrict__ g_rt, int include_flow,
                           const float* __restrict__ flow_scale, PairAdjoint* __restrict__ adj, int BP,
-                          int F, const double* __restrict__ focal_moments = nullptr,
+                          Lay lay, const double* __restrict__ focal_moments = nullptr,
                           const float* __restrict__ k4 = nullptr, double* __restrict__ k4acc = nullptr) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   double g[12];
   for (int k = 0; k < 12; ++k) g[k] = 0.0;
   if (include_flow) {
-    flow_pose_grad(flowacc, state, nullptr, pair, F, g);
+    flow_pose_grad(flowacc, state, nullptr, pair, lay, g);
     const double s = flow_scale ? (double)*flow_scale : 1.0;
     for (int k = 0; k < 12; ++k) g[k] *= s;
   }
@@ -951,31 +948,12 @@ __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* _
   if (focal_moments) {
     double dbl[15];
     procrustes_adjoint(state[pair], g, out, dbl);
-    const int bi = pair / (F - 1), a = bi * F + (pair - bi * (F - 1));
+    const int a = pair + lay.of_pair(pair);
     const double fdf = procrustes_focal_log_grad(state[pair], focal_moments + (size_t)pair * kNumMoments, dbl);
     k4acc[(size_t)a * 4] = fdf / (double)k4[(size_t)a * 4];  // f dL/df = fx dL/dfx
   } else {
     procrustes_adjoint(state[pair], g, out);
   }
-  adj[pair] = out;
-}
-
-// k_adjoint for videos of different lengths (no focal_moments: the splat plan serves one video).
-__global__ void k_adjoint_ragged(const double* __restrict__ flowacc, const PairState* __restrict__ state,
-                                 const float* __restrict__ g_rt, int include_flow, const float* __restrict__ flow_scale,
-                                 PairAdjoint* __restrict__ adj, int BP, Videos v) {
-  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
-  if (pair >= BP) return;
-  double g[12];
-  for (int k = 0; k < 12; ++k) g[k] = 0.0;
-  if (include_flow) {
-    flow_pose_grad_ragged(flowacc, state, pair, v, g);
-    const double s = flow_scale ? (double)*flow_scale : 1.0;
-    for (int k = 0; k < 12; ++k) g[k] *= s;
-  }
-  if (g_rt) for (int k = 0; k < 12; ++k) g[k] += (double)g_rt[(size_t)pair * 12 + k];
-  PairAdjoint out;
-  procrustes_adjoint(state[pair], g, out);
   adj[pair] = out;
 }
 
@@ -1335,29 +1313,16 @@ k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, i
 
 #include "fm_tiled.cuh"
 
+template <class Lay>
 __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
                               int include_flow, const float* __restrict__ flow_scale,
-                              float* __restrict__ g_k4, int B, int F) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= B * F) return;
-  double g[4] = {0, 0, 0, 0};
-  if (include_flow) {
-    flow_k4_grad(flowacc, t, F, g);
-    const double s = flow_scale ? (double)*flow_scale : 1.0;
-    for (int k = 0; k < 4; ++k) g[k] *= s;
-  }
-  for (int k = 0; k < 4; ++k) g_k4[(size_t)t * 4 + k] = (float)(g[k] + k4acc[(size_t)t * 4 + k]);
-}
-
-__global__ void k_k4_finalize_ragged(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                                     int include_flow, const float* __restrict__ flow_scale,
-                                     float* __restrict__ g_k4, int T, Videos v) {
+                              float* __restrict__ g_k4, int T, Lay lay) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
   double g[4] = {0, 0, 0, 0};
   if (include_flow) {  // flow_k4_grad on video b's own frames
-    const int b = v.of_frame(t), f0 = v.first(b);
-    flow_k4_grad(flowacc + (size_t)f0 * kFlowAcc, t - f0, v.frames(b), g);
+    const int b = lay.of_frame(t), f0 = lay.first(b);
+    flow_k4_grad(flowacc + (size_t)f0 * kFlowAcc, t - f0, lay.frames(b), g);
     const double s = flow_scale ? (double)*flow_scale : 1.0;
     for (int k = 0; k < 4; ++k) g[k] *= s;
   }
@@ -1518,18 +1483,17 @@ __device__ __forceinline__ Rigid rigid_from_smem(const float* src) {
   return r;
 }
 
-// RAGGED (k_pose_chain_ragged): block b chains video b of the packed layout from its own frame 0.
-template <bool RAGGED>
-__device__ __forceinline__ void pose_chain_body(const float* __restrict__ rt, float* __restrict__ ext, int F,
-                                                const Videos& v) {
+// Block b chains video b from its own frame 0.
+template <class Lay>
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, Lay lay) {
   __shared__ float s_agg[12 * kChainThreads];
   const int b = blockIdx.x, t = threadIdx.x;
-  const int f0 = RAGGED ? v.first(b) : 0;
-  if (RAGGED) F = v.frames(b);
+  const int f0 = lay.first(b), F = lay.frames(b);
   const int P = F - 1;
   const int chunk = (P + kChainThreads - 1) / kChainThreads;
   const int lo = min(t * chunk, P), hi = min(lo + chunk, P);
-  const float* T = RAGGED ? rt + (size_t)(f0 - b) * 12 : rt + (size_t)b * P * 12;
+  const float* T = rt + (size_t)(f0 - b) * 12;
   Rigid agg = rigid_identity();
   for (int k = lo; k < hi; ++k) agg = rigid_mul(agg, rigid_load(T + (size_t)k * 12));
   rigid_to_smem(s_agg + t, agg);
@@ -1542,7 +1506,7 @@ __device__ __forceinline__ void pose_chain_body(const float* __restrict__ rt, fl
     __syncthreads();
   }
   Rigid run = t > 0 ? rigid_from_smem(s_agg + t - 1) : rigid_identity();  // exclusive prefix = P_lo
-  float* o = RAGGED ? ext + (size_t)f0 * 16 : ext + (size_t)b * F * 16;
+  float* o = ext + (size_t)f0 * 16;
   auto store = [o](int k, const Rigid& r) {
     float4* d = reinterpret_cast<float4*>(o + (size_t)k * 16);
     d[0] = make_float4(r.m[0], r.m[1], r.m[2], r.m[3]);
@@ -1557,35 +1521,25 @@ __device__ __forceinline__ void pose_chain_body(const float* __restrict__ rt, fl
   }
 }
 
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain(const float* __restrict__ rt, float* __restrict__ ext, int B, int F) {
-  pose_chain_body<false>(rt, ext, F, Videos{});
-}
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain_ragged(const float* __restrict__ rt, float* __restrict__ ext, Videos v) {
-  pose_chain_body<true>(rt, ext, 0, v);
-}
-
 // Adjoint of the chain.  With G_a = dL/dP_a (top 3 rows; the bottom row is constant):
 //   S_{F-1} = G_{F-1},  S_a = G_a + S_{a+1} T4_a^T,  dT_k = P_k^T S_{k+1} (3x4 part).
 // S_a = f_a(S_{a+1}) with the affine maps f_a(X) = G_a + X T4_a^T, whose composition
 // f_a o f_b (a < b) is the pair (T_a o T_b, G_a + G_b T4_a^T): a reverse (suffix) scan over the
 // elements a = 1 .. F-1, same block layout as the forward chain.
-template <bool RAGGED>
-__device__ __forceinline__ void pose_chain_bwd_body(const float* __restrict__ rt, const float* __restrict__ ext,
-                                                    const float* __restrict__ g_ext, float* __restrict__ g_rt, int F,
-                                                    const Videos& v) {
+template <class Lay>
+__global__ void __launch_bounds__(kChainThreads)
+k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext, const float* __restrict__ g_ext,
+                 float* __restrict__ g_rt, Lay lay) {
   __shared__ float s_t[12 * kChainThreads];
   __shared__ float s_b[12 * kChainThreads];
   const int b = blockIdx.x, t = threadIdx.x;
-  const int f0 = RAGGED ? v.first(b) : 0;
-  if (RAGGED) F = v.frames(b);
+  const int f0 = lay.first(b), F = lay.frames(b);
   const int n = F - 1;                       // elements j = a - 1 for a = 1 .. F-1
   const int chunk = (n + kChainThreads - 1) / kChainThreads;
   const int lo = min(t * chunk, n), hi = min(lo + chunk, n);
-  const float* T = RAGGED ? rt + (size_t)(f0 - b) * 12 : rt + (size_t)b * n * 12;
-  const float* G = RAGGED ? g_ext + (size_t)f0 * 16 : g_ext + (size_t)b * F * 16;
-  const float* Pm = RAGGED ? ext + (size_t)f0 * 16 : ext + (size_t)b * F * 16;
+  const float* T = rt + (size_t)(f0 - b) * 12;
+  const float* G = g_ext + (size_t)f0 * 16;
+  const float* Pm = ext + (size_t)f0 * 16;
   // element j: (T_a, G_a) with a = j + 1; the last one (a = F-1) has no T: identity
   auto elem_t = [T, n](int j) { return j + 1 < n + 0 ? rigid_load(T + (size_t)(j + 1) * 12) : rigid_identity(); };
   Rigid aggT = rigid_identity(), aggB;
@@ -1624,7 +1578,7 @@ __device__ __forceinline__ void pose_chain_bwd_body(const float* __restrict__ rt
 #pragma unroll
     for (int i = 0; i < 12; ++i) S.m[i] = 0.f;
   }
-  float* out = RAGGED ? g_rt + (size_t)(f0 - b) * 12 : g_rt + (size_t)b * n * 12;
+  float* out = g_rt + (size_t)(f0 - b) * 12;
   for (int j = hi - 1; j >= lo; --j) {
     const Rigid tj = elem_t(j), gj = rigid_load(G + (size_t)(j + 1) * 16);
     const Rigid moved = mul_transposed(S, tj);
@@ -1642,17 +1596,6 @@ __device__ __forceinline__ void pose_chain_bwd_body(const float* __restrict__ rt
     d[1] = make_float4(v[4], v[5], v[6], v[7]);
     d[2] = make_float4(v[8], v[9], v[10], v[11]);
   }
-}
-
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain_bwd(const float* __restrict__ rt, const float* __restrict__ ext,
-                 const float* __restrict__ g_ext, float* __restrict__ g_rt, int B, int F) {
-  pose_chain_bwd_body<false>(rt, ext, g_ext, g_rt, F, Videos{});
-}
-__global__ void __launch_bounds__(kChainThreads)
-k_pose_chain_bwd_ragged(const float* __restrict__ rt, const float* __restrict__ ext,
-                        const float* __restrict__ g_ext, float* __restrict__ g_rt, Videos v) {
-  pose_chain_bwd_body<true>(rt, ext, g_ext, g_rt, 0, v);
 }
 
 // torch.optim.Adam (single-tensor, no amsgrad / weight decay), same operation order.
@@ -1900,18 +1843,32 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
   return ((size_t)max_rows * (kTrackRec + (kTrackThreads / 32) * kTrackAcc) + (size_t)list_cap) * sizeof(float);
 }
 
-// RAGGED (several videos packed along the frame axis, fm_overfit_step_videos): the video of a segment is
-// frame_video[its start frame], and that video's loss sum / valid count go to sums[2 b], sums[2 b + 1].
-template <bool SHARED_K, bool RAGGED>
-__device__ __forceinline__ void track_src_body(const float* __restrict__ depth, const float* __restrict__ k4,
-                                               const float* __restrict__ ext, const int* __restrict__ seg,
-                                               const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
-                                               int mapping, float delta, double* __restrict__ sums,
-                                               unsigned char* __restrict__ flag, float* __restrict__ dq_out,
-                                               double* __restrict__ trackacc, int* __restrict__ next_item,
-                                               int num_items, int max_rows, int list_cap, int H, int W,
-                                               TrackShard sh, float4* sm4, double* red, int* s_wbase, int* s_item,
-                                               const int* frame_video = nullptr) {
+// The tracking kernels' view of the videos: which loss sum / valid count pair a segment's or a frame's terms
+// go to, and how d total / d tracking loss comes (Scale, as for the video layouts).
+struct TrackOneVideo {  // one video, or the standalone op: the one pair at sums[0], sums[1]
+  static constexpr bool kPerFrameK = true;  // per-frame intrinsics as well as one shared focal length
+  using Scale = Uniform::Scale;
+  template <class T> __device__ __forceinline__ T* sums_of(T* sums, int) const { return sums; }
+};
+struct TrackVideos {  // videos packed along the frame axis: frame f's video b has the pair sums[2 b], sums[2 b + 1]
+  static constexpr bool kPerFrameK = false;  // one focal length per video
+  using Scale = Videos::Scale;
+  const int* frame_video;
+  template <class T>
+  __device__ __forceinline__ T* sums_of(T* sums, int f) const { return sums + 2 * __ldg(frame_video + f); }
+};
+
+template <bool SHARED_K, class TL>
+__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS)
+k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,
+            const int* __restrict__ seg, const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
+            int mapping, float delta, double* __restrict__ sums, unsigned char* __restrict__ flag,
+            float* __restrict__ dq_out, double* __restrict__ trackacc, int* __restrict__ next_item, int num_items,
+            int max_rows, int list_cap, int H, int W, TrackShard sh, TL tl) {
+  extern __shared__ float4 sm4[];
+  __shared__ double red[kTrackAcc * (kTrackThreads / 32)];
+  __shared__ int s_wbase[kTrackThreads / 32];
+  __shared__ int s_item[2];
   float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
   constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
@@ -2109,8 +2066,7 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
       }
       __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
-    block_accumulate<2, kTrackThreads>(
-        lc, RAGGED ? sums + 2 * __ldg(frame_video + si.start_frame) : sums, red);
+    block_accumulate<2, kTrackThreads>(lc, tl.sums_of(sums, si.start_frame), red);
     block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
     // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
     // with a barrier, so every slice is complete)
@@ -2124,66 +2080,36 @@ __device__ __forceinline__ void track_src_body(const float* __restrict__ depth, 
   }
 }
 
-#define FM_TRACK_SRC_PARAMS                                                                                  \
-  const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,            \
-      const int* __restrict__ seg, const float* __restrict__ txy, const unsigned char* __restrict__ tvis, \
-      int mapping, float delta, double* __restrict__ sums, unsigned char* __restrict__ flag,              \
-      float* __restrict__ dq_out, double* __restrict__ trackacc, int* __restrict__ next_item, int num_items, \
-      int max_rows, int list_cap, int H, int W, TrackShard sh
-#define FM_TRACK_SRC_ARGS \
-  depth, k4, ext, seg, txy, tvis, mapping, delta, sums, flag, dq_out, trackacc, next_item, num_items, max_rows, list_cap, H, W, sh
-// shared memory is declared by the kernels (a device function's would move the dynamic part)
-#define FM_TRACK_SRC_SHARED                 \
-  extern __shared__ float4 sm4[];          \
-  __shared__ double red[kTrackAcc * (kTrackThreads / 32)]; \
-  __shared__ int s_wbase[kTrackThreads / 32]; \
-  __shared__ int s_item[2];
-template <bool SHARED_K>
-__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src(FM_TRACK_SRC_PARAMS) {
-  FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, false>(FM_TRACK_SRC_ARGS, sm4, red, s_wbase, s_item);
-}
-template <bool SHARED_K>
-__global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS) k_track_src_ragged(FM_TRACK_SRC_PARAMS, const int* frame_video) {
-  FM_TRACK_SRC_SHARED
-  track_src_body<SHARED_K, true>(FM_TRACK_SRC_ARGS, sm4, red, s_wbase, s_item, frame_video);
-}
-#undef FM_TRACK_SRC_SHARED
-#undef FM_TRACK_SRC_PARAMS
-#undef FM_TRACK_SRC_ARGS
-
 __device__ __forceinline__ double track_scale(const double* sums, float loss_weight, const float* go) {
   double cnt = sums[1];
   if (cnt == 0.0) cnt = 1.0;  // loss_tracking.py:61 "valid_sum or 1"
   return (double)loss_weight * (go ? (double)*go : 1.0) / cnt;
 }
-
-__global__ void k_track_loss(const double* __restrict__ sums, float loss_weight, float* __restrict__ loss) {
-  *loss = (float)(track_scale(sums, loss_weight, nullptr) * sums[0]);
+__device__ __forceinline__ double track_scale(const double* sums, float loss_weight, NoScale) {
+  return track_scale(sums, loss_weight, nullptr);
 }
 
-// The packed fused step's tracking losses: thread b reads video b's loss sum / valid count.
+// The tracking losses of B videos: thread b reads video b's loss sum / valid count.
 __global__ void k_track_video_loss(const double* __restrict__ sums, float loss_weight, float* __restrict__ loss, int B) {
   const int b = threadIdx.x;
   if (b < B) loss[b] = (float)(track_scale(sums + 2 * b, loss_weight, nullptr) * sums[2 * b]);
 }
 
-// scale * (stored camera-space adjoint) -> the four depth taps of every source sample.  RAGGED: the scale
-// of the segment's video (frame_video[start frame]), see track_src_body.
-template <bool RAGGED>
-__device__ __forceinline__ void track_apply_body(const float* __restrict__ k4, const int* __restrict__ seg,
-                                                 const float* __restrict__ txy, const unsigned char* __restrict__ flag,
-                                                 const float* __restrict__ dq, const double* __restrict__ sums,
-                                                 float loss_weight, const float* __restrict__ go,
-                                                 float* __restrict__ g_depth, int H, int W, TrackShard sh,
-                                                 const int* frame_video = nullptr) {
+// scale * (stored camera-space adjoint) -> the four depth taps of every source sample, scaled by the sums
+// of the segment's video.
+template <class TL>
+__global__ void __launch_bounds__(kThreads)
+k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
+              const unsigned char* __restrict__ flag, const float* __restrict__ dq, const double* __restrict__ sums,
+              float loss_weight, typename TL::Scale go, float* __restrict__ g_depth, int H, int W, TrackShard sh,
+              TL tl) {
   const SegInfo si = load_seg(seg, blockIdx.z);
   const int row = blockIdx.y;
   const int p = blockIdx.x * kThreads + threadIdx.x;
   if (row >= si.rows || p >= si.n || !sh.owns(si.start_frame + row)) return;
   const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p;
   if (!flag[sidx]) return;
-  const float scale = (float)track_scale(RAGGED ? sums + 2 * __ldg(frame_video + si.start_frame) : sums, loss_weight, go);
+  const float scale = (float)track_scale(tl.sums_of(sums, si.start_frame), loss_weight, go);
   const int frame = si.start_frame + row;
   const GridDims grid = make_grid(H, W);
   const Cam ks = make_cam(load_k4(k4, frame));
@@ -2199,31 +2125,14 @@ __device__ __forceinline__ void track_apply_body(const float* __restrict__ k4, c
   red_add(gd + t.y1 * W + t.x1, t.w11 * (dq0 * rx1 + dq1 * ry1 + dq2));
 }
 
-__global__ void __launch_bounds__(kThreads)
-k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
-              const unsigned char* __restrict__ flag, const float* __restrict__ dq,
-              const double* __restrict__ sums, float loss_weight, const float* __restrict__ go,
-              float* __restrict__ g_depth, int H, int W, TrackShard sh) {
-  track_apply_body<false>(k4, seg, txy, flag, dq, sums, loss_weight, go, g_depth, H, W, sh);
-}
-
-__global__ void __launch_bounds__(kThreads)
-k_track_apply_ragged(const float* __restrict__ k4, const int* __restrict__ seg, const float* __restrict__ txy,
-                     const unsigned char* __restrict__ flag, const float* __restrict__ dq,
-                     const double* __restrict__ sums, float loss_weight, float* __restrict__ g_depth, int H, int W,
-                     TrackShard sh, const int* __restrict__ frame_video) {
-  track_apply_body<true>(k4, seg, txy, flag, dq, sums, loss_weight, nullptr, g_depth, H, W, sh, frame_video);
-}
-
-// RAGGED: frame f scaled by the sums of its video frame_video[f].
-template <bool RAGGED>
-__device__ __forceinline__ void track_finalize_body(const double* __restrict__ trackacc, const double* __restrict__ sums,
-                                                    float loss_weight, const float* __restrict__ go,
-                                                    const float* __restrict__ ext, float* __restrict__ g_ext,
-                                                    float* __restrict__ g_k4, int F, const int* frame_video = nullptr) {
+// Frame f scaled by the sums of its video.
+template <class TL>
+__global__ void k_track_finalize(const double* __restrict__ trackacc, const double* __restrict__ sums,
+                                 float loss_weight, typename TL::Scale go, const float* __restrict__ ext,
+                                 float* __restrict__ g_ext, float* __restrict__ g_k4, int F, TL tl) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
-  const double sc = track_scale(RAGGED ? sums + 2 * __ldg(frame_video + f) : sums, loss_weight, go);
+  const double sc = track_scale(tl.sums_of(sums, f), loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
   for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
   const float* P = ext + (size_t)f * 16;
@@ -2237,19 +2146,6 @@ __device__ __forceinline__ void track_finalize_body(const double* __restrict__ t
   }
   o[3] = (float)(sc * a[7]); o[7] = (float)(sc * a[8]); o[11] = (float)(sc * a[9]);
   o[12] = o[13] = o[14] = o[15] = 0.f;
-}
-
-__global__ void k_track_finalize(const double* __restrict__ trackacc, const double* __restrict__ sums,
-                                 float loss_weight, const float* __restrict__ go,
-                                 const float* __restrict__ ext, float* __restrict__ g_ext,
-                                 float* __restrict__ g_k4, int F) {
-  track_finalize_body<false>(trackacc, sums, loss_weight, go, ext, g_ext, g_k4, F);
-}
-
-__global__ void k_track_finalize_ragged(const double* __restrict__ trackacc, const double* __restrict__ sums,
-                                        float loss_weight, const float* __restrict__ ext, float* __restrict__ g_ext,
-                                        float* __restrict__ g_k4, int T, const int* __restrict__ frame_video) {
-  track_finalize_body<true>(trackacc, sums, loss_weight, nullptr, ext, g_ext, g_k4, T, frame_video);
 }
 
 // ================================================================== focal-length sweep
@@ -2750,37 +2646,34 @@ k_metrics_ragged(const float* __restrict__ gt, const float* __restrict__ pred, M
 }
 
 // ================================================================== fused overfit step helpers
-// focal_lengths_to_intrinsics (intrinsics/common.py:6-20) for a shared focal length, as k4 rows.
-__global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restrict__ k4, int BF, int H, int W) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= BF) return;
-  const float scaled = *focal * sqrtf((float)H * (float)W);  // float32 like the reference
-  k4[t * 4 + 0] = scaled / (float)W;
-  k4[t * 4 + 1] = scaled / (float)H;
-  k4[t * 4 + 2] = 0.5f;
-  k4[t * 4 + 3] = 0.5f;
-}
-
-// k_k4_from_focal for packed videos with one focal length each: frame t of the (T, 4) rows reads the focal
-// length of its video frame_video[t].
-__global__ void k_k4_from_focals_ragged(const float* __restrict__ focal, float* __restrict__ k4, int T, int H, int W,
-                                        Videos v) {
+// focal_lengths_to_intrinsics (intrinsics/common.py:6-20) for one focal length per video, as k4 rows: frame t
+// of the (T, 4) rows reads the focal length of its video.
+template <class Lay>
+__global__ void k_k4_from_focal(const float* __restrict__ focal, float* __restrict__ k4, int T, int H, int W,
+                                Lay lay) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
-  const float scaled = focal[v.of_frame(t)] * sqrtf((float)H * (float)W);
+  const float scaled = focal[lay.of_frame(t)] * sqrtf((float)H * (float)W);  // float32 like the reference
   k4[t * 4 + 0] = scaled / (float)W;
   k4[t * 4 + 1] = scaled / (float)H;
   k4[t * 4 + 2] = 0.5f;
   k4[t * 4 + 3] = 0.5f;
 }
 
-// d loss / d focal from the per-frame k4 gradients (flow-loss part + Procrustes part).
-__device__ __forceinline__ void focal_grad_block(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                                                 const float* __restrict__ extra_g_k4, float* __restrict__ g_focal,
-                                                 int B, int F, int H, int W, const float* __restrict__ flow_scale) {
+// d loss / d focal from the per-frame k4 gradients (flow-loss part + Procrustes part): block b writes
+// g_focal[b] from video b's frames.
+template <class Lay>
+__global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
+                             const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int H, int W,
+                             Lay lay, typename Lay::Scale flow_scale) {
+  const double fs = scale_of(flow_scale);  // d total / d flow loss (the Procrustes part in k4acc carries it already)
+  const size_t f0 = lay.first(blockIdx.x);
+  const int F = lay.frames(blockIdx.x);
+  k4acc += f0 * 4;
+  flowacc += f0 * kFlowAcc;
+  if (extra_g_k4) extra_g_k4 += f0 * 4;
   double sx = 0.0, sy = 0.0;
-  const double fs = flow_scale ? (double)*flow_scale : 1.0;  // d total / d flow loss (the Procrustes part in k4acc carries it already)
-  for (int t = threadIdx.x; t < B * F; t += blockDim.x) {
+  for (int t = threadIdx.x; t < F; t += blockDim.x) {
     double g[4];
     flow_k4_grad(flowacc, t, F, g);
     sx += fs * g[0] + k4acc[(size_t)t * 4 + 0] + (extra_g_k4 ? (double)extra_g_k4[t * 4 + 0] : 0.0);
@@ -2794,24 +2687,8 @@ __device__ __forceinline__ void focal_grad_block(const double* __restrict__ k4ac
     double ax = 0.0, ay = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { ax += sm[0][w]; ay += sm[1][w]; }
     const double sc = sqrt((double)H * (double)W);
-    *g_focal = (float)(ax * sc / W + ay * sc / H);
+    g_focal[blockIdx.x] = (float)(ax * sc / W + ay * sc / H);
   }
-}
-
-__global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                             const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int B,
-                             int F, int H, int W, const float* __restrict__ flow_scale = nullptr) {
-  focal_grad_block(k4acc, flowacc, extra_g_k4, g_focal, B, F, H, W, flow_scale);
-}
-
-// One focal length per video (the packed fused step): block b writes g_focal[b] from video b's frames,
-// summed in the order k_focal_grad uses for one video.
-__global__ void k_focal_grad_ragged(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                                    const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int H, int W,
-                                    Videos v) {
-  const size_t f0 = v.first(blockIdx.x);
-  focal_grad_block(k4acc + f0 * 4, flowacc + f0 * kFlowAcc, extra_g_k4 ? extra_g_k4 + f0 * 4 : nullptr,
-                   g_focal + blockIdx.x, 1, v.frames(blockIdx.x), H, W, nullptr);
 }
 
 // ---------------------------------------------------------------- launch geometry
@@ -2883,63 +2760,47 @@ bool bad_dims(int B, int F, int H, int W) { return B < 1 || F < 2 || H < 1 || W 
 }  // namespace
 
 namespace {
-// intrinsics_mode: 0 = per-frame k4 with full gradients, 1 = one shared focal length (gradient
-// booked as d/dfx of each frame), 2 = constant intrinsics (no gradient).
+// k_flow_lean (one video, or a (B, F) batch with one pooled normaliser) and k_flow_lean_ragged (one normaliser
+// per video) are separate kernels, so that each keeps its code; each layout has its launch.
+template <int VEC, bool FOCAL, class... A>
+void launch_flow_lean(const Uniform& u, int T, int H, int W, int grid, cudaStream_t s, A... a) {
+  k_flow_lean<VEC, FOCAL, 2><<<grid, kThreads, 0, s>>>(a..., u.F, H, W, T);
+}
+template <int VEC, bool FOCAL, class... A>
+void launch_flow_lean(const Videos& v, int T, int H, int W, int grid, cudaStream_t s, A... a) {
+  k_flow_lean_ragged<VEC, FOCAL, 2><<<grid, kThreads, 0, s>>>(a..., H, W, T, v);
+}
+
+// The lean flow loss (focal: one shared focal length per video, else constant intrinsics) of the T frames
+// laid out as `lay`, into the standard per-frame accumulators.
+template <class Lay>
 int launch_flow(const float* depth, const float* k4, const float* rt, const float* ff, const float* fb,
                 const float* mf, const float* mb, const double* mask_sum, int mapping, float delta,
-                float loss_weight, int intrinsics_mode, float* g_depth, double* flowacc, int B, int F,
-                int H, int W, cudaStream_t s) {
-  const int BF = B * F;
+                float loss_weight, bool focal, float* g_depth, double* flowacc, int T, const Lay& lay, int H, int W,
+                cudaStream_t s) {
   const int vec = (W % 4 == 0) ? 4 : 1;
-  dim3 grid(blocks_for(H * W, vec), BF);
-  if (intrinsics_mode == 0) {
-    if (vec == 4) k_flow<4><<<grid, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, nullptr, mapping, delta, loss_weight, g_depth, flowacc, F, H, W);
-    else k_flow<1><<<grid, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, nullptr, mapping, delta, loss_weight, g_depth, flowacc, F, H, W);
-    FM_CHECK_LAUNCH("k_flow");
-    return 0;
-  }
-  const bool focal = intrinsics_mode == 1;
-  const int pg = persistent_grid(2, (long long)BF * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
+  const int pg = persistent_grid(2, (long long)T * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
+#define FM_FLOW_ARGS depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc
   if (vec == 4) {
-    if (focal) k_flow_lean<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-    else k_flow_lean<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+    if (focal) launch_flow_lean<4, true>(lay, T, H, W, pg, s, FM_FLOW_ARGS);
+    else launch_flow_lean<4, false>(lay, T, H, W, pg, s, FM_FLOW_ARGS);
   } else {
-    if (focal) k_flow_lean<1, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
-    else k_flow_lean<1, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, F, H, W, BF);
+    if (focal) launch_flow_lean<1, true>(lay, T, H, W, pg, s, FM_FLOW_ARGS);
+    else launch_flow_lean<1, false>(lay, T, H, W, pg, s, FM_FLOW_ARGS);
   }
+#undef FM_FLOW_ARGS
   FM_CHECK_LAUNCH("k_flow_lean");
-  k_flow_lean_convert<<<(BF + 63) / 64, 64, 0, s>>>(flowacc, rt, k4, focal ? 1 : 0, B, F, H, W);
+  k_flow_lean_convert<<<(T + 63) / 64, 64, 0, s>>>(flowacc, rt, k4, focal ? 1 : 0, T, H, W, lay);
   FM_CHECK_LAUNCH("k_flow_lean_convert");
   return 0;
 }
 
-// The host's view of an fm_video_layout: the device tables and the counts.
-struct Ragged {
-  Videos v;
-  int B, T;  // videos, frames in all (T - B pairs)
-};
-
-// launch_flow with per-video normalisers for videos of different lengths (focal: one shared focal length
-// per video, else constant intrinsics).
-int launch_flow_ragged(const float* depth, const float* k4, const float* rt, const float* ff, const float* fb,
-                       const float* mf, const float* mb, const double* mask_sum, int mapping, float delta,
-                       float loss_weight, bool focal, float* g_depth, double* flowacc, const Ragged& r, int H, int W,
-                       cudaStream_t s) {
-  const int T = r.T;
-  const int vec = (W % 4 == 0) ? 4 : 1;
-  const int pg = persistent_grid(2, (long long)T * ((H * W + kThreads * vec - 1) / (kThreads * vec)));
-  if (vec == 4) {
-    if (focal) k_flow_lean_ragged<4, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
-    else k_flow_lean_ragged<4, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
-  } else {
-    if (focal) k_flow_lean_ragged<1, true, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
-    else k_flow_lean_ragged<1, false, 2><<<pg, kThreads, 0, s>>>(depth, k4, rt, ff, fb, mf, mb, mask_sum, mapping, delta, loss_weight, g_depth, flowacc, H, W, T, r.v);
-  }
-  FM_CHECK_LAUNCH("k_flow_lean_ragged");
-  k_flow_lean_convert_ragged<<<(T + 63) / 64, 64, 0, s>>>(flowacc, rt, k4, focal ? 1 : 0, T, H, W, r.v);
-  FM_CHECK_LAUNCH("k_flow_lean_convert_ragged");
-  return 0;
-}
+// The frame layout of a pair layout and back: one video (or a uniform batch) divides by F, packed videos
+// read their tables.
+Uniform frames_of(const PairLayout& l) { return Uniform{l.F}; }
+const Videos& frames_of(const RaggedPairs& l) { return l.v; }
+PairLayout pairs_of(const Uniform& u, int H, int W) { return dense_layout(u.F, H, W); }
+RaggedPairs pairs_of(const Videos& v, int, int) { return RaggedPairs{v}; }
 }  // namespace
 
 // ---------------------------------------------------------------- tiled path: host side
@@ -3047,33 +2908,6 @@ int launch_backward_tiled(const float* depth, const float* k4, const float* bflo
   return 0;
 }
 
-// k_adjoint and k_k4_finalize find a pair's or a frame's video by dividing by F (one video, or a uniform
-// batch) or in the packed layout's tables; their parameter lists differ, so each layout has its launch.
-int launch_adjoint(const PairLayout& lay, const Workspace& w, const float* g_rt, int include_flow,
-                   const float* flow_scale, int BP, cudaStream_t s) {
-  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow, flow_scale, w.adj, BP, lay.F);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
-  return 0;
-}
-int launch_adjoint(const RaggedPairs& lay, const Workspace& w, const float* g_rt, int include_flow,
-                   const float* flow_scale, int BP, cudaStream_t s) {
-  k_adjoint_ragged<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow, flow_scale, w.adj, BP, lay.v);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint_ragged");
-  return 0;
-}
-int launch_k4_finalize(const PairLayout& lay, const Workspace& w, int include_flow, const float* flow_scale,
-                       float* g_k4, int T, cudaStream_t s) {
-  k_k4_finalize<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow, flow_scale, g_k4, T / lay.F, lay.F);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
-  return 0;
-}
-int launch_k4_finalize(const RaggedPairs& lay, const Workspace& w, int include_flow, const float* flow_scale,
-                       float* g_k4, int T, cudaStream_t s) {
-  k_k4_finalize_ragged<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow, flow_scale, g_k4, T, lay.v);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize_ragged");
-  return 0;
-}
-
 // The Procrustes forward of B videos with T frames (T - B pairs) in all, laid out as `lay`: dense_layout
 // for one video or a uniform batch, RaggedPairs for packed videos of different lengths.  Pair shift,
 // moments, then (solve) the poses.  moments_k4 != NULL: fm_procrustes_moments(_videos) already accumulated
@@ -3139,8 +2973,9 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
     k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)T * H * W);
     FM_CHECK_LAUNCH("fm_procrustes_bwd: k_scale_inplace");
   }
-  int rc = launch_adjoint(lay, w, g_rt, include_flow_loss, flow_scale, BP, s);
-  if (rc) return rc;
+  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP,
+                                          frames_of(lay));
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
   if (indices) {
     dim3 grid(blocks_for_points(num_indices), BP);
     k_distribute<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
@@ -3155,7 +2990,10 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
     k_distribute_dense<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
   }
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
-  return launch_k4_finalize(lay, w, include_flow_loss, flow_scale, g_k4, T, s);
+  k_k4_finalize<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, T,
+                                                frames_of(lay));
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
+  return 0;
 }
 
 // The splat plan's Procrustes forward and backward (fm_tiled.cuh): one video, all pixels, W % 4 == 0.
@@ -3199,14 +3037,17 @@ int procrustes_bwd_planned(const float* depth, const float* k4, const float* bac
   if (adam) af = *adam; else memset(&af, 0, sizeof(af));
   // one focal length shared by all frames (or constant intrinsics): the Procrustes part of the
   // intrinsics gradient comes from the moment sums, the pixel kernel carries no K accumulators
-  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP, F,
-                                          w.moments, k4, w.k4acc);
+  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP,
+                                          Uniform{F}, w.moments, k4, w.k4acc);
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
   const int rc = launch_backward_tiled(depth, k4, backward_flow, const_cast<float*>(weights), wsens,
                                        tiled::plan_carve(plan, F, H, W), plan_ovf_max, w.adj, g_depth, g_weights, af,
                                        F, H, W, s);
   if (rc) return rc;
-  return launch_k4_finalize(dense_layout(F, H, W), w, include_flow_loss, flow_scale, g_k4, F, s);
+  k_k4_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, F,
+                                                Uniform{F});
+  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
+  return 0;
 }
 
 PairLayout sweep_layout(int F, int H, int W, int cand) {
@@ -3283,7 +3124,7 @@ int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensit
   k_sweep_out<<<(items * 12 + 127) / 128, 128, 0, s>>>(w.flowacc, g_rt, items, 1, 12);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_out");
   // per-candidate adjoint constants, collapsed into one per batch element, then ONE distribution pass
-  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, 2);
+  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_adjoint");
   k_sweep_aggregate<<<B, 32, 0, s>>>(w.adj, cand_k4, w.adj + items, B, num_candidates);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_aggregate");
@@ -3479,14 +3320,29 @@ int fm_flow_loss_fwd_bwd(const float* depth, const float* k4, const float* rt,
   const int BP = B * (F - 1), BF = B * F;
   cudaError_t e = cudaMemsetAsync(w.flowacc, 0, (size_t)BF * kFlowAcc * sizeof(double), s);
   if (e != cudaSuccess) return fail("fm_flow_loss_fwd_bwd: memset", e);
-  int rc = launch_flow(depth, k4, rt, forward_flow, backward_flow, forward_mask, backward_mask, mask_sum,
-                       mapping, delta, loss_weight, intrinsics_mode, g_depth, w.flowacc, B, F, H, W, s);
-  if (rc) return rc;
+  if (intrinsics_mode == 0) {  // per-frame k4 with full gradients
+    const int vec = (W % 4 == 0) ? 4 : 1;
+    dim3 grid(blocks_for(H * W, vec), BF);
+    if (vec == 4) k_flow<4><<<grid, kThreads, 0, s>>>(depth, k4, rt, forward_flow, backward_flow, forward_mask, backward_mask, mask_sum, nullptr, mapping, delta, loss_weight, g_depth, w.flowacc, F, H, W);
+    else k_flow<1><<<grid, kThreads, 0, s>>>(depth, k4, rt, forward_flow, backward_flow, forward_mask, backward_mask, mask_sum, nullptr, mapping, delta, loss_weight, g_depth, w.flowacc, F, H, W);
+    FM_CHECK_LAUNCH("k_flow");
+  } else {
+    int rc = launch_flow(depth, k4, rt, forward_flow, backward_flow, forward_mask, backward_mask, mask_sum, mapping,
+                         delta, loss_weight, intrinsics_mode == 1, g_depth, w.flowacc, BF, Uniform{F}, H, W, s);
+    if (rc) return rc;
+  }
   const int n = BF > BP ? BF : BP;
   k_flow_finalize<<<(n + 127) / 128, 128, 0, s>>>(w.flowacc, rt, loss, g_rt, g_k4, B, F);
   FM_CHECK_LAUNCH("fm_flow_loss_fwd_bwd: k_flow_finalize");
   return 0;
 }
+
+extern "C++" {
+// The host's view of an fm_video_layout: the device tables and the counts.
+struct Ragged {
+  Videos v;
+  int B, T;  // videos, frames in all (T - B pairs)
+};
 
 // fm_video_layout -> Ragged; nonzero when the layout is unusable (B >= 1 videos of >= 2 frames each, the
 // per-video tables are the caller's: only their presence and the counts are checked here).
@@ -3500,24 +3356,26 @@ static int ragged_of(const fm_video_layout* l, Ragged* r) {
   return 0;
 }
 
-static int pose_chain_ragged(const float* rt, float* extrinsics, const Ragged& r, void* stream) {
-  k_pose_chain_ragged<<<r.B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, r.v);
-  FM_CHECK_LAUNCH("fm_pose_chain_videos");
+// The extrinsics of B videos laid out as `lay`, chained from each video's frame 0, and their adjoint.
+template <class Lay>
+static int pose_chain(const float* rt, float* extrinsics, int B, const Lay& lay, void* stream) {
+  k_pose_chain<<<B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, lay);
+  FM_CHECK_LAUNCH("fm_pose_chain");
+  return 0;
+}
+template <class Lay>
+static int pose_chain_bwd(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt, int B,
+                          const Lay& lay, void* stream) {
+  k_pose_chain_bwd<<<B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, g_extrinsics, g_rt, lay);
+  FM_CHECK_LAUNCH("fm_pose_chain_bwd");
   return 0;
 }
 
-static int pose_chain_bwd_ragged(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
-                                 const Ragged& r, void* stream) {
-  k_pose_chain_bwd_ragged<<<r.B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, g_extrinsics, g_rt, r.v);
-  FM_CHECK_LAUNCH("fm_pose_chain_bwd_videos");
-  return 0;
-}
+}  // extern "C++"
 
 int fm_pose_chain(const float* rt, float* extrinsics, int B, int F, void* stream) {
   if (!rt || !extrinsics || B < 1 || F < 2) return fail_msg("fm_pose_chain: bad arguments");
-  k_pose_chain<<<B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, B, F);
-  FM_CHECK_LAUNCH("fm_pose_chain");
-  return 0;
+  return pose_chain(rt, extrinsics, B, Uniform{F}, stream);
 }
 
 int fm_trajectory_ate(const float* gt, const float* pred, int T, int F, float* ate, float* aligned_gt,
@@ -3535,9 +3393,7 @@ int fm_trajectory_ate(const float* gt, const float* pred, int T, int F, float* a
 int fm_pose_chain_bwd(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
                       int B, int F, void* stream) {
   if (!rt || !extrinsics || !g_extrinsics || !g_rt || B < 1 || F < 2) return fail_msg("fm_pose_chain_bwd: bad arguments");
-  k_pose_chain_bwd<<<B, kChainThreads, 0, (cudaStream_t)stream>>>(rt, extrinsics, g_extrinsics, g_rt, B, F);
-  FM_CHECK_LAUNCH("fm_pose_chain_bwd");
-  return 0;
+  return pose_chain_bwd(rt, extrinsics, g_extrinsics, g_rt, B, Uniform{F}, stream);
 }
 
 int fm_step_clock_tick(void* clock, double lr, double beta1, double beta2, unsigned long long base_seed,
@@ -3617,15 +3473,17 @@ size_t fm_track_reduce_bytes(int F) {
   return align_up(4 * sizeof(double), 256) + align_up((size_t)F * kTrackAcc * sizeof(double), 256);
 }
 
-// vsums != NULL (the packed fused step): the frames are B videos packed along the frame axis, the video of
-// a segment's start frame is frame_video[that frame], and each video's loss sum and valid count go to
-// vsums[2 b], vsums[2 b + 1] (zeroed here) instead of the head of ws; `loss` then receives B values.
+extern "C++" {
+// The frames are B videos laid out as `tl`; each video's loss sum and valid count go to sums[2 b],
+// sums[2 b + 1] (zeroed here): the head of ws for one video, the caller's B pairs for packed videos.  `loss`
+// receives B values.
+template <class TL>
 static int track_fwd_impl(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                           int num_segments, int max_rows, int max_points, const float* track_xy,
                           const unsigned char* track_vis, long long total_samples, int mapping, float delta,
                           float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
-                          int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream,
-                          double* vsums = nullptr, int B = 1, const int* frame_video = nullptr) {
+                          int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream, double* sums,
+                          int B, const TL& tl) {
   if (!depth || !k4 || !extrinsics || !segments || !track_xy || !track_vis || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_fwd: bad arguments");
@@ -3637,7 +3495,7 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
   // sums, work counter, accumulators
   cudaError_t e = cudaMemsetAsync(w.sums, 0, (char*)w.dq - (char*)w.sums, s);
   if (e != cudaSuccess) return fail("fm_track_loss_fwd: memset", e);
-  if (vsums && (e = cudaMemsetAsync(vsums, 0, (size_t)B * 2 * sizeof(double), s)) != cudaSuccess)
+  if (sums != w.sums && (e = cudaMemsetAsync(sums, 0, (size_t)B * 2 * sizeof(double), s)) != cudaSuccess)
     return fail("fm_track_loss_fwd: memset", e);
   const int list_cap = max_points < kTrackListCap ? max_points : kTrackListCap;
   const size_t smem = track_smem_bytes(max_rows, list_cap);
@@ -3649,41 +3507,28 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
   if (per_sm > FM_TRACK_BPS) per_sm = FM_TRACK_BPS;
   if (per_sm < 1) per_sm = 1;
   const int grid = persistent_grid(per_sm, items);
+  auto src = k_track_src<true, TL>;
+  if constexpr (TL::kPerFrameK) {
+    if (!shared_intrinsics) src = k_track_src<false, TL>;
+  } else if (!shared_intrinsics) {
+    return fail_msg("fm_track_loss_fwd: packed videos have one focal length each");
+  }
   if (smem > 48 * 1024) {
-    cudaError_t ea = shared_intrinsics
-        ? cudaFuncSetAttribute(k_track_src<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-        : cudaFuncSetAttribute(k_track_src<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t ea = cudaFuncSetAttribute(src, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (ea != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ea);
   }
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
-  if (vsums) {  // one focal length per video: shared intrinsics
-    static const cudaError_t ev = cudaFuncSetAttribute(k_track_src_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (ev != cudaSuccess) return fail("fm_track_loss_fwd: shared memory", ev);
-    k_track_src_ragged<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis,
-                                                               mapping, delta, vsums, w.flag, w.dq, w.acc, w.next_item,
-                                                               (int)items, max_rows, list_cap, H, W, sh, frame_video);
-    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src_ragged");
-    if (loss) {
-      k_track_video_loss<<<1, 32 * ((B + 31) / 32), 0, s>>>(vsums, loss_weight, loss, B);
-      FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_video_loss");
-    }
-    return 0;
-  }
-  if (shared_intrinsics)
-    k_track_src<true><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping,
-                                                        delta, w.sums, w.flag, w.dq, w.acc, w.next_item, (int)items,
-                                                        max_rows, list_cap, H, W, sh);
-  else
-    k_track_src<false><<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping,
-                                                         delta, w.sums, w.flag, w.dq, w.acc, w.next_item, (int)items,
-                                                         max_rows, list_cap, H, W, sh);
+  src<<<grid, kTrackThreads, smem, s>>>(depth, k4, extrinsics, segments, track_xy, track_vis, mapping, delta, sums,
+                                        w.flag, w.dq, w.acc, w.next_item, (int)items, max_rows, list_cap, H, W, sh, tl);
   FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_src");
   if (loss) {
-    k_track_loss<<<1, 1, 0, s>>>(w.sums, loss_weight, loss);
-    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_loss");
+    k_track_video_loss<<<1, 32 * ((B + 31) / 32), 0, s>>>(sums, loss_weight, loss, B);
+    FM_CHECK_LAUNCH("fm_track_loss_fwd: k_track_video_loss");
   }
   return 0;
 }
+
+}  // extern "C++"
 
 int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                               int num_segments, int max_rows, int max_points, const float* track_xy,
@@ -3692,7 +3537,7 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
                               int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream) {
   return track_fwd_impl(depth, k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, track_vis,
                         total_samples, mapping, delta, loss_weight, loss, ws, F, H, W, depth_frame0, src_frame_lo,
-                        src_frame_hi, shared_intrinsics, stream);
+                        src_frame_hi, shared_intrinsics, stream, (double*)ws, 1, TrackOneVideo{});
 }
 
 int fm_track_loss_fwd(const float* depth, const float* k4, const float* extrinsics, const int* segments,
@@ -3707,19 +3552,22 @@ int fm_track_loss_fwd(const float* depth, const float* k4, const float* extrinsi
 
 int fm_track_loss_value(const void* ws, float loss_weight, float* loss, void* stream) {
   if (!ws || !loss) return fail_msg("fm_track_loss_value: bad arguments");
-  k_track_loss<<<1, 1, 0, (cudaStream_t)stream>>>((const double*)ws, loss_weight, loss);
+  k_track_video_loss<<<1, 32, 0, (cudaStream_t)stream>>>((const double*)ws, loss_weight, loss, 1);
   FM_CHECK_LAUNCH("fm_track_loss_value");
   return 0;
 }
 
+extern "C++" {
 // The depth scatter of the tracking loss (k_track_apply, REDs into g_depth) and the pose / intrinsics
-// gradients (k_track_finalize) are independent: `apply_stream` may differ from `s`.
+// gradients (k_track_finalize) are independent: `apply_stream` may differ from `s`.  `sums` and `tl` as in
+// track_fwd_impl.
+template <class TL>
 static int track_bwd_impl(const float* k4, const float* extrinsics, const int* segments, int num_segments,
                           int max_rows, int max_points, const float* track_xy, long long total_samples,
                           float loss_weight, const float* grad_out, float* g_depth, float* g_extrinsics,
                           float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
-                          int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream,
-                          const double* vsums = nullptr, const int* frame_video = nullptr) {
+                          int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream, const double* sums,
+                          const TL& tl) {
   if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !g_k4 || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_bwd: bad arguments");
@@ -3728,23 +3576,16 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
   TrackWs w = carve_track(ws, F, total_samples);
   dim3 grid((max_points + kThreads - 1) / kThreads, max_rows, num_segments);
   const TrackShard sh = {depth_frame0, src_frame_lo, src_frame_hi};
-  if (vsums) {  // per-video scales (track_fwd_impl); grad_out is 1 in the packed step
-    k_track_apply_ragged<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, vsums, loss_weight,
-                                                             g_depth, H, W, sh, frame_video);
-    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply_ragged");
-    k_track_finalize_ragged<<<(F + 63) / 64, 64, 0, s>>>(w.acc, vsums, loss_weight, extrinsics, g_extrinsics, g_k4,
-                                                         F, frame_video);
-    FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize_ragged");
-    return 0;
-  }
-  k_track_apply<<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, w.sums, loss_weight,
-                                                    grad_out, g_depth, H, W, sh);
+  k_track_apply<TL><<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, sums, loss_weight,
+                                                        grad_out, g_depth, H, W, sh, tl);
   FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply");
-  k_track_finalize<<<(F + 63) / 64, 64, 0, s>>>(w.acc, w.sums, loss_weight, grad_out, extrinsics, g_extrinsics,
-                                               g_k4, F);
+  k_track_finalize<TL><<<(F + 63) / 64, 64, 0, s>>>(w.acc, sums, loss_weight, grad_out, extrinsics, g_extrinsics,
+                                                   g_k4, F, tl);
   FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize");
   return 0;
 }
+
+}  // extern "C++"
 
 int fm_track_loss_bwd_sharded(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                               int num_segments, int max_rows, int max_points, const float* track_xy,
@@ -3755,7 +3596,8 @@ int fm_track_loss_bwd_sharded(const float* depth, const float* k4, const float* 
   (void)depth; (void)track_vis; (void)mapping; (void)delta;
   return track_bwd_impl(k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, total_samples,
                         loss_weight, grad_out, g_depth, g_extrinsics, g_k4, ws, F, H, W, depth_frame0,
-                        src_frame_lo, src_frame_hi, (cudaStream_t)stream, (cudaStream_t)stream);
+                        src_frame_lo, src_frame_hi, (cudaStream_t)stream, (cudaStream_t)stream, (const double*)ws,
+                        TrackOneVideo{});
 }
 
 int fm_track_loss_bwd(const float* depth, const float* k4, const float* extrinsics, const int* segments,
@@ -3797,7 +3639,7 @@ int fm_align_rigid_bwd(const float* p, const float* q, const float* weights, con
   cudaStream_t s = (cudaStream_t)stream;
   Workspace w = carve(ws, items, 2);
   // items "pairs" of a 2-frame layout: k_adjoint indexes state / adj by pair
-  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, 2);
+  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
   FM_CHECK_LAUNCH("fm_align_rigid_bwd: k_adjoint");
   dim3 grid(blocks_for(n, 1), items);
   k_points_distribute<<<grid, kThreads, 0, s>>>(p, q, weights, w.adj, g_p, g_q, g_w, n);
@@ -3906,59 +3748,83 @@ static SideLane* side_lane(int which = 0) {
   return l.state == 1 ? &l : nullptr;
 }
 
-// rag == NULL: one video of a->F frames.  rag != NULL (fm_overfit_step_videos): B independent videos packed
-// along the frame axis; a->B and a->F are then ignored, B and T come from the layout, and every per-video
-// scalar is an array of B values.
-static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, void* stream) {
+extern "C++" {
+// What only one video supports: the packed step refuses it (nullptr: nothing to refuse).
+const char* step_refusal(const fm_overfit_step_args* a, const Uniform&) {
+  return a->B > 1 ? "fm_overfit_step: one video per call (B = 0 or 1); several videos go to fm_overfit_step_videos"
+                  : nullptr;
+}
+const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
+  if (a->phase != FM_STEP_ALL || a->splat_plan) return "fm_overfit_step_videos: serves whole steps without a splat plan";
+  if (a->defer_adam == 1 && a->step > 0 && a->weight_logits)
+    return "fm_overfit_step_videos: does not fuse the logit update of a deferred step (pass step = 0)";
+  if (a->metrics_log && !a->gt_fxfy) return "fm_overfit_step_videos: metrics need gt_fxfy";
+  return nullptr;
+}
+
+// The tracking kernels' layout, and where the step keeps the tracking loss sums: the head of the tracking
+// workspace for one video (fm_track_loss_value reads them there), one pair per video in the step's for packed
+// videos.
+TrackOneVideo track_layout(const Uniform&) { return TrackOneVideo{}; }
+TrackVideos track_layout(const Videos& v) { return TrackVideos{v.frame_video}; }
+double* step_track_sums(const Uniform&, const Workspace&, void* track_ws) { return (double*)track_ws; }
+double* step_track_sums(const Videos&, const Workspace& w, void*) { return w.track_sums; }
+
+// The metrics row: one video reads the scalar gt_fx / gt_fy through k_trajectory_ate's row mode, packed
+// videos the (B, 2) gt_fxfy.
+int launch_metrics(const fm_overfit_step_args* a, const MetricsRow& row, int B, int T, const Uniform&,
+                   cudaStream_t ms) {
+  k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, T, nullptr, nullptr,
+                                              nullptr, nullptr, row);
+  FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
+  return 0;
+}
+int launch_metrics(const fm_overfit_step_args* a, const MetricsRow& row, int B, int, const Videos& v,
+                   cudaStream_t ms) {
+  k_metrics_ragged<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, row, a->gt_fxfy, v);
+  FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_ragged");
+  return 0;
+}
+
+// B videos with T frames in all, laid out as `lay`: one video of a->F frames (Uniform, fm_overfit_step), or
+// independent videos packed along the frame axis (Videos, fm_overfit_step_videos), where a->B and a->F are
+// ignored and every per-video scalar is an array of B values.
+template <class Lay>
+static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const Lay& lay, void* stream) {
   if (!a || !a->depth || !a->fflow || !a->bflow || !a->fmask || !a->bmask || !a->mask_sum ||
-      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 ||
-      (rag ? bad_dims(rag->B, 2, a->H, a->W) : bad_dims(1, a->F, a->H, a->W)))
+      !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 || T < 2 * B || bad_dims(B, 2, a->H, a->W))
     return fail_msg("fm_overfit_step: bad arguments");
-  if (!rag && a->B > 1)
-    return fail_msg("fm_overfit_step: one video per call (B = 0 or 1); several videos go to fm_overfit_step_videos");
-  const int B = rag ? rag->B : 1;
-  if (rag && (a->phase != FM_STEP_ALL || a->splat_plan))
-    return fail_msg("fm_overfit_step_videos: serves whole steps without a splat plan");
-  if (rag && a->defer_adam == 1 && a->step > 0 && a->weight_logits)
-    return fail_msg("fm_overfit_step_videos: does not fuse the logit update of a deferred step (pass step = 0)");
-  if (rag && a->metrics_log && !a->gt_fxfy) return fail_msg("fm_overfit_step_videos: metrics need gt_fxfy");
+  if (const char* why = step_refusal(a, lay)) return fail_msg(why);
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
   if (a->metrics_log && (a->phase != FM_STEP_ALL || !a->clock || !a->extrinsics || a->metrics_capacity < 1))
     return fail_msg("fm_overfit_step: metrics_log needs FM_STEP_ALL, a clock, extrinsics and metrics_capacity >= 1");
   cudaStream_t s = (cudaStream_t)stream;
-  const int F = rag ? 0 : a->F, H = a->H, W = a->W, BP = F - 1;
+  const int H = a->H, W = a->W;
   const size_t N = (size_t)H * W;
   // frames and pairs of all videos
-  const size_t TF = rag ? (size_t)rag->T : (size_t)F, TP = rag ? (size_t)(rag->T - B) : (size_t)BP;
-  const int* frame_video = rag ? rag->v.frame_video : nullptr;
-  Workspace w = rag ? carve_rows(a->ws, B, TF, TP) : carve(a->ws, B, F);
+  const size_t TF = (size_t)T, TP = (size_t)(T - B);
+  Workspace w = carve_rows(a->ws, B, TF, TP);
+  const auto pairs = pairs_of(lay, H, W);
   int rc;
   cudaError_t e;
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
   // the splat plan of this video's backward flows serves the dense path (all-pixel Procrustes)
-  void* plan = (!rag && a->splat_plan && !a->indices && tiled_shape_ok(F, H, W)) ? a->splat_plan : nullptr;
-  // runs a Procrustes launcher on the pairs of the packed videos or of the one video
-  auto on_pairs = [&](auto launch) { return rag ? launch(RaggedPairs{rag->v}) : launch(dense_layout(F, H, W)); };
+  void* plan = (a->splat_plan && !a->indices && tiled_shape_ok(T, H, W)) ? a->splat_plan : nullptr;
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
-    if (a->focal && rag) {
-      k_k4_from_focals_ragged<<<(rag->T + 63) / 64, 64, 0, s>>>(a->focal, k4, rag->T, H, W, rag->v);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focals_ragged");
-    } else if (a->focal) {
-      k_k4_from_focal<<<(F + 63) / 64, 64, 0, s>>>(a->focal, k4, F, H, W);
+    if (a->focal) {
+      k_k4_from_focal<<<(T + 63) / 64, 64, 0, s>>>(a->focal, k4, T, H, W, lay);
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
     if ((rc = plan ? procrustes_fwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
-                                            a->rt, a->ws, F, H, W, s)
-                   : on_pairs([&](const auto& lay) {
-                       return procrustes_fwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                             a->indices, a->num_indices, a->rt, a->ws, B, (int)TF, lay, H, W, s,
-                                             a->indices ? nullptr : a->moments_k4, /*solve=*/true);
-                     })))
+                                            a->rt, a->ws, T, H, W, s)
+                   : procrustes_fwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                                    a->num_indices, a->rt, a->ws, B, T, pairs, H, W, s,
+                                    a->indices ? nullptr : a->moments_k4, /*solve=*/true)))
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
     // two branches of the step (the tracking sweep is issue-bound, the flow kernel waits on memory:
@@ -3971,35 +3837,23 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     // LossFlow forward + direct gradients (loss_flow.py:31-70)
     e = cudaMemsetAsync(w.flowacc, 0, TF * kFlowAcc * sizeof(double), s);
     if (e != cudaSuccess) return fail("fm_overfit_step: memset", e);
-    if (rag) {
-      if ((rc = launch_flow_ragged(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum, a->mapping,
-                                   a->delta, a->flow_weight, a->focal != nullptr, a->g_depth, w.flowacc, *rag, H, W, s)))
-        return rc;
-    } else if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum,
-                          a->mapping, a->delta, a->flow_weight, a->focal ? 1 : 2, a->g_depth, w.flowacc, 1, F,
-                          H, W, s)))
+    if ((rc = launch_flow(a->depth, k4, a->rt, a->fflow, a->bflow, a->fmask, a->bmask, a->mask_sum, a->mapping,
+                          a->delta, a->flow_weight, a->focal != nullptr, a->g_depth, w.flowacc, T, lay, H, W, s)))
       return rc;
-    if (rag) {
-      k_flow_video_loss_ragged<<<B, 128, 0, s>>>(w.flowacc, a->loss, rag->v);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss_ragged");
-    } else {
-      k_flow_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.flowacc, a->rt, a->loss, nullptr, nullptr, 1, F);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_flow_finalize");
-    }
+    k_flow_video_loss<<<B, 128, 0, s>>>(w.flowacc, a->loss, lay);
+    FM_CHECK_LAUNCH("fm_overfit_step: k_flow_video_loss");
     // LossTracking (loss_tracking.py:28-61) on the chained poses: the forward sweep belongs to the
     // forward half of a split step, its scaling / scatter to the backward half
     if (a->tracks) {
       const fm_packed_tracks* t = a->tracks;
       void* ts = fwd_lane ? (void*)fwd_lane->stream : stream;
-      if ((rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ts) : fm_pose_chain(a->rt, a->extrinsics, 1, F, ts)))
-        return rc;
-      // one focal length (or constant intrinsics) for all frames: only the summed K gradient is used.
-      // Several videos: the segments of video b start at frames frame_offset[b] + s, and its sums go to
-      // w.track_sums[b]
+      if ((rc = pose_chain(a->rt, a->extrinsics, B, lay, ts))) return rc;
+      // one focal length (or constant intrinsics) for all frames of a video: only the summed K gradient is
+      // used.  Several videos: the segments of video b start at frames frame_offset[b] + s
       if ((rc = track_fwd_impl(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
                                t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
-                               a->track_weight, a->track_loss, a->track_ws, (int)TF, H, W, 0, 0, (int)TF, 1, ts,
-                               rag ? w.track_sums : nullptr, B, frame_video)))
+                               a->track_weight, a->track_loss, a->track_ws, T, H, W, 0, 0, T, 1, ts,
+                               step_track_sums(lay, w, a->track_ws), B, track_layout(lay))))
         return rc;
       if (fwd_lane) {
         if ((e = cudaEventRecord(fwd_lane->join, fwd_lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
@@ -4020,9 +3874,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
       ms = mlane->stream;
     }
     // the camera centres: the tracking loss chained the poses already, a flow-only step chains them here
-    if (!a->tracks &&
-        (rc = rag ? pose_chain_ragged(a->rt, a->extrinsics, *rag, ms) : fm_pose_chain(a->rt, a->extrinsics, 1, F, ms)))
-      return rc;
+    if (!a->tracks && (rc = pose_chain(a->rt, a->extrinsics, B, lay, ms))) return rc;
     MetricsRow row;
     row.log = a->metrics_log;
     row.capacity = a->metrics_capacity;
@@ -4032,14 +3884,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     row.k4 = k4;
     row.gt_fx = a->gt_fx;
     row.gt_fy = a->gt_fy;
-    if (rag) {
-      k_metrics_ragged<<<B, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, row, a->gt_fxfy, rag->v);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_metrics_ragged");
-    } else {
-      k_trajectory_ate<<<1, kAteThreads, 0, ms>>>(a->gt_positions, a->extrinsics + 3, 16, 4, F, nullptr, nullptr,
-                                                  nullptr, nullptr, row);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_trajectory_ate");
-    }
+    if ((rc = launch_metrics(a, row, B, T, lay, ms))) return rc;
     if (mlane && (e = cudaEventRecord(mlane->join, mlane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   }
   if (a->phase == FM_STEP_FORWARD) return 0;
@@ -4067,13 +3912,11 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
     }
     if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
                              t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
-                             a->track_ws, (int)TF, H, W, 0, 0, (int)TF, s, apply_stream,
-                             rag ? w.track_sums : nullptr, frame_video)))
+                             a->track_ws, T, H, W, 0, 0, T, s, apply_stream, step_track_sums(lay, w, a->track_ws),
+                             track_layout(lay))))
       return rc;
     if (lane && (e = cudaEventRecord(lane->join, lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
-    if ((rc = rag ? pose_chain_bwd_ragged(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, *rag, stream)
-                  : fm_pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, 1, F, stream)))
-      return rc;
+    if ((rc = pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, lay, stream))) return rc;
     g_rt = a->g_rt;
     track_g_k4 = a->track_g_k4;
   }
@@ -4085,9 +3928,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   AdamFuse af;
   memset(&af, 0, sizeof(af));
   const bool defer = a->defer_adam != 0;  // softmin stage: the sweep's backward still adds gradients
-  // several videos with defer_adam = 1 would have to defer pair 0 of EVERY video (first_pair counts pairs
-  // of the whole batch): that step leaves the logits to the caller instead
-  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0 && !(rag && a->defer_adam == 1);
+  // (several videos with defer_adam = 1 would have to defer pair 0 of EVERY video, as first_pair counts pairs
+  // of the whole batch: step_refusal leaves the logits of that step to the caller)
+  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0;
   const StepClock* clock = (const StepClock*)a->clock;
   if (fuse_w) {  // the weight gradient is final inside k_distribute: update the logits there
     af.consts = clock ? &clock->step_size : nullptr;
@@ -4101,13 +3944,10 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   // g_depth was scaled by fscale above
   if ((rc = plan ? procrustes_bwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
                                           a->splat_overflow_max, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4,
-                                          a->ws, F, H, W, s, fuse_w ? &af : nullptr)
-                 : on_pairs([&](const auto& lay) {
-                     return procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity,
-                                           a->indices, a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights,
-                                           a->g_k4, a->ws, B, (int)TF, lay, H, W, s, fuse_w ? &af : nullptr,
-                                           /*depth_prescaled=*/true);
-                   })))
+                                          a->ws, T, H, W, s, fuse_w ? &af : nullptr)
+                 : procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                                  a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4, a->ws, B, T,
+                                  pairs, H, W, s, fuse_w ? &af : nullptr, /*depth_prescaled=*/true)))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   // Adam (model_wrapper_overfit.py:104-105)
@@ -4122,13 +3962,8 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
       return rc;
   }
   if (a->focal) {  // d loss / d focal, then (update steps) its Adam
-    if (rag) {
-      k_focal_grad_ragged<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, H, W, rag->v);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad_ragged");
-    } else {
-      k_focal_grad<<<1, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, 1, F, H, W, fscale);
-      FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
-    }
+    k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, H, W, lay, fscale);
+    FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
     if (a->step > 0 && !defer) {
       const int fstep = a->focal_step > 0 ? a->focal_step : a->step;
       if ((rc = clock ? fm_adam_step_clock(a->focal, a->g_focal, a->m_focal, a->v_focal, B, clock, 1, a->beta1,
@@ -4143,12 +3978,17 @@ static int overfit_step_impl(const fm_overfit_step_args* a, const Ragged* rag, v
   return 0;
 }
 
-int fm_overfit_step(const fm_overfit_step_args* a, void* stream) { return overfit_step_impl(a, nullptr, stream); }
+}  // extern "C++"
+
+int fm_overfit_step(const fm_overfit_step_args* a, void* stream) {
+  const int F = a ? a->F : 0;
+  return overfit_step_impl(a, 1, F, Uniform{F}, stream);
+}
 
 int fm_overfit_step_videos(const fm_overfit_step_args* a, const fm_video_layout* layout, void* stream) {
   Ragged r;
   if (ragged_of(layout, &r)) return fail_msg("fm_overfit_step_videos: bad video layout");
-  return overfit_step_impl(a, &r, stream);
+  return overfit_step_impl(a, r.B, r.T, r.v, stream);
 }
 
 size_t fm_workspace_bytes_videos(int B, int T) {
@@ -4214,7 +4054,7 @@ int fm_adam_step_clock_frames_videos(float* param, const float* grad, float* exp
 int fm_pose_chain_videos(const float* rt, float* extrinsics, const fm_video_layout* layout, void* stream) {
   Ragged r;
   if (!rt || !extrinsics || ragged_of(layout, &r)) return fail_msg("fm_pose_chain_videos: bad arguments");
-  return pose_chain_ragged(rt, extrinsics, r, stream);
+  return pose_chain(rt, extrinsics, r.B, r.v, stream);
 }
 
 int fm_pose_chain_bwd_videos(const float* rt, const float* extrinsics, const float* g_extrinsics, float* g_rt,
@@ -4222,7 +4062,7 @@ int fm_pose_chain_bwd_videos(const float* rt, const float* extrinsics, const flo
   Ragged r;
   if (!rt || !extrinsics || !g_extrinsics || !g_rt || ragged_of(layout, &r))
     return fail_msg("fm_pose_chain_bwd_videos: bad arguments");
-  return pose_chain_bwd_ragged(rt, extrinsics, g_extrinsics, g_rt, r, stream);
+  return pose_chain_bwd(rt, extrinsics, g_extrinsics, g_rt, r.B, r.v, stream);
 }
 
 }  // extern "C"

@@ -75,7 +75,7 @@ def _walk(units, per_unit, grid, rounds, video):
 
 def launch_geometry(frames, h, w, sms, l2_bytes=L2_BYTES):
     """{kernel: (rounds, multi, cross)} of the persistent launches of procrustes_fwd<RaggedPairs>
-    (k_moments_dense<..., RaggedPairs>), launch_flow_ragged (k_flow_lean_ragged) and procrustes_bwd<RaggedPairs>
+    (k_moments_dense<..., RaggedPairs>), launch_flow<Videos> (k_flow_lean_ragged) and procrustes_bwd<RaggedPairs>
     (k_distribute_window<RaggedPairs> for W % 4 == 0, else k_distribute_dense<RaggedPairs>) in fm_kernels.cu:
     256-thread chunks of 4 pixels (W % 4 == 0) or 1, 64 x 32 window tiles, 3 / 2 / 3 blocks per SM."""
     pair_video = [b for b, f in enumerate(frames) for _ in range(f - 1)]
