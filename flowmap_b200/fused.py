@@ -14,10 +14,19 @@ step (fm_overfit_step, FM_STEP_FORWARD / FM_STEP_BACKWARD):
     backward half and hands the finished parameter gradients to autograd (no intermediate tensors,
     no per-op ATen glue).
 
+A network backbone (any backbone but BackboneExplicitDepth, e.g. the reference's BackboneMidas: a CNN
+for the depths, a per-pixel MLP or sigmoid(s * weights) for the correspondence weights) stays in
+torch.  `Model.forward` runs it once, under autograd, and the LazyModelOutput keeps its BackboneOutput.
+The root's inputs are then that step's depths and weights, converted to contiguous float32 inside the
+graph; the halves read them with weight sensitivity 0 (the weights themselves, not logits), and the
+root's backward hands d loss / d depths and d loss / d weights to autograd, which carries them on into
+the network.  Outputs read before or after the losses reuse the stored BackboneOutput: the backbone
+never runs twice in one step.
+
 Anything the fused step does not cover (a consumer that reads `model_output.extrinsics` under
-autograd, another backbone, per-frame intrinsics, different mappings for the two losses) makes the
-LazyModelOutput materialise itself through the per-op autograd Functions of flowmap_b200.ops: same
-results, the former speed.
+autograd, a batch of several videos, per-frame intrinsics, different mappings for the two losses)
+makes the LazyModelOutput materialise itself through the per-op autograd Functions of
+flowmap_b200.ops: same results, the former speed.
 """
 from __future__ import annotations
 
@@ -27,11 +36,12 @@ import torch
 from torch import Tensor
 
 from . import ops
-from .types import Batch, Flows, ModelOutput
+from .types import BackboneOutput, Batch, Flows, ModelOutput
 
 
 class _StepRoot(torch.autograd.Function):
-    """Root of one fused step: token = f(parameters).  Its backward runs the backward half."""
+    """Root of one fused step: token = f(parameters, or a network backbone's depths / weights).  Its
+    backward runs the backward half."""
 
     @staticmethod
     def forward(ctx, step, *params):
@@ -40,7 +50,8 @@ class _StepRoot(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, _g_token):
-        return (None, *ctx.step.run_backward())
+        grads = ctx.step.run_backward()
+        return (None, *(g if need else None for g, need in zip(grads, ctx.needs_input_grad[1:])))
 
 
 class _LossNode(torch.autograd.Function):
@@ -60,8 +71,10 @@ class _LossNode(torch.autograd.Function):
 class FusedStep:
     """State of one optimisation step evaluated through the fused halves."""
 
-    def __init__(self, model, batch: Batch, flows: Flows, global_step: int):
+    def __init__(self, model, batch: Batch, flows: Flows, global_step: int,
+                 backbone_out: Optional[BackboneOutput] = None):
         self.model, self.batch, self.flows, self.global_step = model, batch, flows, global_step
+        self.backbone_out = backbone_out  # a network backbone's output of this step, else None
         self.engine = None
         self.token: Optional[Tensor] = None
         self.scales = {}
@@ -78,12 +91,20 @@ class FusedStep:
         self.engine = eng
         eng.cfg.flow_weight, eng.cfg.flow_enable_after = loss_mod.cfg.weight, loss_mod.cfg.enable_after
         eng._msum.copy_(loss_mod._mask_total(self.flows))
-        params = self.model._fused_params(self.global_step)
+        inputs = None
+        if self.backbone_out is not None:  # the kernels read float32 rows; the casts stay in the graph
+            bo = self.backbone_out
+            inputs = [bo.depths.to(torch.float32).contiguous()]
+            if eng.cfg.use_correspondence_weights:
+                inputs.append(bo.weights.to(torch.float32).contiguous())
+        params = self.model._fused_params(self.global_step, inputs)
         for p, buf in zip(params, self._grad_buffers(params)):
-            if p.grad is not None and buf is not None and p.grad.data_ptr() == buf.data_ptr():
+            if p.is_leaf and p.grad is not None and buf is not None and p.grad.data_ptr() == buf.data_ptr():
                 p.grad = p.grad.clone()  # a kept gradient must not alias the buffer about to be rewritten
         self._params = params
-        value = eng.forward_phase(self.global_step, training=self.model.training)
+        value = eng.forward_phase(self.global_step, training=self.model.training,
+                                  depth=None if inputs is None else inputs[0].detach(),
+                                  weights=inputs[1].detach() if inputs is not None and len(inputs) > 1 else None)
         self.token = _StepRoot.apply(self, *params)
         self.flow_done = True
         return _LossNode.apply(self.token, self, "flow", value)
@@ -133,34 +154,45 @@ class FusedStep:
             k = torch.zeros(1, f, 3, 3, device=k4.device)
             k[..., 0, 0], k[..., 1, 1], k[..., 0, 2], k[..., 1, 2], k[..., 2, 2] = \
                 k4[..., 0], k4[..., 1], k4[..., 2], k4[..., 3], 1.0
-            bo = model.backbone.forward(self.batch, self.flows)
+            bo = self.backbone_out
+            if bo is None:
+                bo = model.backbone.forward(self.batch, self.flows)
             weights = bo.weights if model.cfg.use_correspondence_weights else torch.ones_like(bo.weights)
-            return ModelOutput(bo.depths, None, k, ops.pose_chain(rt), weights, relative=rt, k4=k4,
+            return ModelOutput(bo.depths.detach(), None, k, ops.pose_chain(rt), weights.detach(), relative=rt, k4=k4,
                                k_mode="shared_focal")
 
 
 class LazyModelOutput(ModelOutput):
-    """ModelOutput of a fused step: `depths` is the parameter itself, everything else is computed
-    when (and only if) somebody reads it: before the losses through the differentiable per-op path
-    (which retires the fused step for this iteration), after them as detached values of the step
+    """ModelOutput of a fused step: `depths` is the parameter itself (explicit depth) or the network
+    backbone's output, as are a network backbone's `backward_correspondence_weights`; everything else is
+    computed when (and only if) somebody reads it: before the losses through the differentiable per-op
+    path (which retires the fused step for this iteration), after them as detached values of the step
     the fused forward half evaluated."""
 
-    def __init__(self, model, batch: Batch, flows: Flows, global_step: int):
-        object.__setattr__(self, "_lazy", (model, batch, flows, global_step))
+    def __init__(self, model, batch: Batch, flows: Flows, global_step: int,
+                 backbone_out: Optional[BackboneOutput] = None):
+        object.__setattr__(self, "_lazy", (model, batch, flows, global_step, backbone_out))
         object.__setattr__(self, "_full", None)
-        object.__setattr__(self, "_fused", FusedStep(model, batch, flows, global_step))
-        object.__setattr__(self, "depths", model.backbone.depth[None])
+        object.__setattr__(self, "_fused", FusedStep(model, batch, flows, global_step, backbone_out))
+        if backbone_out is None:
+            object.__setattr__(self, "depths", model.backbone.depth[None])
+        else:
+            weights = backbone_out.weights
+            if not model.cfg.use_correspondence_weights:  # model.py:67-68
+                weights = torch.ones_like(weights)
+            object.__setattr__(self, "depths", backbone_out.depths)
+            object.__setattr__(self, "backward_correspondence_weights", weights)
 
     def _materialize(self) -> ModelOutput:
         full = object.__getattribute__(self, "_full")
         if full is None:
-            model, batch, flows, step = object.__getattribute__(self, "_lazy")
+            model, batch, flows, step, backbone_out = object.__getattribute__(self, "_lazy")
             fused = object.__getattribute__(self, "_fused")
             if fused.flow_done:  # the fused losses already consumed this output: values only
                 full = fused.snapshot()
             else:
                 fused.dead = True
-                full = model._forward_materialized(batch, flows, step)
+                full = model._forward_materialized(batch, flows, step, backbone_out)
             object.__setattr__(self, "_full", full)
         return full
 

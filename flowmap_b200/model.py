@@ -265,22 +265,39 @@ class Model(nn.Module):
         self.intrinsics = get_intrinsics(cfg.intrinsics)
         self.extrinsics = get_extrinsics(cfg.extrinsics, num_frames)
 
-    # ---- fused evaluation (flowmap_b200.fused): Model.forward launches nothing, the losses run the
-    # two halves of the fused step
+    # ---- fused evaluation (flowmap_b200.fused): Model.forward launches nothing but a network backbone,
+    # the losses run the two halves of the fused step
     fused_enabled = True  # class-wide switch (tests compare the two evaluation orders)
 
-    def _fusable(self, batch: Batch, flows: Flows) -> bool:
-        return (self.fused_enabled and torch.is_grad_enabled() and self.training and
-                isinstance(self.backbone, BackboneExplicitDepth) and
+    def _fusable(self, batch: Batch, flows: Flows, backbone_out: Optional[BackboneOutput] = None) -> bool:
+        """Whether the losses of this step can run on the fused halves.  A network backbone (any backbone
+        but BackboneExplicitDepth, e.g. the reference's BackboneMidas) is judged on the BackboneOutput of
+        the step: one video of CUDA depths (1, F, H, W) and weights (1, F-1, H, W)."""
+        if not (self.fused_enabled and torch.is_grad_enabled() and self.training and
                 isinstance(self.extrinsics, ExtrinsicsProcrustes) and
                 isinstance(self.intrinsics, (IntrinsicsRegressed, IntrinsicsSoftmin)) and
-                batch.videos.shape[0] == 1 and self.backbone.depth.is_cuda and flows.forward.is_cuda)
+                batch.videos.shape[0] == 1 and flows.forward.is_cuda):
+            return False
+        if isinstance(self.backbone, BackboneExplicitDepth):
+            return self.backbone.depth.is_cuda
+        if backbone_out is None:
+            return False
+        _, f, _, h, w = batch.videos.shape
+        d, wt = backbone_out.depths, backbone_out.weights
+        return (isinstance(d, Tensor) and isinstance(wt, Tensor) and d.is_floating_point() and
+                wt.is_floating_point() and d.device == wt.device == flows.forward.device and
+                tuple(d.shape) == (1, f, h, w) and tuple(wt.shape) == (1, f - 1, h, w))
 
-    def _fused_params(self, global_step: int):
-        """Parameters that receive a gradient from the fused step, in the order of FusedStep's buffers."""
-        params = [self.backbone.depth]
-        if self.cfg.use_correspondence_weights:
-            params.append(self.backbone.weights)
+    def _fused_params(self, global_step: int, inputs=None):
+        """Tensors that receive a gradient from the fused step, in the order of FusedStep's buffers:
+        the explicit-depth parameters, or a network backbone's float32 `inputs` (depths [, weights]) of
+        this step, then the focal length that is being learned."""
+        if inputs is not None:
+            params = list(inputs)
+        else:
+            params = [self.backbone.depth]
+            if self.cfg.use_correspondence_weights:
+                params.append(self.backbone.weights)
         intr = self.intrinsics
         if isinstance(intr, IntrinsicsRegressed):
             params.append(intr.focal_length)
@@ -298,10 +315,13 @@ class Model(nn.Module):
                lm.name, getattr(lm, "delta", 0.01))
         eng = getattr(self, "_engine", None)
         if eng is None or self._engine_key != key:
+            explicit = isinstance(self.backbone, BackboneExplicitDepth)
             soft = isinstance(self.intrinsics, IntrinsicsSoftmin)
             reg = ic.regression if soft else None
+            # a network backbone's BackboneOutput holds the weights themselves: sensitivity 0 to the kernels
             cfg = OverfitCfg(
-                initial_depth=bc.initial_depth, weight_sensitivity=bc.weight_sensitivity,
+                initial_depth=bc.initial_depth if explicit else 0.0,
+                weight_sensitivity=bc.weight_sensitivity if explicit else 0.0,
                 use_correspondence_weights=mc.use_correspondence_weights, procrustes_points=ec.num_points,
                 procrustes_randomize=ec.randomize_points, intrinsics="softmin" if soft else "regressed",
                 softmin_points=ic.num_procrustes_points if soft else 8192,
@@ -312,7 +332,8 @@ class Model(nn.Module):
                 flow_weight=flow_loss.cfg.weight, flow_enable_after=flow_loss.cfg.enable_after,
                 use_tracking=tracks is not None, tracking_enable_after=0, mapping=lm.name,
                 delta=getattr(lm, "delta", 0.01))
-            eng = FusedOverfitter(cfg, batch, flows, tracks, device=self.backbone.depth.device, model=self)
+            dev = self.backbone.depth.device if explicit else flows.forward.device
+            eng = FusedOverfitter(cfg, batch, flows, tracks, device=dev, model=self)
             object.__setattr__(self, "_engine", eng)
             object.__setattr__(self, "_engine_key", key)
             object.__setattr__(self, "_engine_flows", None)
@@ -323,15 +344,24 @@ class Model(nn.Module):
         return eng
 
     def forward(self, batch: Batch, flows: Flows, global_step: int) -> ModelOutput:
-        if self._fusable(batch, flows):
-            from .fused import LazyModelOutput
-            return LazyModelOutput(self, batch, flows, global_step)
-        return self._forward_materialized(batch, flows, global_step)
-
-    def _forward_materialized(self, batch: Batch, flows: Flows, global_step: int) -> ModelOutput:
+        from .fused import LazyModelOutput
+        if isinstance(self.backbone, BackboneExplicitDepth):
+            if self._fusable(batch, flows):
+                return LazyModelOutput(self, batch, flows, global_step)
+            return self._forward_materialized(batch, flows, global_step)
+        # a network backbone runs once per step, under autograd as usual; the fused halves take its output
         backbone_out = self.backbone.forward(batch, flows)
+        if self._fusable(batch, flows, backbone_out):
+            return LazyModelOutput(self, batch, flows, global_step, backbone_out)
+        return self._forward_materialized(batch, flows, global_step, backbone_out)
+
+    def _forward_materialized(self, batch: Batch, flows: Flows, global_step: int,
+                              backbone_out: Optional[BackboneOutput] = None) -> ModelOutput:
+        """The per-op evaluation; `backbone_out` is this step's output of the backbone when it already ran."""
+        if backbone_out is None:
+            backbone_out = self.backbone.forward(batch, flows)
         if not self.cfg.use_correspondence_weights:  # model.py:67-68
-            backbone_out.weights = torch.ones_like(backbone_out.weights)
+            backbone_out = BackboneOutput(backbone_out.depths, torch.ones_like(backbone_out.weights))
         intrinsics = self.intrinsics.forward(batch, flows, backbone_out, global_step)
         k4 = ops.intrinsics_to_k4(intrinsics)
         extrinsics, rt = self.extrinsics.forward(batch, flows, backbone_out, k4)

@@ -13,7 +13,7 @@ from torch import Tensor
 from . import ops
 from .loss import (LossFlowCfg, LossTrackingCfg, MappingHuberCfg, MappingL1Cfg, MappingL2Cfg,
                    get_losses)
-from .model import (BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsRegressedCfg,
+from .model import (BackboneExplicitDepth, BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsRegressedCfg,
                     IntrinsicsSoftminCfg, Model, ModelCfg, RegressionCfg)
 from .types import Batch, Flows
 
@@ -180,11 +180,16 @@ class FusedOverfitter(Overfitter):
       one (B, F-1, ...) Flows.
     - `batch` a list of B one-video Batches of the same H, W, `flows` a list of their Flows (1, F_b - 1, ...):
       videos of different lengths.  training_step() returns the (B,) totals and a list of the videos'
-      relative poses; extrinsics(), intrinsics_k4() and gradients() hand out per-video lists."""
+      relative poses; extrinsics(), intrinsics_k4() and gradients() hand out per-video lists.
+
+    Bound to a Model whose backbone is a network (any backbone but BackboneExplicitDepth, the drop-in
+    surface of flowmap_b200.fused), the optimiser owns no depth or weight buffers and no Adam state for
+    them: every step's depths and weights come from the network, through forward_phase, and only the
+    split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight)."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):
-        self._layout, self._tensor_batch = None, False
+        self._layout, self._tensor_batch, self._network = None, False, False
         if isinstance(batch, (list, tuple)):
             self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
         elif batch.videos.shape[0] > 1:
@@ -222,7 +227,10 @@ class FusedOverfitter(Overfitter):
         self._use_plan = use_splat_plan and cfg.procrustes_points is None and not cfg.procrustes_randomize
         self._plan = ops.SplatPlan(self.flows.backward) if self._use_plan else None
         self.models = [self.model]
-        self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
+        if isinstance(self.model.backbone, BackboneExplicitDepth):
+            self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
+        else:  # a network backbone: the step's depths / weights arrive with forward_phase
+            self._network, self._depth, self._wlog = True, None, None
         intr = self.model.intrinsics
         if cfg.intrinsics != "softmin":
             self._focal = intr.focal_length.data
@@ -328,9 +336,12 @@ class FusedOverfitter(Overfitter):
             self._k4_base = self._cand_k4.reshape(-1, 4)[0].expand(T, 4).contiguous()
             self.window = []
             self.injected_indices = None
-        z = lambda t: torch.zeros_like(t)  # noqa: E731
+        z = lambda t: None if t is None else torch.zeros_like(t)  # noqa: E731
         self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog), z(self._focal), z(self._focal)]
-        self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
+        if self._network:
+            self._g_depth, self._g_w = torch.empty(T, h, w, device=dev), torch.empty(T - B, h, w, device=dev)
+        else:
+            self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
         self._g_focal = torch.zeros_like(self._focal)
         self._k4, self._g_k4 = torch.empty(T, 4, device=dev), torch.empty(T, 4, device=dev)
         self.rt = torch.empty(*pair_dims, 3, 4, device=dev)
@@ -576,14 +587,21 @@ class FusedOverfitter(Overfitter):
         intr = self.model.intrinsics
         return intr.window if hasattr(intr, "window") and self.optimizer is None else self.window
 
-    def forward_phase(self, global_step: int, training: bool = True):
+    def forward_phase(self, global_step: int, training: bool = True, depth: Optional[Tensor] = None,
+                      weights: Optional[Tensor] = None):
         """Poses + flow loss with its direct gradients (fm_overfit_step, FM_STEP_FORWARD; the
         candidate sweep first in the softmin stage).  Returns the weighted flow loss (device scalar,
-        a buffer that the next call overwrites)."""
+        a buffer that the next call overwrites).  Bound to a network backbone, `depth` (1, F, H, W) and,
+        with correspondence weights, `weights` (1, F-1, H, W) are the step's contiguous float32 inputs;
+        they stay referenced until the next call (backward_phase reads them)."""
         from ._lib import check
         self._refuse_videos("the split-step surface")
         c, a, L = self.cfg, self._args, self._lib
         _, f, _, h, w = self.batch.videos.shape
+        if self._network:
+            self._bind_inputs(depth, weights, f, h, w)
+        elif depth is not None or weights is not None:
+            raise ValueError("flowmap_b200: an explicit-depth optimiser reads its own depth and weights")
         dev = self.rt.device
         st = torch.cuda.current_stream().cuda_stream
         P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
@@ -627,6 +645,19 @@ class FusedOverfitter(Overfitter):
                 a.phase = 0
         return self._loss
 
+    def _bind_inputs(self, depth, weights, f, h, w):
+        """Point the step at a network backbone's depths / weights of this step."""
+        use_w = self.cfg.use_correspondence_weights
+        for name, t, shape in (("depth", depth, (1, f, h, w)), ("weights", weights if use_w else None, (1, f - 1, h, w))):
+            if t is None and (name == "depth" or use_w):
+                raise ValueError(f"flowmap_b200: a network backbone's step needs its `{name}`")
+            if t is not None and (tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()
+                                  or t.device != self.rt.device):
+                raise ValueError(f"flowmap_b200: `{name}` must be a contiguous float32 {shape} tensor on {self.rt.device}")
+        self._depth, self._wlog = depth, weights if use_w else None
+        self._args.depth = depth.data_ptr()
+        self._args.weight_logits = weights.data_ptr() if use_w else None
+
     def tracking_forward_phase(self):
         """Chained poses + tracking loss of the step begun by forward_phase (loss_tracking.py:28-61).
         Returns the weighted tracking loss (device scalar buffer)."""
@@ -658,11 +689,17 @@ class FusedOverfitter(Overfitter):
         a.tracks = self._ctypes.pointer(self._pk_c) if with_tracking else None
         a.flow_grad_scale, a.track_grad_scale = P(flow_scale), P(track_scale)
         a.phase, a.step, a.defer_adam = 2, 0, 0  # FM_STEP_BACKWARD
+        # Without tracks this phase adds g_rt / track_g_k4 as a caller's pose / intrinsics gradient: a step
+        # whose tracking loss is not enabled yet (loss.py:40-41) has none, whatever those buffers hold.
+        kept = a.g_rt, a.track_g_k4
+        if not with_tracking:
+            a.g_rt = a.track_g_k4 = None
         with torch.cuda.device(self.rt.device):
             try:
                 check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (backward)")
             finally:
                 a.phase, a.tracks, a.flow_grad_scale, a.track_grad_scale = 0, None, None, None
+                a.g_rt, a.track_g_k4 = kept
             if self._sweep_idx is not None:
                 idx, n = self._sweep_idx, c.softmin_candidates
                 wl = P(self._wlog) if c.use_correspondence_weights else None
@@ -730,6 +767,9 @@ class FusedOverfitter(Overfitter):
         """Returns (total loss (device tensor: a scalar, or the (B,) per-video totals), relative poses
         rt (B, F-1, 3, 4), or a list of (F_b - 1, 3, 4) for videos of different lengths)."""
         c, a = self.cfg, self._args
+        if self._network:
+            raise ValueError("flowmap_b200: a network backbone's step runs through the model's losses "
+                             "(forward_phase / backward_phase), not training_step")
         if c.procrustes_randomize:
             self._indices = self.model.extrinsics.select_indices(*self._hw, self.rt.device)
         a.indices = None if self._indices is None else self._indices.data_ptr()
