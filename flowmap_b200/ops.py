@@ -490,9 +490,11 @@ class _TrackLoss(torch.autograd.Function):
 
 def track_loss(depths, extrinsics, k4, packed: PackedTracks, mapping="huber", delta=0.01,
                weight=1.0, shared_k: bool = False) -> Tensor:
-    """shared_k: all frames share their intrinsics (k4 derives from one focal length or is constant)
-    and the caller only uses the sum over frames of d loss / d k4 (true when k4 is an expand of one
-    row): lets the kernel skip the per-target-frame reduction of the intrinsics terms."""
+    """shared_k: the caller only uses the sum over frames of d loss / d k4 -- true when k4 is an expand
+    of one row (one focal length), and when the intrinsics take no gradient at all (ground-truth K,
+    k_mode "const", which may differ per frame).  The loss, depth and pose gradients still use every
+    frame's own k4; only the intrinsics gradient is left unreduced per target frame, so g_k4 is then
+    meaningful only as its sum over frames."""
     return _TrackLoss.apply(depths, extrinsics, k4, packed, mapping, delta, weight, shared_k)
 
 

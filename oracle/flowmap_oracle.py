@@ -426,7 +426,7 @@ class OverfitConfig:
     use_correspondence_weights: bool = True  # overfit.yaml:44-45
     procrustes_points: Optional[int] = None  # ablation_explicit_depth.yaml:11-12 (default 1000)
     procrustes_randomize: bool = False
-    intrinsics: str = "softmin"  # "softmin" | "regressed"
+    intrinsics: str = "softmin"  # "softmin" | "regressed" | "ground_truth" (K given to OverfitOracle)
     initial_focal: float = 0.85  # model/intrinsics/regressed.yaml
     softmin_points: int = 8192  # model/intrinsics/softmin.yaml
     softmin_min: float = 0.5
@@ -459,12 +459,17 @@ class OverfitOracle:
 
     Restates model.py:54-90 (forward), loss.py:31-47 (gating/weighting),
     model_wrapper_overfit.py:51-73 (training_step) and :104-105 (Adam(lr)).
-    ``global_step`` is the number of optimiser steps already taken.
+    ``global_step`` is the number of optimiser steps already taken.  With ``intrinsics="ground_truth"``
+    (intrinsics_ground_truth.py:18-27: K is the batch's) ``intrinsics`` is that K, (f, 3, 3) or
+    (1, f, 3, 3), per frame; the focal length then takes no part and gets no gradient.
     """
 
     def __init__(self, cfg: OverfitConfig, num_frames: int, h: int, w: int,
-                 dtype=torch.float32):
+                 dtype=torch.float32, intrinsics: Optional[Tensor] = None):
         self.cfg, self.f, self.h, self.w, self.dtype = cfg, num_frames, h, w, dtype
+        if (cfg.intrinsics == "ground_truth") != (intrinsics is not None):
+            raise ValueError("intrinsics are given exactly when cfg.intrinsics is 'ground_truth'")
+        self.k_given = None if intrinsics is None else intrinsics.to(dtype).reshape(1, num_frames, 3, 3)
         self.depth = torch.full((num_frames, h, w), cfg.initial_depth, dtype=dtype,
                                 requires_grad=True)
         self.weights = torch.zeros((num_frames - 1, h, w), dtype=dtype, requires_grad=True)
@@ -485,6 +490,8 @@ class OverfitOracle:
                     softmin_indices: Optional[Tensor]):
         c = self.cfg
         b = depths.shape[0]
+        if c.intrinsics == "ground_truth":
+            return self.k_given.expand(b, self.f, 3, 3)
         regress = c.intrinsics == "regressed" or (
             c.regression_after is not None and step >= c.regression_after)
         if regress:

@@ -4,6 +4,7 @@ Run where a checkout of the reference is available (FLOWMAP_REFERENCE names its 
 
     python tests/golden/make_golden.py            # float32 run of the reference
     python tests/golden/make_golden.py --f64      # float64 run of the same modules
+    python tests/golden/make_golden.py --only gt_intrinsics [--f64]   # write one case only
 
 The reference ships no tests or golden vectors for this path (SURVEY.md section 4), so
 these files are the pin for ``oracle/flowmap_oracle.py`` and, through it, for the CUDA
@@ -67,6 +68,7 @@ def _tracks(seed, segments, n_points, dtype):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--f64", action="store_true")
+    ap.add_argument("--only", help="write only this case (every case is still computed)")
     args = ap.parse_args()
 
     real_f32 = torch.float32
@@ -93,6 +95,7 @@ def main():
     from flowmap.model.backbone.backbone_explicit_depth import BackboneExplicitDepthCfg
     from flowmap.model.extrinsics.extrinsics_procrustes import ExtrinsicsProcrustesCfg
     from flowmap.model.intrinsics.common import focal_lengths_to_intrinsics
+    from flowmap.model.intrinsics.intrinsics_ground_truth import IntrinsicsGroundTruthCfg
     from flowmap.model.intrinsics.intrinsics_regressed import IntrinsicsRegressedCfg
     from flowmap.model.intrinsics.intrinsics_softmin import (IntrinsicsSoftminCfg,
                                                              RegressionCfg)
@@ -108,9 +111,11 @@ def main():
                 "l2": MappingL2Cfg("l2")}[name]
 
     def build(f, h, w, inp, intr="regressed", focal=0.85, npts=None, mapping="huber",
-              tracking=False, softmin_pts=300, regression=None):
+              tracking=False, softmin_pts=300, regression=None, k=None):
         if intr == "regressed":
             icfg = IntrinsicsRegressedCfg("regressed", focal)
+        elif intr == "ground_truth":  # K is the batch's (intrinsics_ground_truth.py)
+            icfg = IntrinsicsGroundTruthCfg("ground_truth")
         else:
             icfg = IntrinsicsSoftminCfg("softmin", softmin_pts, 0.5, 2.0, 60, regression)
         mcfg = ModelCfg(BackboneExplicitDepthCfg("explicit_depth", 0.1, 100.0), icfg,
@@ -124,7 +129,8 @@ def main():
             lcfgs.append(LossTrackingCfg(0, 100.0, "tracking", mapping_cfg(mapping)))
         losses = get_losses(lcfgs)
         batch = Batch(torch.zeros((1, f, 3, h, w), dtype=dtype),
-                      torch.arange(f)[None], ["s"], ["d"])
+                      torch.arange(f)[None], ["s"], ["d"],
+                      intrinsics=None if k is None else k.to(dtype))
         flows = Flows(inp["fwd"].to(dtype), inp["bwd"].to(dtype), inp["fmask"].to(dtype),
                       inp["bmask"].to(dtype))
         return model, losses, batch, flows
@@ -146,6 +152,8 @@ def main():
         return {k: npy(v) for k, v in d.items() if v is not None}
 
     def save(name, **arrays):
+        if args.only and name != args.only:
+            return
         path = OUT / f"{name}{suffix}.npz"
         arrays = {k: (np.asarray(v) if not isinstance(v, torch.Tensor) else npy(v))
                   for k, v in arrays.items()}
@@ -269,6 +277,52 @@ def main():
 
     run_traj("traj_generic", 5, 16, 24, seed=31, steps=6, from_init=False)
     run_traj("traj_init", 4, 16, 24, seed=32, steps=6, from_init=True)
+
+    # ------------------------------------------------------------------ ground-truth intrinsics
+    # model/intrinsics: ground_truth on calibrated data: a K per frame, off-centre and anisotropic.
+    # fx grows 1.5x and fy 1.4x over the video (fx != fy H / W), the principal point drifts from
+    # (0.3, 0.7) to (0.7, 0.3).  Flow + tracking (overlapping segments, tracks leaving the frame).
+    f, h, w = 6, 20, 28
+    inp = _inputs(41, f, h, w)
+    s_ = (h * w) ** 0.5
+    t_ = torch.linspace(0.0, 1.0, f, dtype=torch.float64)
+    kgt = torch.zeros(1, f, 3, 3, dtype=torch.float64)
+    kgt[0, :, 0, 0] = 0.8 * s_ / w * (1 + 0.5 * t_)
+    kgt[0, :, 1, 1] = 0.95 * s_ / h * (1 + 0.4 * t_)
+    kgt[0, :, 0, 2] = 0.3 + 0.4 * t_
+    kgt[0, :, 1, 2] = 0.7 - 0.4 * t_
+    kgt[0, :, 2, 2] = 1.0
+    model, losses, batch, flows = build(f, h, w, inp, intr="ground_truth", tracking=True, k=kgt)
+    tracks, raw = _tracks(42, [(0, 4), (2, 4)], 60, dtype)
+    out, parts, total = step(model, losses, batch, flows, tracks, 0)
+    total.backward()
+    tr = {}
+    for i, (txy, tvis, s) in enumerate(raw):
+        tr[f"trk{i}_xy"], tr[f"trk{i}_vis"], tr[f"trk{i}_start"] = txy.numpy(), tvis.numpy(), s
+    fwd_xy = P.compute_forward_flow(out.surfaces, out.extrinsics, out.intrinsics)
+    bwd_xy = P.compute_backward_flow(out.surfaces, out.extrinsics, out.intrinsics)
+    tgt1, vis1 = P.compute_track_flow(out.surfaces[:, 2:6], out.extrinsics[:, 2:6],
+                                      out.intrinsics[:, 2:6], tracks[1])
+    # projection unit under the same K: unproject, project (world points, incl. the nan_to_num
+    # branch at z = -1e-5 in camera space) and reproject_points
+    g = torch.Generator().manual_seed(43)
+    kd = kgt.to(dtype)
+    z = (0.5 + torch.rand(1, f, h, w, generator=g, dtype=torch.float64)).to(dtype)
+    xy, _ = P.sample_image_grid((h, w))
+    u_surf = P.unproject(xy.to(dtype), z, kd[:, :, None, None])
+    cam = torch.randn(1, f, 40, 3, generator=g, dtype=torch.float64).to(dtype)
+    cam[..., 2] = cam[..., 2].abs() + 0.3
+    cam[0, :, :5, 2] = -cam[0, :, :5, 2]  # behind the camera
+    cam[0, 0, 5, 2] = -1e-5
+    cam[0, 1, 6] = torch.tensor([0.0, 0.0, -1e-5], dtype=dtype)
+    eye = torch.eye(4, dtype=dtype).expand(1, f, 4, 4)
+    p_xy, p_front = P.project(cam, eye[:, :, None], kd[:, :, None])
+    rel_t = out.extrinsics.detach()
+    r_xy = P.reproject_points(cam, rel_t[:, :, None], kd[:, :, None])
+    save("gt_intrinsics", **input_arrays(inp), **tr, intrinsics=kgt, loss=total, loss_flow=parts[0],
+         loss_tracking=parts[1], extrinsics=out.extrinsics, fwd_xy=fwd_xy[:, :2], bwd_xy=bwd_xy[:, :2],
+         trk1_target=tgt1, trk1_valid=vis1, unit_z=z, unit_surfaces=u_surf, unit_cam=cam, unit_proj_xy=p_xy,
+         unit_proj_front=p_front, unit_rel=rel_t, unit_reproj_xy=r_xy, **grads_of(model))
 
 
 if __name__ == "__main__":

@@ -164,14 +164,24 @@ def test_metrics_log_without_ground_truth_is_nan():
 def test_metrics_log_leaves_the_optimisation_unchanged():
     """Log on vs off: the same losses and parameters up to the run-to-run noise of the float atomics,
     and per step one more launch with the tracking loss, two without (the pose chain).  Launches are
-    counted on the eager steps (graph replays launch nothing from the host)."""
+    counted on the eager steps (graph replays launch nothing from the host).
+
+    The parameters after 10 Adam steps carry that noise amplified: Adam divides each gradient by its own
+    running magnitude, so the last bits of a near-zero gradient move its parameter by up to the learning
+    rate.  Runs with the log off differ from each other by 1e-8 to 5e-7 in the weights (four runs on one
+    H100), and a run with the log on was seen 1.1e-6 away.  So the parameters are held to 1e-6 or 3x the
+    largest difference among three runs without the log, whichever is larger."""
     on, _, _ = _run(16)
-    off, _, _ = _run(0)
+    offs = [_run(0)[0] for _ in range(3)]
+    off = offs[0]
     for s in range(STEPS):
         a, b = float(on["total"][s]), float(off["total"][s])
         assert abs(a - b) <= 1e-6 * abs(b), (s, a, b)
-    assert rel_l2(on["depth"], off["depth"]) <= 1e-6
-    assert rel_l2(on["weights"], off["weights"]) <= 1e-6
+    for name in ("depth", "weights"):
+        e = rel_l2(on[name], off[name])
+        noise = max(rel_l2(offs[i][name], offs[j][name]) for i in range(3) for j in range(i + 1, 3))
+        print(f"{name}: log on vs off {e:.1e}, off vs off {noise:.1e}")
+        assert e <= max(1e-6, 3 * noise), (name, e, noise)
     extra = [a - b for a, b in zip(on["launches"][:6], off["launches"][:6])]  # steps 0-5 run eagerly
     assert extra == [2, 2, 1, 1, 1, 1], extra
 

@@ -60,56 +60,73 @@ def flow_k4_grad(flowacc, B, F):
     return g
 
 
-def run_emulated_step(emu, g, mapping=0, focal=0.85, indices=None, delta=0.01, weight=1000.0,
-                      lean=False):
-    depth = np.ascontiguousarray(g["in_depth"], dtype=np.float32)
-    F_, H, W = depth.shape
-    B = 1
-    wparam = torch.as_tensor(g["in_wparam"], dtype=torch.float32)
-    w = torch.sigmoid(100.0 * wparam).numpy()
-    ff = np.ascontiguousarray(g["in_fwd"], dtype=np.float32)
-    fb = np.ascontiguousarray(g["in_bwd"], dtype=np.float32)
-    mf = np.ascontiguousarray(g["in_fmask"], dtype=np.float32)
-    mb = np.ascontiguousarray(g["in_bmask"], dtype=np.float32)
-    s = (H * W) ** 0.5
-    k4 = np.tile(np.array([focal * s / W, focal * s / H, 0.5, 0.5], dtype=np.float32), (F_, 1))
-    BP = F_ - 1
+def _emulate(emu, depth, w, ff, fb, mf, mb, k4, indices, mapping, delta, weight, lean, focal_mode):
+    """One flow-loss step through the per-pixel headers: Procrustes forward, the flow loss (k_flow's
+    code, or k_flow_lean's with FOCAL = focal_mode), the pose gradient, the Procrustes backward.
+    depth (B, F, H, W), w the weights (B, F-1, H, W), flows in their layouts, k4 (B*F, 4), all float32.
+    Returns the loss, rt (B*(F-1), 12), the depth gradient, d loss / d weights, the intrinsics gradient
+    (B*F, 4: flow_k4_grad's per-frame part plus the Procrustes backward's) and the flow loss's own depth
+    gradient (`direct`)."""
+    B, F_, H, W = depth.shape
+    BP = B * (F_ - 1)
     rt = np.zeros((BP, 12), dtype=np.float32)
     state = np.zeros(BP * emu.emu_state_bytes(), dtype=np.uint8)
     idx = None if indices is None else np.ascontiguousarray(indices, dtype=np.int64)
     n_idx = 0 if idx is None else len(idx)
-    emu.emu_procrustes_fwd(_p(depth), _p(k4), _p(fb), _p(w), _p(idx), n_idx, _p(rt), _p(state),
-                           B, F_, H, W)
+    emu.emu_procrustes_fwd(_p(depth), _p(k4), _p(fb), _p(w), _p(idx), n_idx, _p(rt), _p(state), B, F_, H, W)
     mask_sum = float(mf.astype(np.float64).sum() + mb.astype(np.float64).sum())
     g_depth = np.zeros_like(depth)
-    flowacc = np.zeros((F_, 40), dtype=np.float64)
-    if lean:  # shared-focal kernel: twist pose accumulators, one focal accumulator
-        emu.emu_flow_lean(_p(depth), _p(k4), _p(rt), _p(ff), _p(fb), _p(mf), _p(mb),
-                          ctypes.c_double(mask_sum), mapping, ctypes.c_float(delta),
-                          ctypes.c_float(weight), 1, _p(g_depth), _p(flowacc), B, F_, H, W)
+    flowacc = np.zeros((B * F_, 40), dtype=np.float64)
+    if lean:
+        emu.emu_flow_lean(_p(depth), _p(k4), _p(rt), _p(ff), _p(fb), _p(mf), _p(mb), ctypes.c_double(mask_sum),
+                          mapping, ctypes.c_float(delta), ctypes.c_float(weight), focal_mode, _p(g_depth),
+                          _p(flowacc), B, F_, H, W)
     else:
-        emu.emu_flow(_p(depth), _p(k4), _p(rt), _p(ff), _p(fb), _p(mf), _p(mb),
-                     ctypes.c_double(mask_sum), mapping, ctypes.c_float(delta),
-                     ctypes.c_float(weight), _p(g_depth), _p(flowacc), B, F_, H, W)
-    loss = flowacc[:, 0].sum()
+        emu.emu_flow(_p(depth), _p(k4), _p(rt), _p(ff), _p(fb), _p(mf), _p(mb), ctypes.c_double(mask_sum), mapping,
+                     ctypes.c_float(delta), ctypes.c_float(weight), _p(g_depth), _p(flowacc), B, F_, H, W)
     g_rt = flow_pose_grad(flowacc, rt, B, F_)
     g_w = np.zeros_like(w)
-    k4acc = np.zeros((F_, 4), dtype=np.float64)
+    k4acc = np.zeros((B * F_, 4), dtype=np.float64)
     direct = g_depth.copy()
-    emu.emu_procrustes_bwd(_p(depth), _p(k4), _p(fb), _p(w), _p(idx), n_idx, _p(state), _p(g_rt),
-                           _p(g_depth), _p(g_w), _p(k4acc), B, F_, H, W)
-    g_k4 = flow_k4_grad(flowacc, B, F_) + k4acc
-    g_focal = (g_k4[:, 0] * s / W + g_k4[:, 1] * s / H).sum()
-    wt = torch.as_tensor(w, dtype=torch.float64)
-    g_wparam = torch.as_tensor(g_w, dtype=torch.float64) * 100.0 * wt * (1 - wt)
-    # chain the relative poses (float64 here; the float32 chain is checked on the GPU)
-    P = [np.eye(4)]
-    for i in range(BP):
-        T = np.eye(4)
-        T[:3] = rt[i].reshape(3, 4)
-        P.append(P[-1] @ T)
-    return dict(loss=loss, extrinsics=np.stack(P)[None], g_depth=g_depth, g_wparam=g_wparam.numpy(),
-                g_focal=g_focal, direct=direct, rt=rt)
+    emu.emu_procrustes_bwd(_p(depth), _p(k4), _p(fb), _p(w), _p(idx), n_idx, _p(state), _p(g_rt), _p(g_depth),
+                           _p(g_w), _p(k4acc), B, F_, H, W)
+    return dict(loss=flowacc[:, 0].sum(), rt=rt, g_depth=g_depth, g_w=g_w, direct=direct,
+                g_k4=flow_k4_grad(flowacc, B, F_) + k4acc)
+
+
+def _chain(rt, B, F_):
+    """Camera-to-world extrinsics (B, F, 4, 4) of the relative poses, chained in float64 (the float32
+    chain is checked on the GPU)."""
+    ext = []
+    for bi in range(B):
+        P = [np.eye(4)]
+        for i in range(F_ - 1):
+            T = np.eye(4)
+            T[:3] = rt[bi * (F_ - 1) + i].reshape(3, 4)
+            P.append(P[-1] @ T)
+        ext.append(np.stack(P))
+    return np.stack(ext)
+
+
+def _wparam_grad(g_w, wt):
+    """d loss / d weight logits from d loss / d weights (weights = sigmoid(100 logits))."""
+    return torch.as_tensor(g_w, dtype=torch.float64) * 100.0 * wt * (1 - wt)
+
+
+def run_emulated_step(emu, g, mapping=0, focal=0.85, indices=None, delta=0.01, weight=1000.0,
+                      lean=False):
+    """One video of a golden case, K from one focal length; lean: k_flow_lean with FOCAL = true."""
+    depth = np.ascontiguousarray(g["in_depth"], dtype=np.float32)
+    F_, H, W = depth.shape
+    wt = torch.sigmoid(100.0 * torch.as_tensor(g["in_wparam"], dtype=torch.float32))
+    ff, fb, mf, mb = (np.ascontiguousarray(g[k], dtype=np.float32) for k in ("in_fwd", "in_bwd", "in_fmask", "in_bmask"))
+    s = (H * W) ** 0.5
+    k4 = np.tile(np.array([focal * s / W, focal * s / H, 0.5, 0.5], dtype=np.float32), (F_, 1))
+    r = _emulate(emu, depth[None], wt.numpy(), ff, fb, mf, mb, k4, indices, mapping, delta, weight, lean, 1)
+    g_focal = (r["g_k4"][:, 0] * s / W + r["g_k4"][:, 1] * s / H).sum()
+    return dict(loss=r["loss"], extrinsics=_chain(r["rt"], 1, F_), g_depth=r["g_depth"][0],
+                g_wparam=_wparam_grad(r["g_w"], wt.double()).numpy(), g_focal=g_focal, direct=r["direct"][0],
+                rt=r["rt"])
 
 
 CASES = [("flow_huber", 0, 0.85, None), ("flow_l1", 1, 0.85, None), ("flow_l2", 2, 0.85, None),
@@ -209,3 +226,62 @@ def test_emulated_step_in_flow_regimes_vs_float64_oracle(emu, regime_cases, kind
                g_w=torch.as_tensor(r["g_wparam"]), g_focal=r["g_focal"])
     check(errors(out, refs[64], per_item=False), noise, f"{kind} {f}x{h}x{w} lean={lean}",
           loss_tol=1e-4, pose_tol=1e-5, floor=2e-5)
+
+
+def run_emulated_step_k4(emu, depth, wparam, flows, k4, indices=None, lean=False):
+    """One flow-loss step on b videos (b, f, h, w) under per-frame intrinsics k4 (b, f, 4).  lean:
+    k_flow_lean's code with FOCAL = false (k_mode "const": the flow loss gives K no gradient), else
+    k_flow's (k_mode "full").  g_k4 (b, f, 4)."""
+    B, F_, H, W = depth.shape
+    wt = torch.sigmoid(100.0 * wparam.float())
+    f32 = lambda t: np.ascontiguousarray(t.numpy(), dtype=np.float32)  # noqa: E731
+    r = _emulate(emu, f32(depth), f32(wt), f32(flows.forward), f32(flows.backward), f32(flows.forward_mask),
+                 f32(flows.backward_mask), f32(k4), indices, 0, 0.01, 1000.0, lean, 0)
+    return dict(loss=r["loss"], ext=torch.as_tensor(_chain(r["rt"], B, F_)), g_depth=torch.as_tensor(r["g_depth"]),
+                g_w=_wparam_grad(r["g_w"], wt.double()), g_k4=torch.as_tensor(r["g_k4"]).reshape(B, F_, 4))
+
+
+@pytest.fixture(scope="module")
+def k4_cases():
+    """Oracle results under per-frame intrinsics, computed once per (K regime, flows, points)."""
+    return {}
+
+
+@pytest.mark.parametrize("lean", [False, True], ids=["full", "lean-const"])
+@pytest.mark.parametrize("points", [None, "linspace"], ids=["all", "pts300"])
+@pytest.mark.parametrize("flows", ["shift", "scene"])
+@pytest.mark.parametrize("kregime", ["offcentre", "zoom", "corner", "videos"])
+def test_emulated_step_with_per_frame_intrinsics_vs_float64_oracle(emu, k4_cases, kregime, flows, points, lean):
+    """The per-pixel code under the intrinsics of calibrated videos (flow_regime_checks.k4_regime): per-frame,
+    off-centre, anisotropic K, a different K per video (B = 2), on the all-pixel and the index Procrustes
+    paths.  A frame that reads its neighbour's K, or a principal point taken as 0.5, is wrong here and nowhere
+    with the focal-length K of the other cases.  The intrinsics gradient is checked per video, frame and
+    component: both routes that place it (flow_k4_grad's neighbour slots, distribute_point's kacc halves)."""
+    from oracle import flowmap_oracle as O
+    from flow_regime_checks import check, errors, k4_errors, k4_regime, k4_scene, oracle_steps_k4
+    b, f, h, w = 2, 4, 24, 32
+    key = (kregime, flows, points)
+    if key not in k4_cases:
+        k4 = k4_regime(kregime, b, f, h, w)
+        if flows == "scene":
+            depth, fl = k4_scene(k4, h, w, seed=11)
+        else:
+            depth, fl, _, _ = O.flow_regime(flows, f, h, w, seed=11, b=b)
+        depth = depth * (1.0 + 0.02 * torch.randn(depth.shape, generator=torch.Generator().manual_seed(12),
+                                                  dtype=torch.float64))
+        # the kernels see float32 inputs: give the oracle the same values, so input rounding is not error
+        depth, k4 = depth.float().double(), k4.float().double()
+        fl = O.Flows(*(t.float().double() for t in (fl.forward, fl.backward, fl.forward_mask, fl.backward_mask)))
+        wparam = (0.01 * torch.randn(b, f - 1, h, w, generator=torch.Generator().manual_seed(13),
+                                     dtype=torch.float64)).float().double()
+        idx = None if points is None else torch.linspace(0, h * w - 1, 300, dtype=torch.int64)
+        refs = oracle_steps_k4(depth, wparam, fl, k4, idx)
+        k4_cases[key] = (depth, wparam, fl, k4, idx, refs)
+    depth, wparam, fl, k4, idx, refs = k4_cases[key]
+    r = run_emulated_step_k4(emu, depth, wparam, fl, k4, None if idx is None else idx.numpy(), lean)
+    gk = "g_k4_const" if lean else "g_k4"
+    noise = errors(refs[32], refs[64])
+    noise.update(k4_errors(refs[32][gk], refs[64][gk], noise=True))
+    errs = errors(dict(r, g_focal=None), refs[64])
+    errs.update(k4_errors(r["g_k4"], refs[64][gk]))
+    check(errs, noise, f"{kregime} {flows} {points} lean={lean}", loss_tol=1e-4, pose_tol=1e-5, floor=2e-5)

@@ -72,6 +72,57 @@ def test_flow_step(name, kw, f64):
 
 
 @pytest.mark.parametrize("f64", [False, True])
+def test_ground_truth_intrinsics(f64):
+    """OverfitOracle with intrinsics="ground_truth" against the reference's Model with
+    IntrinsicsGroundTruth on a K per frame (fx x1.5, fy x1.4 over the video, principal point drifting
+    from (0.3, 0.7) to (0.7, 0.3)), flow + tracking loss: poses, loss parts, gradients, the induced flow
+    positions (K of the later / earlier frame) and the track targets of a segment that starts at frame 2.
+    Then the projection unit under the same K: unproject, project (incl. the nan_to_num branch) and
+    reproject_points."""
+    g = load_golden("gt_intrinsics", f64)
+    dt = torch.float64 if f64 else torch.float32
+    f, h, w = g["in_depth"].shape
+    st = O.OverfitOracle(O.OverfitConfig(intrinsics="ground_truth", use_tracking=True, tracking_enable_after=0),
+                         f, h, w, dtype=dt, intrinsics=T(g["intrinsics"]))
+    with torch.no_grad():
+        st.depth.copy_(T(g["in_depth"]).to(dt))
+        st.weights.copy_(T(g["in_wparam"]).to(dt))
+    flows = O.Flows(*(T(g[k]).to(dt) for k in ("in_fwd", "in_bwd", "in_fmask", "in_bmask")))
+    tracks = [O.Tracks(T(g[f"trk{i}_xy"]).to(dt), T(g[f"trk{i}_vis"]), int(g[f"trk{i}_start"])) for i in range(2)]
+    tol = 1e-11 if f64 else 2e-5
+    out = st.forward(flows, 0)
+    assert max_abs(out.extrinsics.detach(), g["extrinsics"]) <= tol
+    # the first two pairs, as stored
+    fwd = O.forward_flow_positions(out.surfaces, out.extrinsics, out.intrinsics).detach()
+    bwd = O.backward_flow_positions(out.surfaces, out.extrinsics, out.intrinsics).detach()
+    assert max_abs(fwd[:, :2], g["fwd_xy"]) <= tol
+    assert max_abs(bwd[:, :2], g["bwd_xy"]) <= tol
+    tgt, valid = O.track_positions(out.surfaces[:, 2:6], out.extrinsics[:, 2:6], out.intrinsics[:, 2:6], tracks[1])
+    assert bool((valid.numpy() == g["trk1_valid"]).all())
+    v = T(g["trk1_valid"])
+    assert max_abs(tgt.detach()[v], T(g["trk1_target"])[v]) <= (1e-10 if f64 else 1e-4)
+    r = st.training_step(flows, tracks)
+    lt, gt = (1e-10, 1e-7) if f64 else (5e-5, 5e-3)
+    assert abs(r["loss"] - float(g["loss"])) <= lt * abs(float(g["loss"]))
+    assert abs(r["parts"]["flow"] - float(g["loss_flow"])) <= lt * abs(float(g["loss_flow"]))
+    assert abs(r["parts"]["tracking"] - float(g["loss_tracking"])) <= lt * abs(float(g["loss_tracking"]))
+    assert rel_l2(r["grads"]["depth"], g["g_depth"]) <= gt
+    assert rel_l2(r["grads"]["weights"], g["g_wparam"]) <= gt
+    assert r["grads"]["focal"] is None
+
+    k = T(g["intrinsics"]).to(dt)
+    surf = O.unproject(O.pixel_grid(h, w, dt), T(g["unit_z"]), k[:, :, None, None])
+    assert max_abs(surf, g["unit_surfaces"]) <= tol * 10
+    cam = T(g["unit_cam"])
+    xy = O.project_camera_space(cam, k[:, :, None])  # identity extrinsics: world = camera space
+    assert np.allclose(xy.numpy(), g["unit_proj_xy"], rtol=1e-5 if not f64 else 1e-12, atol=tol)
+    assert bool(((cam[..., 2] >= 0).numpy() == g["unit_proj_front"]).all())
+    rxy = O.reproject(cam, T(g["unit_rel"])[:, :, None], k[:, :, None])
+    # float32: a moved point 1e-3 in front of the camera plane amplifies rounding of the transform by 1e3
+    assert np.allclose(rxy.numpy(), g["unit_reproj_xy"], rtol=1e-4 if not f64 else 1e-12, atol=tol)
+
+
+@pytest.mark.parametrize("f64", [False, True])
 def test_flow_positions(f64):
     g = load_golden("flow_huber", f64)
     dt = torch.float64 if f64 else torch.float32
