@@ -969,7 +969,10 @@ struct AdamFuse {
   const float* consts;  // device {step_size, bc2_sqrt} of a step clock (CUDA-graph replays), or NULL
 };
 
-template <int VEC, class Lay>
+// KGRAD (this kernel and the two dense ones): accumulate the intrinsics gradient into k4acc.  Without it
+// (constant intrinsics: the fused step's ground-truth K) the pixel loop carries no K accumulators and
+// k4acc is not touched.
+template <int VEC, bool KGRAD, class Lay>
 __global__ void __launch_bounds__(kThreads, 3)
 k_distribute(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow,
              float* weights, const int64_t* __restrict__ indices, int num_indices,
@@ -1006,16 +1009,16 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4, cons
       const int r = j / W, c = j - r * W;
       float gdj, gwj;
       const float wj = wt ? weight_of(__ldg(wt + j), wsens) : 1.f;
-      distribute_point(g, ad, pix_coord(c, g.grid.Wf, g.grid.invW),
-                       pix_coord(r, g.grid.Hf, g.grid.invH), __ldg(db + j),
-                       wj, __ldg(fl + 2 * j), __ldg(fl + 2 * j + 1), load_a,
-                       scatter, gdj, gwj, kacc);
+      distribute_point<KGRAD>(g, ad, pix_coord(c, g.grid.Wf, g.grid.invW),
+                              pix_coord(r, g.grid.Hf, g.grid.invH), __ldg(db + j),
+                              wj, __ldg(fl + 2 * j), __ldg(fl + 2 * j + 1), load_a,
+                              scatter, gdj, gwj, kacc);
       red_add(gdb + j, gdj);
       if (gw) red_add(gw + j, wsens != 0.f ? gwj * wsens * wj * (1.0f - wj) : gwj);
     }
   }
   // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
-  block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
+  if (KGRAD) block_accumulate<8>(kacc, k4acc + (size_t)a * 4, smem);
 }
 
 // Per-pixel work of the dense phase D2 for the VEC consecutive pixels of row r from column c0
@@ -1023,7 +1026,7 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4, cons
 // earlier frame's taps go to `scatter`, the later frame's depth gradient is one aligned RED, then the
 // weight gradient and (fuse_adam) the Adam update of the logits.  The weight-shaped arrays are passed
 // without the pair's offset.
-template <int VEC, typename Scatter>
+template <int VEC, bool KGRAD, typename Scatter>
 __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairAdjoint& ad, const float* da,
                                                   const float* db, const float* fl, float* weights, float* gdb,
                                                   float* g_weights, float wsens, const AdamFuse& adam,
@@ -1050,8 +1053,8 @@ __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairA
   const float y = pix_coord(r, g.grid.Hf, g.grid.invH);
 #pragma unroll
   for (int v = 0; v < VEC; ++v)
-    distribute_point(g, ad, pix_coord(c0 + v, g.grid.Wf, g.grid.invW), y, dv[v], wv[v],
-                     fv[2 * v], fv[2 * v + 1], load_a, scatter, gdv[v], gwv[v], kacc);
+    distribute_point<KGRAD>(g, ad, pix_coord(c0 + v, g.grid.Wf, g.grid.invW), y, dv[v], wv[v],
+                            fv[2 * v], fv[2 * v + 1], load_a, scatter, gdv[v], gwv[v], kacc);
   if (VEC == 4) red_add4(gdb + base, gdv[0], gdv[1], gdv[2], gdv[3]);
   else red_add(gdb + base, gdv[0]);
   if (wt) {
@@ -1090,7 +1093,7 @@ __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairA
   const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ bflow, float* weights, \
       const PairAdjoint* __restrict__ adj, float* __restrict__ g_depth, float* __restrict__ g_weights,        \
       double* __restrict__ k4acc, float wsens
-template <class Lay>
+template <bool KGRAD, class Lay>
 __global__ void __launch_bounds__(kThreads, 3)
 k_distribute_dense(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, int W, int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
@@ -1123,13 +1126,13 @@ k_distribute_dense(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, in
 #pragma unroll 1
     for (int c = cb; c < ce; ++c, base += kThreads) {
       if (base < N)
-        distribute_pixels<1>(g, ad, da, da + N, bflow + pa.flow, weights, gda + N, g_weights, wsens, adam, false,
-                             pa.weight + base, base, r, c0, scatter, kacc);
+        distribute_pixels<1, KGRAD>(g, ad, da, da + N, bflow + pa.flow, weights, gda + N, g_weights, wsens, adam,
+                                    false, pa.weight + base, base, r, c0, scatter, kacc);
       r += dr; c0 += dc;
       if (c0 >= W) { c0 -= W; ++r; }
     }
     // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
-    block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
+    if (KGRAD) block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
     i += ce - cb;
   }
   }
@@ -1199,7 +1202,7 @@ namespace {
 // neighbouring windows overlap, and k_track_apply adds into the same gradient concurrently in
 // fm_overfit_step) and zeroed.  This replaces ~2.6 scattered 32-byte RED requests per pixel (bound by
 // the L2 atomic units) with ~0.7 coalesced ones.
-template <class Lay>
+template <bool KGRAD, class Lay>
 __global__ void __launch_bounds__(kThreads, FM_WIN_CTAS)
 k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, int W, int BP, int rounds) {
   __shared__ double smem[8 * (kThreads / 32)];
@@ -1286,8 +1289,8 @@ k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, i
 #pragma unroll 1
       for (int r = Y0 + (int)threadIdx.x / kWinRowThreads; r < Y0 + kWinTH; r += kWinRowsPerPass)
         if (r < H && c0 < W)
-          distribute_pixels<4>(g, ad, da, da + N, fl, weights, gda + N, g_weights, wsens, adam, fuse_adam,
-                               pa.weight + r * W + c0, r * W + c0, r, c0, scatter, kacc);
+          distribute_pixels<4, KGRAD>(g, ad, da, da + N, fl, weights, gda + N, g_weights, wsens, adam, fuse_adam,
+                                      pa.weight + r * W + c0, r * W + c0, r, c0, scatter, kacc);
       __syncthreads();
       const float inv_s = s_fix[1];
       for (int k = threadIdx.x; k < kWinH * (kWinPitch / 4); k += kThreads) {
@@ -1304,7 +1307,7 @@ k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, i
       __syncthreads();  // the window is zero again before the next tile's taps
     }
     // kacc[0..3] -> frame a, kacc[4..7] -> frame b = a + 1: contiguous in k4acc
-    block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
+    if (KGRAD) block_accumulate<8>(kacc, k4acc + (size_t)pa.k4_frame_a * 4, smem);
     i += te - tb;
   }
   }
@@ -1822,6 +1825,8 @@ __device__ __forceinline__ float warp_sum_n(float* v, int lane) {
 // SHARED_K: every frame has the same intrinsics (one focal length, or constants), so only the SUM
 // over frames of the intrinsics gradient matters: the target-frame terms are then added to the
 // thread's own (source-frame) accumulators and only the 6 pose values go through the reduction.
+// KGRAD = false: constant intrinsics (the fused step's ground-truth K), no intrinsics terms at all; the 6
+// pose values go through the reduction and the K slots of the per-frame accumulators stay untouched.
 constexpr int kTrackThreads = 128;
 #ifndef FM_TRACK_PPT
 #define FM_TRACK_PPT 2  // source points per lane (1 or 2); 2 measured faster on H100
@@ -1845,20 +1850,22 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
 
 // The tracking kernels' view of the videos: which loss sum / valid count pair a segment's or a frame's terms
 // go to, and how d total / d tracking loss comes (Scale, as for the video layouts).
+// kPerFrameK: whether the layout serves a per-frame intrinsics GRADIENT (k_track_src<false, true, TL>); every
+// layout reads each frame's own k4 row.
 struct TrackOneVideo {  // one video, or the standalone op: the one pair at sums[0], sums[1]
   static constexpr bool kPerFrameK = true;  // per-frame intrinsics as well as one shared focal length
   using Scale = Uniform::Scale;
   template <class T> __device__ __forceinline__ T* sums_of(T* sums, int) const { return sums; }
 };
 struct TrackVideos {  // videos packed along the frame axis: frame f's video b has the pair sums[2 b], sums[2 b + 1]
-  static constexpr bool kPerFrameK = false;  // one focal length per video
+  static constexpr bool kPerFrameK = false;  // one focal length per video, or constant intrinsics
   using Scale = Videos::Scale;
   const int* frame_video;
   template <class T>
   __device__ __forceinline__ T* sums_of(T* sums, int f) const { return sums + 2 * __ldg(frame_video + f); }
 };
 
-template <bool SHARED_K, class TL>
+template <bool SHARED_K, bool KGRAD, class TL>
 __global__ void __launch_bounds__(kTrackThreads, FM_TRACK_BPS)
 k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const float* __restrict__ ext,
             const int* __restrict__ seg, const float* __restrict__ txy, const unsigned char* __restrict__ tvis,
@@ -1871,7 +1878,7 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
   __shared__ int s_item[2];
   float* sm = reinterpret_cast<float*>(sm4);
   constexpr int NW = kTrackThreads / 32;
-  constexpr int NRED = SHARED_K ? 6 : kTrackAcc;
+  constexpr int NRED = (SHARED_K || !KGRAD) ? 6 : kTrackAcc;
   constexpr int SLOT0 = kTrackAcc - NRED;  // twist values live in slots 4..9 either way
   float* s_tgt = sm + (size_t)max_rows * kTrackRec;  // [warp][target row][kTrackAcc]
   int* s_list = reinterpret_cast<int*>(s_tgt + (size_t)NW * max_rows * kTrackAcc);
@@ -2016,18 +2023,20 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
               const float g2 = fm_fma(r.R[6], d0, fm_fma(r.R[7], d1, __fmul_rn(r.R[8], d2)));
               G[j][0] = __fadd_rn(G[j][0], g0); G[j][1] = __fadd_rn(G[j][1], g1); G[j][2] = __fadd_rn(G[j][2], g2);
               // target-frame K gradient: duv = d (P_z + eps) / f and uv - c = f P / (P_z + eps)
-              const float ex = __fmul_rn(d0, r.k.ifx), ey = __fmul_rn(d1, r.k.ify);
-              if (SHARED_K) {  // straight into the thread's own intrinsics sums
-                acc[0] = fm_fma(ex, lt.P0, acc[0]); acc[1] = fm_fma(ey, lt.P1, acc[1]);
-                acc[2] = fm_fma(ex, lt.P2, acc[2]); acc[3] = fm_fma(ey, lt.P2, acc[3]);
-              } else {
-                c[0] = __fadd_rn(c[0], __fmul_rn(ex, lt.P0)); c[1] = __fadd_rn(c[1], __fmul_rn(ey, lt.P1));
-                c[2] = __fadd_rn(c[2], __fmul_rn(ex, lt.P2)); c[3] = __fadd_rn(c[3], __fmul_rn(ey, lt.P2));
+              if (KGRAD) {
+                const float ex = __fmul_rn(d0, r.k.ifx), ey = __fmul_rn(d1, r.k.ify);
+                if (SHARED_K) {  // straight into the thread's own intrinsics sums
+                  acc[0] = fm_fma(ex, lt.P0, acc[0]); acc[1] = fm_fma(ey, lt.P1, acc[1]);
+                  acc[2] = fm_fma(ex, lt.P2, acc[2]); acc[3] = fm_fma(ey, lt.P2, acc[3]);
+                } else {
+                  c[0] = __fadd_rn(c[0], __fmul_rn(ex, lt.P0)); c[1] = __fadd_rn(c[1], __fmul_rn(ey, lt.P1));
+                  c[2] = __fadd_rn(c[2], __fmul_rn(ex, lt.P2)); c[3] = __fadd_rn(c[3], __fmul_rn(ey, lt.P2));
+                }
               }
               // twist of the target pose: (Xw - t) x g, -g (an invalid point has g = 0)
               const float e0 = __fsub_rn(Xw[j][0], r.t[0]), e1 = __fsub_rn(Xw[j][1], r.t[1]);
               const float e2 = __fsub_rn(Xw[j][2], r.t[2]);
-              float* tw = c + (SHARED_K ? 0 : 4);
+              float* tw = c + (NRED - 6);
               tw[0] = __fadd_rn(tw[0], fm_fma(e2, g1, -__fmul_rn(e1, g2)));
               tw[1] = __fadd_rn(tw[1], fm_fma(e0, g2, -__fmul_rn(e2, g0)));
               tw[2] = __fadd_rn(tw[2], fm_fma(e1, g0, -__fmul_rn(e0, g1)));
@@ -2055,8 +2064,10 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
           const float dq1 = fm_fma(rs.R[1], G0, fm_fma(rs.R[4], G1, rs.R[7] * G2));
           const float dq2 = fm_fma(rs.R[2], G0, fm_fma(rs.R[5], G1, rs.R[8] * G2));
           dq_out[sidx * 3 + 0] = dq0; dq_out[sidx * 3 + 1] = dq1; dq_out[sidx * 3 + 2] = dq2;
-          const float e0 = dq0 * rs.k.ifx, e1 = dq1 * rs.k.ify;
-          acc[0] -= e0 * q[0]; acc[1] -= e1 * q[1]; acc[2] -= e0 * q[2]; acc[3] -= e1 * q[2];
+          if (KGRAD) {  // the resampled point q only feeds the source-frame K terms
+            const float e0 = dq0 * rs.k.ifx, e1 = dq1 * rs.k.ify;
+            acc[0] -= e0 * q[0]; acc[1] -= e1 * q[1]; acc[2] -= e0 * q[2]; acc[3] -= e1 * q[2];
+          }
           const float c0 = Xw[j][0] - rs.t[0], c1 = Xw[j][1] - rs.t[1], c2 = Xw[j][2] - rs.t[2];
           acc[4] += c1 * G2 - c2 * G1;
           acc[5] += c2 * G0 - c0 * G2;
@@ -2067,11 +2078,12 @@ k_track_src(const float* __restrict__ depth, const float* __restrict__ k4, const
       __syncthreads();  // s_list / s_wbase are rewritten by the next round
     }
     block_accumulate<2, kTrackThreads>(lc, tl.sums_of(sums, si.start_frame), red);
-    block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
+    if (KGRAD) block_accumulate<kTrackAcc, kTrackThreads>(acc, trackacc + (size_t)frame * kTrackAcc, red);
+    else block_accumulate<6, kTrackThreads>(acc + 4, trackacc + (size_t)frame * kTrackAcc + 4, red);
     // fold the warps' target-side slices into the per-frame accumulators (block_accumulate ended
     // with a barrier, so every slice is complete)
     for (int i = threadIdx.x; i < si.rows * kTrackAcc; i += kTrackThreads) {
-      if (SHARED_K && i % kTrackAcc < 4) continue;  // those slots are not written in this mode
+      if (NRED == 6 && i % kTrackAcc < 4) continue;  // those slots are not written in this mode
       double t = 0.0;
 #pragma unroll
       for (int w = 0; w < NW; ++w) t += (double)s_tgt[(size_t)w * si.rows * kTrackAcc + i];
@@ -2125,8 +2137,8 @@ k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const f
   red_add(gd + t.y1 * W + t.x1, t.w11 * (dq0 * rx1 + dq1 * ry1 + dq2));
 }
 
-// Frame f scaled by the sums of its video.
-template <class TL>
+// Frame f scaled by the sums of its video.  KGRAD = false (constant intrinsics): no g_k4.
+template <class TL, bool KGRAD>
 __global__ void k_track_finalize(const double* __restrict__ trackacc, const double* __restrict__ sums,
                                  float loss_weight, typename TL::Scale go, const float* __restrict__ ext,
                                  float* __restrict__ g_ext, float* __restrict__ g_k4, int F, TL tl) {
@@ -2134,7 +2146,8 @@ __global__ void k_track_finalize(const double* __restrict__ trackacc, const doub
   if (f >= F) return;
   const double sc = track_scale(tl.sums_of(sums, f), loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
-  for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
+  if (KGRAD)
+    for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
   const float* P = ext + (size_t)f * 16;
   const double w0 = 0.5 * sc * a[4], w1 = 0.5 * sc * a[5], w2 = 0.5 * sc * a[6];
   float* o = g_ext + (size_t)f * 16;
@@ -2952,18 +2965,21 @@ int procrustes_fwd(const float* depth, const float* k4, const float* backward_fl
 
 // The Procrustes backward in the layout of procrustes_fwd: d loss / d (depth, weights, K) from the pose
 // gradient g_rt and (include_flow_loss) the flow loss's, scaled by flow_scale.  The direct depth gradient
-// already in g_depth is scaled here too unless the caller did (depth_prescaled).
+// already in g_depth is scaled here too unless the caller did (depth_prescaled).  g_k4 == NULL: constant
+// intrinsics, no K gradient (the K-free phase D2 kernels, no k4acc, no k_k4_finalize); only the fused step
+// passes it.
 template <class Lay>
 int procrustes_bwd(const float* depth, const float* k4, const float* backward_flow, const float* weights, float wsens,
                    const int64_t* indices, int num_indices, const float* g_rt, int include_flow_loss,
                    const float* flow_scale, float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int T,
                    const Lay& lay, int H, int W, cudaStream_t s, const AdamFuse* adam, bool depth_prescaled) {
-  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || T < 2 * B || bad_dims(B, 2, H, W))
+  if (!depth || !k4 || !backward_flow || !g_depth || !ws || T < 2 * B || bad_dims(B, 2, H, W))
     return fail_msg("fm_procrustes_bwd: bad arguments");
   if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
   const int BP = T - B;
   Workspace w = carve_rows(ws, B, T, BP);
-  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)T * 4 * sizeof(double), s);
+  const bool kgrad = g_k4 != nullptr;
+  cudaError_t e = kgrad ? cudaMemsetAsync(w.k4acc, 0, (size_t)T * 4 * sizeof(double), s) : cudaSuccess;
   if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
   AdamFuse af;
   if (adam) af = *adam; else memset(&af, 0, sizeof(af));
@@ -2978,18 +2994,22 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
   if (indices) {
     dim3 grid(blocks_for_points(num_indices), BP);
-    k_distribute<1><<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
+    auto kern = kgrad ? k_distribute<1, true, Lay> : k_distribute<1, false, Lay>;
+    kern<<<grid, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, indices, num_indices, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W);
   } else if (W % 4 == 0) {
     const long long items = (long long)BP * ((W + kWinTW - 1) / kWinTW) * ((H + kWinTH - 1) / kWinTH);
     const int pg = persistent_grid(FM_WIN_CTAS, items);
     const long long chunks = items * (kWinTW * kWinTH) / (kThreads * 4);  // rounds are sized in 1024-pixel chunks
-    k_distribute_window<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
+    auto kern = kgrad ? k_distribute_window<true, Lay> : k_distribute_window<false, Lay>;
+    kern<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, chunks, pg, false));
   } else {
     const long long items = (long long)BP * ((H * W + kThreads - 1) / kThreads);
     const int pg = persistent_grid(3, items);
-    k_distribute_dense<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
+    auto kern = kgrad ? k_distribute_dense<true, Lay> : k_distribute_dense<false, Lay>;
+    kern<<<pg, kThreads, 0, s>>>(depth, k4, backward_flow, weights_rw, w.adj, g_depth, g_weights, w.k4acc, wsens, lay, af, H, W, BP, procrustes_rounds(H, W, items / 4, pg, false));
   }
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
+  if (!kgrad) return 0;
   k_k4_finalize<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, T,
                                                 frames_of(lay));
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
@@ -3026,6 +3046,7 @@ int procrustes_bwd_planned(const float* depth, const float* k4, const float* bac
                            int H, int W, cudaStream_t s, const AdamFuse* adam) {
   if (!tiled_shape_ok(F, H, W))
     return fail_msg("fm_procrustes_bwd: the splat plan serves the dense single-video path with W % 4 == 0");
+  if (!g_k4) return fail_msg("fm_procrustes_bwd: the splat plan always computes the intrinsics gradient (g_k4)");
   if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || bad_dims(1, F, H, W))
     return fail_msg("fm_procrustes_bwd: bad arguments");
   if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
@@ -3131,9 +3152,9 @@ int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensit
   AdamFuse af;
   memset(&af, 0, sizeof(af));
   dim3 grid1(blocks_for_points(num_indices), B);
-  k_distribute<1><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights), indices,
-                                            num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
-                                            weight_sensitivity, lay1, af, H, W);
+  k_distribute<1, true><<<grid1, kThreads, 0, s>>>(depth, base_k4, backward_flow, const_cast<float*>(weights),
+                                                  indices, num_indices, w.adj + items, g_depth, g_weights, w.k4acc,
+                                                  weight_sensitivity, lay1, af, H, W);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_distribute");
   return 0;
 }
@@ -3213,6 +3234,7 @@ int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward
                       const float* g_rt, int include_flow_loss, const float* flow_scale,
                       float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int F, int H,
                       int W, void* stream) {
+  if (!g_k4) return fail_msg("fm_procrustes_bwd: bad arguments");
   return procrustes_bwd(depth, k4, backward_flow, weights, 0.f, indices, num_indices, g_rt, include_flow_loss,
                         flow_scale, g_depth, g_weights, g_k4, ws, B, B * F, dense_layout(F, H, W), H, W,
                         (cudaStream_t)stream, nullptr, /*depth_prescaled=*/false);
@@ -3483,7 +3505,7 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
                           const unsigned char* track_vis, long long total_samples, int mapping, float delta,
                           float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
                           int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream, double* sums,
-                          int B, const TL& tl) {
+                          int B, const TL& tl, bool k_grad) {
   if (!depth || !k4 || !extrinsics || !segments || !track_xy || !track_vis || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_fwd: bad arguments");
@@ -3507,9 +3529,10 @@ static int track_fwd_impl(const float* depth, const float* k4, const float* extr
   if (per_sm > FM_TRACK_BPS) per_sm = FM_TRACK_BPS;
   if (per_sm < 1) per_sm = 1;
   const int grid = persistent_grid(per_sm, items);
-  auto src = k_track_src<true, TL>;
+  // k_grad = false (constant intrinsics, the fused step only) implies shared_intrinsics
+  auto src = k_grad ? k_track_src<true, true, TL> : k_track_src<true, false, TL>;
   if constexpr (TL::kPerFrameK) {
-    if (!shared_intrinsics) src = k_track_src<false, TL>;
+    if (!shared_intrinsics) src = k_track_src<false, true, TL>;
   } else if (!shared_intrinsics) {
     return fail_msg("fm_track_loss_fwd: packed videos have one focal length each");
   }
@@ -3537,7 +3560,7 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
                               int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream) {
   return track_fwd_impl(depth, k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, track_vis,
                         total_samples, mapping, delta, loss_weight, loss, ws, F, H, W, depth_frame0, src_frame_lo,
-                        src_frame_hi, shared_intrinsics, stream, (double*)ws, 1, TrackOneVideo{});
+                        src_frame_hi, shared_intrinsics, stream, (double*)ws, 1, TrackOneVideo{}, true);
 }
 
 int fm_track_loss_fwd(const float* depth, const float* k4, const float* extrinsics, const int* segments,
@@ -3560,7 +3583,7 @@ int fm_track_loss_value(const void* ws, float loss_weight, float* loss, void* st
 extern "C++" {
 // The depth scatter of the tracking loss (k_track_apply, REDs into g_depth) and the pose / intrinsics
 // gradients (k_track_finalize) are independent: `apply_stream` may differ from `s`.  `sums` and `tl` as in
-// track_fwd_impl.
+// track_fwd_impl.  g_k4 == NULL: constant intrinsics, no intrinsics gradient (the fused step only).
 template <class TL>
 static int track_bwd_impl(const float* k4, const float* extrinsics, const int* segments, int num_segments,
                           int max_rows, int max_points, const float* track_xy, long long total_samples,
@@ -3568,7 +3591,7 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
                           float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
                           int src_frame_hi, cudaStream_t s, cudaStream_t apply_stream, const double* sums,
                           const TL& tl) {
-  if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !g_k4 || !ws ||
+  if (!k4 || !extrinsics || !segments || !track_xy || !g_depth || !g_extrinsics || !ws ||
       num_segments < 1 || max_rows < 1 || max_points < 1 || F < 1)
     return fail_msg("fm_track_loss_bwd: bad arguments");
   if (depth_frame0 < 0 || src_frame_lo < depth_frame0 || src_frame_hi > F || src_frame_lo > src_frame_hi)
@@ -3579,8 +3602,8 @@ static int track_bwd_impl(const float* k4, const float* extrinsics, const int* s
   k_track_apply<TL><<<grid, kThreads, 0, apply_stream>>>(k4, segments, track_xy, w.flag, w.dq, sums, loss_weight,
                                                         grad_out, g_depth, H, W, sh, tl);
   FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_apply");
-  k_track_finalize<TL><<<(F + 63) / 64, 64, 0, s>>>(w.acc, sums, loss_weight, grad_out, extrinsics, g_extrinsics,
-                                                   g_k4, F, tl);
+  auto fin = g_k4 ? k_track_finalize<TL, true> : k_track_finalize<TL, false>;
+  fin<<<(F + 63) / 64, 64, 0, s>>>(w.acc, sums, loss_weight, grad_out, extrinsics, g_extrinsics, g_k4, F, tl);
   FM_CHECK_LAUNCH("fm_track_loss_bwd: k_track_finalize");
   return 0;
 }
@@ -3594,6 +3617,7 @@ int fm_track_loss_bwd_sharded(const float* depth, const float* k4, const float* 
                               float* g_k4, void* ws, int F, int H, int W, int depth_frame0, int src_frame_lo,
                               int src_frame_hi, void* stream) {
   (void)depth; (void)track_vis; (void)mapping; (void)delta;
+  if (!g_k4) return fail_msg("fm_track_loss_bwd: bad arguments");
   return track_bwd_impl(k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, total_samples,
                         loss_weight, grad_out, g_depth, g_extrinsics, g_k4, ws, F, H, W, depth_frame0,
                         src_frame_lo, src_frame_hi, (cudaStream_t)stream, (cudaStream_t)stream, (const double*)ws,
@@ -3812,6 +3836,11 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
   // the splat plan of this video's backward flows serves the dense path (all-pixel Procrustes)
   void* plan = (a->splat_plan && !a->indices && tiled_shape_ok(T, H, W)) ? a->splat_plan : nullptr;
+  // g_k4 == NULL: constant intrinsics (ground truth), the backward computes no intrinsics gradient
+  const bool kgrad = a->g_k4 != nullptr;
+  if (!kgrad && (a->focal || a->track_g_k4))
+    return fail_msg("fm_overfit_step: g_k4 == NULL (constant intrinsics) needs focal == NULL and track_g_k4 == NULL");
+  if (!kgrad && plan) return fail_msg("fm_overfit_step: the splat plan does not serve constant intrinsics (g_k4 == NULL)");
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
@@ -3853,7 +3882,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       if ((rc = track_fwd_impl(a->depth, k4, a->extrinsics, t->segments, t->num_segments, t->max_rows,
                                t->max_points, t->xy, t->vis, t->total_samples, a->mapping, a->delta,
                                a->track_weight, a->track_loss, a->track_ws, T, H, W, 0, 0, T, 1, ts,
-                               step_track_sums(lay, w, a->track_ws), B, track_layout(lay))))
+                               step_track_sums(lay, w, a->track_ws), B, track_layout(lay), kgrad)))
         return rc;
       if (fwd_lane) {
         if ((e = cudaEventRecord(fwd_lane->join, fwd_lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);

@@ -490,9 +490,10 @@ FM_HD void lean_to_standard(const T* lean, const float* rtF, const float* rtB, d
 // ---------------------------------------------------------------------------------
 // Phase D2: per-point adjoints of the Procrustes inputs.  `scatter(row, x0, v0, v1)` adds
 // v0 / v1 into the earlier frame's depth gradient at columns x0 / x0 + 1 of a row; returns the aligned later-frame depth gradient and
-// the weight gradient.  kacc[0..3] += dK_a (through q), kacc[4..7] += dK_b (through p).
+// the weight gradient.  kacc[0..3] += dK_a (through q), kacc[4..7] += dK_b (through p); KGRAD = false
+// (constant intrinsics) leaves kacc alone.
 // ---------------------------------------------------------------------------------
-template <typename LoadA, typename Scatter>
+template <bool KGRAD = true, typename LoadA, typename Scatter>
 FM_HD void distribute_point(const PairGeom& g, const PairAdjoint& ad, float x, float y, float db,
                             float w, float flx, float fly, LoadA load_a, Scatter scatter,
                             float& g_db, float& g_w, float* kacc) {
@@ -507,11 +508,13 @@ FM_HD void distribute_point(const PairGeom& g, const PairAdjoint& ad, float x, f
   float rx, ry;
   ray_of(x, y, g.kb, rx, ry);
   g_db = pb[0] * rx + pb[1] * ry + pb[2];
-  const float eb0 = pb[0] * g.kb.ifx, eb1 = pb[1] * g.kb.ify;
-  kacc[4] -= eb0 * p[0];
-  kacc[5] -= eb1 * p[1];
-  kacc[6] -= eb0 * db;
-  kacc[7] -= eb1 * db;
+  if (KGRAD) {
+    const float eb0 = pb[0] * g.kb.ifx, eb1 = pb[1] * g.kb.ify;
+    kacc[4] -= eb0 * p[0];
+    kacc[5] -= eb1 * p[1];
+    kacc[6] -= eb0 * db;
+    kacc[7] -= eb1 * db;
+  }
   // q = sum_n w_n D_n (rx_n, ry_n, 1): scatter into the four taps of the earlier frame
   float rx0, ry0, rx1, ry1;
   tap_rays(t, g.grid, g.ka, rx0, ry0, rx1, ry1);
@@ -522,12 +525,14 @@ FM_HD void distribute_point(const PairGeom& g, const PairAdjoint& ad, float x, f
   // one call per tap row: (row y, x0, value at x0, value at x0 + 1); a clamped x1 has weight 0
   scatter(t.y0, t.x0, t.w00 * b00, t.w01 * b01);
   scatter(t.y1, t.x0, t.w10 * b10, t.w11 * b11);
-  const float qz_true = q[2] + g.z0;
-  const float ea0 = qb[0] * g.ka.ifx, ea1 = qb[1] * g.ka.ify;
-  kacc[0] -= ea0 * q[0];
-  kacc[1] -= ea1 * q[1];
-  kacc[2] -= ea0 * qz_true;
-  kacc[3] -= ea1 * qz_true;
+  if (KGRAD) {
+    const float qz_true = q[2] + g.z0;
+    const float ea0 = qb[0] * g.ka.ifx, ea1 = qb[1] * g.ka.ify;
+    kacc[0] -= ea0 * q[0];
+    kacc[1] -= ea1 * q[1];
+    kacc[2] -= ea0 * qz_true;
+    kacc[3] -= ea1 * qz_true;
+  }
 }
 
 // Order of magnitude of the largest tap value distribute_point scatters for a pair, from its

@@ -13,8 +13,9 @@ from torch import Tensor
 from . import ops
 from .loss import (LossFlowCfg, LossTrackingCfg, MappingHuberCfg, MappingL1Cfg, MappingL2Cfg,
                    get_losses)
-from .model import (BackboneExplicitDepth, BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsRegressedCfg,
-                    IntrinsicsSoftminCfg, Model, ModelCfg, RegressionCfg)
+from .model import (BackboneExplicitDepth, BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsGroundTruth,
+                    IntrinsicsGroundTruthCfg, IntrinsicsRegressedCfg, IntrinsicsSoftminCfg, Model, ModelCfg,
+                    RegressionCfg)
 from .types import Batch, Flows
 
 
@@ -52,6 +53,8 @@ def _mapping_cfg(name: str, delta: float):
 def build_model_and_losses(cfg: OverfitCfg, num_frames: int, image_shape):
     if cfg.intrinsics == "regressed":
         icfg = IntrinsicsRegressedCfg("regressed", cfg.initial_focal)
+    elif cfg.intrinsics == "ground_truth":  # intrinsics_ground_truth.py: K comes with the batch
+        icfg = IntrinsicsGroundTruthCfg("ground_truth")
     else:
         reg = None if cfg.regression_after is None else RegressionCfg(cfg.regression_after,
                                                                       cfg.regression_window)
@@ -185,11 +188,20 @@ class FusedOverfitter(Overfitter):
     Bound to a Model whose backbone is a network (any backbone but BackboneExplicitDepth, the drop-in
     surface of flowmap_b200.fused), the optimiser owns no depth or weight buffers and no Adam state for
     them: every step's depths and weights come from the network, through forward_phase, and only the
-    split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight)."""
+    split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight).
+
+    cfg.intrinsics "ground_truth" (intrinsics_ground_truth.py, calibrated data) takes K as given: from
+    `batch.intrinsics` (1, F, 3, 3), (B, F, 3, 3) for a tensor batch, or each Batch's own for a list, normalised
+    as in the reference and possibly different for every frame.  There is no focal parameter and the step
+    computes no intrinsics gradient (fm_overfit_step with focal = g_k4 = track_g_k4 = NULL); set_intrinsics
+    swaps K in place.  The splat plan and pair sharding do not serve it."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
                  use_splat_plan: bool = False, model=None):
         self._layout, self._tensor_batch, self._network = None, False, False
+        self._gt = cfg.intrinsics == "ground_truth"
+        if self._gt and use_splat_plan:
+            raise ValueError("flowmap_b200: the splat plan does not serve ground-truth intrinsics")
         if isinstance(batch, (list, tuple)):
             self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
         elif batch.videos.shape[0] > 1:
@@ -210,11 +222,17 @@ class FusedOverfitter(Overfitter):
         else:
             self._init_one(cfg, batch, flows, tracks, device, use_splat_plan, model)
         self._init_step(cfg)
+        if self._gt:
+            self.set_intrinsics(self.batch.intrinsics if self._layout is None or self._tensor_batch
+                                else [bt.intrinsics for bt in self.batches])
         if self._tensor_batch:  # the parameters as (B, F, ...) / (B, F-1, ...) views of the packed buffers
             self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
 
     def _init_one(self, cfg, batch, flows, tracks, device, use_splat_plan, model):
         """The one-video optimiser: its parameters are the Model's own tensors."""
+        if model is not None and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
+            raise ValueError(f"flowmap_b200: the bound model's intrinsics ({type(model.intrinsics).__name__}) do not "
+                             f"match cfg.intrinsics = {cfg.intrinsics!r}")
         super().__init__(cfg, batch, flows, tracks, device, model=model)
         _, f, _, h, w = batch.videos.shape
         # the kernels read raw pointers: canonical (contiguous float32) copies, kept alive here
@@ -232,7 +250,9 @@ class FusedOverfitter(Overfitter):
         else:  # a network backbone: the step's depths / weights arrive with forward_phase
             self._network, self._depth, self._wlog = True, None, None
         intr = self.model.intrinsics
-        if cfg.intrinsics != "softmin":
+        if self._gt:
+            self._focal = None
+        elif cfg.intrinsics != "softmin":
             self._focal = intr.focal_length.data
         elif cfg.regression_after is not None:
             self._focal = intr.intrinsics_regressed.focal_length.data
@@ -306,7 +326,9 @@ class FusedOverfitter(Overfitter):
             return buf
         self._depth = pack([m.backbone.depth for m in self.models])
         self._wlog = pack([m.backbone.weights for m in self.models])
-        if cfg.intrinsics != "softmin":
+        if self._gt:
+            self._focal = None
+        elif cfg.intrinsics != "softmin":
             self._focal = stack([m.intrinsics.focal_length for m in self.models])
         elif cfg.regression_after is not None:
             self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
@@ -342,8 +364,9 @@ class FusedOverfitter(Overfitter):
             self._g_depth, self._g_w = torch.empty(T, h, w, device=dev), torch.empty(T - B, h, w, device=dev)
         else:
             self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
-        self._g_focal = torch.zeros_like(self._focal)
-        self._k4, self._g_k4 = torch.empty(T, 4, device=dev), torch.empty(T, 4, device=dev)
+        # ground-truth K: no focal parameter, and no intrinsics gradient buffers (the constant-intrinsics step)
+        self._g_focal = z(self._focal)
+        self._k4, self._g_k4 = torch.empty(T, 4, device=dev), None if self._gt else torch.empty(T, 4, device=dev)
         self.rt = torch.empty(*pair_dims, 3, 4, device=dev)
         self._loss = torch.zeros(video_dims, device=dev)
         self._track_loss = torch.zeros_like(self._loss)
@@ -383,7 +406,7 @@ class FusedOverfitter(Overfitter):
             self._ext = torch.empty(*frame_dims, 4, 4, device=dev)
             self._g_ext = torch.empty(*frame_dims, 4, 4, device=dev)
             self._g_rt = torch.empty(*pair_dims, 3, 4, device=dev)
-            self._tg_k4 = torch.empty(T, 4, device=dev)
+            self._tg_k4 = None if self._gt else torch.empty(T, 4, device=dev)
             self._tws = torch.empty(lib().fm_track_workspace_bytes(T, pk.total), dtype=torch.uint8, device=dev)
             a.track_weight = cfg.tracking_weight
             a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
@@ -637,7 +660,7 @@ class FusedOverfitter(Overfitter):
             else:
                 if self._softmin and global_step == c.regression_after and training:
                     self._focal.copy_(torch.stack(self._window()).mean())
-                a.focal = self._focal.data_ptr()
+                a.focal = None if self._focal is None else self._focal.data_ptr()
             a.phase = 1  # FM_STEP_FORWARD
             try:
                 check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (forward)")
@@ -722,7 +745,7 @@ class FusedOverfitter(Overfitter):
         from ._lib import check
         c, a = self.cfg, self._args
         if update:
-            self._clock.tick(tick_focal=not sweep)
+            self._clock.tick(tick_focal=not sweep and not self._gt)
         a.tracks = self._ctypes.pointer(self._pk_c) if track_on else None
         a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
         # the metrics row is indexed by the step clock, which only update steps advance
@@ -731,7 +754,7 @@ class FusedOverfitter(Overfitter):
             if sweep:
                 self._step_softmin(update)
             else:
-                a.focal = self._focal.data_ptr()
+                a.focal = None if self._focal is None else self._focal.data_ptr()
                 a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
                 with torch.cuda.device(self.rt.device):
                     self._call_step()
@@ -786,13 +809,14 @@ class FusedOverfitter(Overfitter):
         key = (track_on, sweep, self.global_step >= c.flow_enable_after)
         graphable = (update and self.use_cuda_graph and not c.procrustes_randomize and not window_on and
                      getattr(self, "injected_indices", None) is None)
-        self._run_body(key, graphable, lambda upd=update: self._step_body(upd, track_on, sweep), not sweep)
+        ticks_focal = not sweep and not self._gt
+        self._run_body(key, graphable, lambda upd=update: self._step_body(upd, track_on, sweep), ticks_focal)
         if update:
             if window_on:
                 self.window.append(self._window_entry())
             self.global_step += 1
             self.optimizer_steps += 1
-            self.focal_steps += int(not sweep)
+            self.focal_steps += int(ticks_focal)
         if self._layout is not None:
             return self._total.clone(), self._per_video(self.rt, pairs=True)
         return self._total.clone(), self.rt
@@ -805,10 +829,47 @@ class FusedOverfitter(Overfitter):
         return [ops.pose_chain(r[None])[0] for r in self._per_video(self.rt, pairs=True)]
 
     def gradients(self):
+        """d loss / d depth, weights and focal length of the last step; "focal" is None with ground-truth K."""
         if self._layout is None:
             return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
+        g_focal = self._g_focal
+        if g_focal is not None and not self._tensor_batch:
+            g_focal = list(g_focal.unbind())
         return {"depth": self._per_video(self._g_depth), "weights": self._per_video(self._g_w, pairs=True),
-                "focal": self._g_focal if self._tensor_batch else list(self._g_focal.unbind())}
+                "focal": g_focal}
+
+    def set_intrinsics(self, intrinsics):
+        """Ground-truth intrinsics for the following steps, copied into the step's k4 buffer (captured CUDA
+        graphs stay valid): (1, F, 3, 3) for one video, (B, F, 3, 3) for a tensor batch, a list of the videos'
+        (1, F_b, 3, 3) for a list of Batches; normalised as in the reference.  ValueError on a missing, wrongly
+        shaped or non-finite K."""
+        if not self._gt:
+            raise ValueError("flowmap_b200: set_intrinsics needs cfg.intrinsics = 'ground_truth'")
+        if intrinsics is None:
+            raise ValueError("flowmap_b200: ground-truth intrinsics need batch.intrinsics")
+        if isinstance(intrinsics, (list, tuple)):
+            if self._layout is None or self._tensor_batch:
+                raise ValueError("flowmap_b200: one intrinsics tensor for this optimiser, not a list")
+            per = list(intrinsics)
+        else:
+            if self._layout is not None and not self._tensor_batch:
+                raise ValueError(f"flowmap_b200: videos of different lengths need a list of {self.B} intrinsics")
+            if intrinsics.dim() != 4:
+                raise ValueError(f"flowmap_b200: intrinsics must be (B, F, 3, 3), got {tuple(intrinsics.shape)}")
+            per = [intrinsics[i:i + 1] for i in range(intrinsics.shape[0])]
+        if len(per) != self.B:
+            raise ValueError(f"flowmap_b200: intrinsics for {len(per)} videos, the optimiser holds {self.B}")
+        rows = []
+        for i, (k, f) in enumerate(zip(per, self.frames)):
+            if k is None:
+                raise ValueError(f"flowmap_b200: video {i} carries no intrinsics (batch.intrinsics)")
+            if tuple(k.shape) != (1, f, 3, 3):
+                raise ValueError(f"flowmap_b200: the intrinsics of video {i} must be (1, {f}, 3, 3), got "
+                                 f"{tuple(k.shape)}")
+            if not bool(torch.isfinite(k).all()):
+                raise ValueError(f"flowmap_b200: the intrinsics of video {i} are not finite")
+            rows.append(ops.intrinsics_to_k4(k[0].to(device=self._k4.device, dtype=torch.float32)))
+        self._k4.copy_(torch.cat(rows))
 
     def intrinsics_k4(self) -> Tensor:
         """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for a (B, F) tensor batch; a list of
@@ -904,6 +965,8 @@ class ShardedFusedOverfitter(FusedOverfitter):
         from ._lib import lib
         if isinstance(batch, (list, tuple)) or batch.videos.shape[0] != 1:
             raise ValueError("flowmap_b200: pair sharding optimises one video (batch size 1)")
+        if cfg.intrinsics == "ground_truth":
+            raise ValueError("flowmap_b200: pair sharding does not serve ground-truth intrinsics")
         super().__init__(replace(cfg, use_tracking=False), batch, flows, None, device)
         self.cfg = cfg
         self.plan, self.group = plan, group

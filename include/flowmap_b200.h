@@ -295,7 +295,11 @@ typedef struct {
  * The correspondence weights are sigmoid(weight_sensitivity * weight_logits)
  * (backbone_explicit_depth.py:40), evaluated inside the kernels; weight_logits == NULL means
  * use_correspondence_weights = false (model.py:67-68).  focal == NULL keeps k4 as given
- * (no intrinsics gradient).  step <= 0 computes loss and gradients but skips Adam.
+ * (no focal gradient).  focal == NULL together with g_k4 == NULL and track_g_k4 == NULL is the
+ * constant-intrinsics step (intrinsics_ground_truth.py: K given per frame, e.g. calibrated data): it
+ * computes no intrinsics gradient at all -- the Procrustes backward and the tracking sweep run without
+ * their K accumulators -- and needs no splat plan; g_k4 == NULL with a focal parameter or a track_g_k4 is
+ * refused.  step <= 0 computes loss and gradients but skips Adam.
  * Gradients of the step are left in g_depth / g_weights / g_focal / g_k4. */
 typedef struct {
   int F, H, W;
