@@ -224,5 +224,43 @@ void emu_procrustes_bwd(const float* depth, const float* k4, const float* bflow,
     }
   }
 }
+
+// Phase D2 on every pixel through distribute_point<true> (kgrad 1) or <false> (kgrad 0, the constant-intrinsics
+// kernels): per point (pair * N + j) its g_db, its g_w and the two scatter calls in call order (row, x0, v0,
+// v1) -> taps[8 per point].  kacc starts at a sentinel for every point; kacc_moved counts the points whose kacc
+// changed.
+void emu_distribute(const float* depth, const float* k4, const float* bflow, const float* weights,
+                    const PairState* state, const double* g_rt, int kgrad, float* g_db, float* g_w, float* taps,
+                    long long* kacc_moved, int B, int F, int H, int W) {
+  const int N = H * W, BP = B * (F - 1);
+  const float sentinel = 0.3125f;
+  *kacc_moved = 0;
+  for (int pair = 0; pair < BP; ++pair) {
+    PairAdjoint ad;
+    procrustes_adjoint(state[pair], g_rt + (size_t)pair * 12, ad);
+    int a;
+    PairGeom g = geom(k4, pair, F, H, W, ad.shift[2], a);
+    const float* da = depth + (size_t)a * N; const float* db = da + N;
+    for (int j = 0; j < N; ++j) {
+      const size_t o = (size_t)pair * N + j;
+      float kacc[8];
+      for (int k = 0; k < 8; ++k) kacc[k] = sentinel;
+      float* tp = taps + o * 8;
+      int call = 0;
+      auto scatter = [tp, &call](int y0, int x0, float v0, float v1) {
+        float* t = tp + 4 * call++;
+        t[0] = (float)y0; t[1] = (float)x0; t[2] = v0; t[3] = v1;
+      };
+      auto load_a = [da](int q) { return da[q]; };
+      const float x = pix_coord(j % W, g.grid.Wf, g.grid.invW), y = pix_coord(j / W, g.grid.Hf, g.grid.invH);
+      const float w = weights ? weights[o] : 1.f, flx = bflow[o * 2], fly = bflow[o * 2 + 1];
+      if (kgrad) distribute_point<true>(g, ad, x, y, db[j], w, flx, fly, load_a, scatter, g_db[o], g_w[o], kacc);
+      else distribute_point<false>(g, ad, x, y, db[j], w, flx, fly, load_a, scatter, g_db[o], g_w[o], kacc);
+      bool moved = false;
+      for (int k = 0; k < 8; ++k) moved |= kacc[k] != sentinel;
+      *kacc_moved += moved;
+    }
+  }
+}
 }
 

@@ -285,3 +285,65 @@ def test_emulated_step_with_per_frame_intrinsics_vs_float64_oracle(emu, k4_cases
     errs = errors(dict(r, g_focal=None), refs[64])
     errs.update(k4_errors(r["g_k4"], refs[64][gk]))
     check(errs, noise, f"{kregime} {flows} {points} lean={lean}", loss_tol=1e-4, pose_tol=1e-5, floor=2e-5)
+
+
+def _distribute_both(emu, depth, wt, fl, k4):
+    """distribute_point<true> and <false> (the constant-intrinsics kernels' phase D2) on every pixel of one step's
+    pose gradient: {kgrad: (g_db, g_w, taps, points whose kacc moved)}."""
+    B, F_, H, W = depth.shape
+    BP, N = B * (F_ - 1), H * W
+    f32 = lambda t: np.ascontiguousarray(t.numpy(), dtype=np.float32)  # noqa: E731
+    d, w, k = f32(depth), f32(wt), f32(k4)
+    ff, fb, mf, mb = (f32(getattr(fl, n)) for n in ("forward", "backward", "forward_mask", "backward_mask"))
+    rt = np.zeros((BP, 12), dtype=np.float32)
+    state = np.zeros(BP * emu.emu_state_bytes(), dtype=np.uint8)
+    emu.emu_procrustes_fwd(_p(d), _p(k), _p(fb), _p(w), None, 0, _p(rt), _p(state), B, F_, H, W)
+    flowacc = np.zeros((B * F_, 40), dtype=np.float64)
+    mask_sum = float(mf.astype(np.float64).sum() + mb.astype(np.float64).sum())
+    emu.emu_flow(_p(d), _p(k), _p(rt), _p(ff), _p(fb), _p(mf), _p(mb), ctypes.c_double(mask_sum), 0,
+                 ctypes.c_float(0.01), ctypes.c_float(1000.0), _p(np.zeros_like(d)), _p(flowacc), B, F_, H, W)
+    g_rt = np.ascontiguousarray(flow_pose_grad(flowacc, rt, B, F_))
+    out = {}
+    for kgrad in (1, 0):
+        g_db, g_w = np.zeros(BP * N, np.float32), np.zeros(BP * N, np.float32)
+        taps = np.zeros(BP * N * 8, np.float32)
+        moved = np.zeros(1, np.int64)
+        emu.emu_distribute(_p(d), _p(k), _p(fb), _p(w), _p(state), _p(g_rt), kgrad, _p(g_db), _p(g_w), _p(taps),
+                           _p(moved), B, F_, H, W)
+        out[kgrad] = (g_db, g_w, taps, int(moved[0]))
+    return out
+
+
+DISTRIBUTE_CASES = ([("flows", kind, (1, 4, 40, 64)) for kind in ("iid", "shift", "leave", "outliers", "zoom", "scene")] +
+                    [("flows", kind, (1, 4, 38, 63)) for kind in ("iid", "shift", "leave", "outliers", "zoom", "scene")] +
+                    [(kregime, flows, (2, 4, 24, 32)) for kregime in ("offcentre", "zoom", "corner", "videos")
+                     for flows in ("shift", "scene")])
+
+
+@pytest.mark.parametrize("kregime,flows,shape", DISTRIBUTE_CASES,
+                         ids=[f"{k}-{fl}-{'x'.join(map(str, s))}" for k, fl, s in DISTRIBUTE_CASES])
+def test_constant_intrinsics_distribute_equals_k_carrying(emu, kregime, flows, shape):
+    """distribute_point<false> (k_distribute*<false>, the constant-intrinsics step's phase D2) against <true> on
+    the flow regimes (focal-length K) and the per-frame K regimes: the later frame's depth gradient, the weight
+    gradient and every scattered tap (row, column, both values) are bit-identical, and the K accumulators are
+    not touched (<true> moves them)."""
+    from oracle import flowmap_oracle as O
+    from flow_regime_checks import k4_regime, k4_scene
+    b, f, h, w = shape
+    if kregime == "flows":
+        depth, fl, focal, _ = O.flow_regime(flows, f, h, w, seed=3)
+        s = (h * w) ** 0.5
+        k4 = torch.tensor([focal * s / w, focal * s / h, 0.5, 0.5], dtype=torch.float64).expand(b, f, 4)
+    else:
+        k4 = k4_regime(kregime, b, f, h, w)
+        if flows == "scene":
+            depth, fl = k4_scene(k4, h, w, seed=11)
+        else:
+            depth, fl, _, _ = O.flow_regime(flows, f, h, w, seed=11, b=b)
+    wt = torch.sigmoid(100.0 * 0.01 * torch.randn(b, f - 1, h, w, generator=torch.Generator().manual_seed(4),
+                                                  dtype=torch.float64))
+    out = _distribute_both(emu, depth, wt, fl, k4.reshape(b * f, 4))
+    assert out[1][3] > 0 and out[0][3] == 0, (out[1][3], out[0][3])
+    for name, a, c in zip(("g_db", "g_w", "taps"), out[1][:3], out[0][:3]):
+        assert np.isfinite(a).all() and np.abs(a).max() > 0, name
+        assert np.array_equal(a.view(np.uint32), c.view(np.uint32)), (name, int((a != c).sum()))
