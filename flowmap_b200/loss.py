@@ -77,18 +77,10 @@ class LossFlow(Loss):
         super().__init__(cfg)
         self._mask_key = None
         self._mask_sum = None
-        self._mask_override = None
-
-    def set_global_mask_sum(self, total):
-        """Pair-sharded runs: the normaliser is the mask sum over ALL ranks' pairs
-        (flowmap_b200.parallel.global_mask_sum); None restores the local computation."""
-        self._mask_override = total
 
     def _mask_total(self, flows: Flows) -> Tensor:
         # The denominator depends on the (constant) masks only: recompute when the mask
         # tensors change identity or are written to.
-        if self._mask_override is not None:
-            return self._mask_override
         fm, bm = flows.forward_mask, flows.backward_mask
         key = self._mask_key
         hit = (key is not None and key[0]() is fm and key[1]() is bm and

@@ -16,6 +16,7 @@ from .loss import (LossFlowCfg, LossTrackingCfg, MappingHuberCfg, MappingL1Cfg, 
 from .model import (BackboneExplicitDepth, BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsGroundTruth,
                     IntrinsicsGroundTruthCfg, IntrinsicsRegressedCfg, IntrinsicsSoftminCfg, Model, ModelCfg,
                     RegressionCfg)
+from .ops import _ptr
 from .types import Batch, Flows
 
 
@@ -372,20 +373,20 @@ class FusedOverfitter(Overfitter):
         self._track_loss = torch.zeros_like(self._loss)
         self._indices = self.model.extrinsics.select_indices(h, w, dev) if not cfg.procrustes_randomize else None
         a = OverfitStepArgs()
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         a.F, a.H, a.W = T if self._layout is None else 0, h, w  # F: ignored by fm_overfit_step_videos
-        a.depth = P(self._depth)
-        a.weight_logits = P(self._wlog) if cfg.use_correspondence_weights else None
+        a.depth = _ptr(self._depth)
+        a.weight_logits = _ptr(self._wlog) if cfg.use_correspondence_weights else None
         a.weight_sensitivity = cfg.weight_sensitivity
-        a.focal, a.k4 = P(self._focal), P(self._k4)
-        a.fflow, a.bflow = P(self.flows.forward), P(self.flows.backward)
-        a.fmask, a.bmask = P(self.flows.forward_mask), P(self.flows.backward_mask)
-        a.mask_sum = P(self._msum)
+        a.focal, a.k4 = _ptr(self._focal), _ptr(self._k4)
+        a.fflow, a.bflow = _ptr(self.flows.forward), _ptr(self.flows.backward)
+        a.fmask, a.bmask = _ptr(self.flows.forward_mask), _ptr(self.flows.backward_mask)
+        a.mask_sum = _ptr(self._msum)
         a.mapping, a.delta, a.flow_weight = ops.MAPPINGS[cfg.mapping], cfg.delta, cfg.flow_weight
-        (a.m_depth, a.v_depth, a.m_weights, a.v_weights, a.m_focal, a.v_focal) = [P(t) for t in self._state]
+        (a.m_depth, a.v_depth, a.m_weights, a.v_weights, a.m_focal, a.v_focal) = [_ptr(t) for t in self._state]
         a.lr, a.beta1, a.beta2, a.eps = cfg.lr, 0.9, 0.999, 1e-8
-        a.g_depth, a.g_weights, a.g_focal, a.g_k4 = P(self._g_depth), P(self._g_w), P(self._g_focal), P(self._g_k4)
-        a.rt, a.loss, a.ws = P(self.rt), P(self._loss), P(self._ws)
+        a.g_depth, a.g_weights = _ptr(self._g_depth), _ptr(self._g_w)
+        a.g_focal, a.g_k4 = _ptr(self._g_focal), _ptr(self._g_k4)
+        a.rt, a.loss, a.ws = _ptr(self.rt), _ptr(self._loss), _ptr(self._ws)
         # step-dependent scalars live in device memory: every step is the same launch sequence
         self._clock = ops.StepClock(dev, cfg.lr)
         self._side_stream = torch.cuda.Stream(device=dev)  # parallel branch of the step (see _step_softmin)
@@ -401,16 +402,16 @@ class FusedOverfitter(Overfitter):
             assert self.tracks is not None
             pk = ops.PackedTracks(self.tracks, dev, self._track_frames)
             self._packed = pk
-            self._pk_c = PackedTracksC(P(pk.seg), P(pk.xy), P(pk.vis), pk.num_segments, pk.max_rows, pk.max_points,
-                                       pk.total)
+            self._pk_c = PackedTracksC(_ptr(pk.seg), _ptr(pk.xy), _ptr(pk.vis), pk.num_segments, pk.max_rows,
+                                       pk.max_points, pk.total)
             self._ext = torch.empty(*frame_dims, 4, 4, device=dev)
             self._g_ext = torch.empty(*frame_dims, 4, 4, device=dev)
             self._g_rt = torch.empty(*pair_dims, 3, 4, device=dev)
             self._tg_k4 = None if self._gt else torch.empty(T, 4, device=dev)
             self._tws = torch.empty(lib().fm_track_workspace_bytes(T, pk.total), dtype=torch.uint8, device=dev)
             a.track_weight = cfg.tracking_weight
-            a.extrinsics, a.g_extrinsics, a.g_rt = P(self._ext), P(self._g_ext), P(self._g_rt)
-            a.track_g_k4, a.track_loss, a.track_ws = P(self._tg_k4), P(self._track_loss), P(self._tws)
+            a.extrinsics, a.g_extrinsics, a.g_rt = _ptr(self._ext), _ptr(self._g_ext), _ptr(self._g_rt)
+            a.track_g_k4, a.track_loss, a.track_ws = _ptr(self._tg_k4), _ptr(self._track_loss), _ptr(self._tws)
         self._args, self._ctypes = a, ctypes
         self._lib = lib()
         self._mlog = None  # per-step metrics ring (enable_metrics_log)
@@ -498,72 +499,132 @@ class FusedOverfitter(Overfitter):
                 self._clock.ptr, 0, self._clock.betas[0], self._clock.betas[1], 1e-8,
                 torch.cuda.current_stream().cuda_stream), "fm_adam_step_clock_frames_videos")
 
-    def _window_entry(self) -> Tensor:
-        """The sweep's focal estimate for the hand-over window: a scalar, or (B,) for several videos."""
-        return self._sw_focal[0].clone() if self._layout is None else self._sw_focal.clone()
-
     def _softmin_stage(self) -> bool:
         c = self.cfg
         return self._softmin and not (c.regression_after is not None and
                                       self.global_step >= c.regression_after)
+
+    def _begin_step(self):
+        """The step's Procrustes point subset, redrawn every step under procrustes_randomize, and its flow
+        weight, 0 before flow_enable_after (loss.py:40-41)."""
+        c, a = self.cfg, self._args
+        if c.procrustes_randomize:
+            self._indices = self.model.extrinsics.select_indices(*self._hw, self.rt.device)
+        a.indices = _ptr(self._indices)
+        a.num_indices = 0 if self._indices is None else self._indices.numel()
+        a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
+
+    def _sweep_indices(self, clocked: bool = False, split: bool = False) -> Tensor:
+        """The sweep's point sample (intrinsics_softmin.py:90): injected_indices when set -- on the split
+        step also the model's own -- else a random subset, seeded by the step clock when `clocked` (the
+        update steps of training_step, which a CUDA graph may replay)."""
+        idx = self.injected_indices
+        if idx is None and split:
+            idx = getattr(self.model.intrinsics, "injected_indices", None)
+        if idx is None:
+            hw = self._hw[0] * self._hw[1]
+            if clocked:
+                idx = ops.random_subset_clock(self._clock, hw, self._idx_buf)
+            else:
+                idx = ops.random_subset(hw, min(self.cfg.softmin_points, hw), self.rt.device)
+        return idx.contiguous()
+
+    def _weight_args(self):
+        """(pointer, sensitivity) of the correspondence weights that the sweep and the moment pass read."""
+        if not self.cfg.use_correspondence_weights:
+            return None, 0.0
+        return _ptr(self._wlog), self.cfg.weight_sensitivity
+
+    def _sweep_forward(self, idx: Tensor, stream):
+        """Candidate sweep on the first pair of every video at the points `idx`, and its softmin focal
+        estimate into _sw_focal (intrinsics_softmin.py:84-131), on the CUDA stream handle `stream`."""
+        from ._lib import check
+        L, n, (h, w) = self._lib, self.cfg.softmin_candidates, self._hw
+        wl, sens = self._weight_args()
+        head = (_ptr(self._depth), wl, sens, _ptr(self.flows.backward), _ptr(idx), idx.numel(), _ptr(self._cand_k4),
+                n, _ptr(self._sw_err), _ptr(self._sw_rt), _ptr(self._sw_ws))
+        if self._layout is not None:
+            check(L.fm_softmin_sweep_fwd_videos(*head, self._layout_ref, h, w, stream), "fm_softmin_sweep_fwd_videos")
+        else:
+            check(L.fm_softmin_sweep_fwd(*head, 1, self.T, h, w, stream), "fm_softmin_sweep_fwd")
+        check(L.fm_softmin_focal(_ptr(self._sw_err), _ptr(self._cand_f), n, self.B, _ptr(self._sw_sm),
+                                 _ptr(self._sw_focal), stream), "fm_softmin_focal")
+
+    def _sweep_backward(self, idx: Tensor, stream):
+        """The sweep's backward from d loss / d focal in _g_focal: adds to the gradients of frames 0 / 1 and
+        pair 0 of every video."""
+        from ._lib import check
+        L, n, (h, w) = self._lib, self.cfg.softmin_candidates, self._hw
+        wl, sens = self._weight_args()
+        check(L.fm_softmin_focal_bwd(_ptr(self._sw_sm), _ptr(self._cand_f), _ptr(self._sw_focal),
+                                     _ptr(self._g_focal), n, self.B, _ptr(self._sw_gerr), stream),
+              "fm_softmin_focal_bwd")
+        head = (_ptr(self._depth), wl, sens, _ptr(self.flows.backward), _ptr(idx), idx.numel(), _ptr(self._cand_k4),
+                n, _ptr(self._sw_rt), _ptr(self._sw_gerr), _ptr(self._g_depth), _ptr(self._g_w) if wl else None,
+                _ptr(self._sw_ws))
+        if self._layout is not None:
+            check(L.fm_softmin_sweep_bwd_videos(*head, self._layout_ref, h, w, stream), "fm_softmin_sweep_bwd_videos")
+        else:
+            check(L.fm_softmin_sweep_bwd(*head, 1, self.T, h, w, stream), "fm_softmin_sweep_bwd")
+
+    def _window(self, split: bool = False):
+        """The hand-over window of the softmin stage (intrinsics_softmin.py:133-139): on the split step
+        of a bound model that has one, the model's own list (drop-in surface), else this optimiser's."""
+        intr = self.model.intrinsics
+        return intr.window if split and hasattr(intr, "window") and self.optimizer is None else self.window
+
+    def _window_open(self) -> bool:
+        """Whether this step's sweep estimate joins the hand-over window."""
+        c = self.cfg
+        return (self._softmin_stage() and c.regression_after is not None and
+                self.global_step >= c.regression_after - c.regression_window)
+
+    def _append_window(self, split: bool = False):
+        """Append the sweep's focal estimate to the open window: a scalar, or (B,) for several videos."""
+        if self._window_open():
+            self._window(split).append(self._sw_focal[0].clone() if self._layout is None else self._sw_focal.clone())
+
+    def _hand_over(self, split: bool = False):
+        """At global_step == regression_after, seed the regressed focal length (each video's) with the
+        window's mean; the stacked window is (n,) for one video, (n, B) for several."""
+        if self._softmin and self.global_step == self.cfg.regression_after:
+            self._focal.copy_(torch.stack(self._window(split)).mean(0))
 
     def _step_softmin(self, update: bool):
         """Sweep stage (intrinsics_softmin.py:84-141): focal estimate from the candidate sweep,
         the step itself with that focal length, the sweep's backward, then Adam."""
         from ._lib import check
         c, a, L = self.cfg, self._args, self._lib
-        b, f, (h, w) = self.B, max(self.frames), self._hw
-        dev = self.rt.device
+        f, (h, w) = max(self.frames), self._hw
         st = torch.cuda.current_stream().cuda_stream
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        n = c.softmin_candidates
         rag = self._layout is not None
-        wl = P(self._wlog) if c.use_correspondence_weights else None
-        sens = c.weight_sensitivity if c.use_correspondence_weights else 0.0
         # All-pixel Procrustes: the moment pass of the step does not have to wait for the focal length
         # the sweep is about to produce -- the sums for one K follow exactly from the sums for another
         # (fm_overfit_step_args.moments_k4) -- so it runs beside the sweep, on the candidate-0 intrinsics.
         early_moments = update and self._indices is None and self._plan is None
         cur = torch.cuda.current_stream()
-        with torch.cuda.device(dev):
+        with torch.cuda.device(self.rt.device):
             if early_moments:
                 self._side_stream.wait_stream(cur)
+                wl, sens = self._weight_args()
                 if rag:
-                    check(L.fm_procrustes_moments_videos(P(self._depth), P(self._k4_base), P(self.flows.backward), wl,
-                                                         sens, P(self._ws), self._layout_ref, h, w, st),
-                          "fm_procrustes_moments_videos")
+                    check(L.fm_procrustes_moments_videos(_ptr(self._depth), _ptr(self._k4_base),
+                                                         _ptr(self.flows.backward), wl, sens, _ptr(self._ws),
+                                                         self._layout_ref, h, w, st), "fm_procrustes_moments_videos")
                 else:
-                    check(L.fm_procrustes_moments(P(self._depth), P(self._k4_base), P(self.flows.backward), wl, sens,
-                                                  P(self._ws), f, h, w, st), "fm_procrustes_moments")
+                    check(L.fm_procrustes_moments(_ptr(self._depth), _ptr(self._k4_base), _ptr(self.flows.backward),
+                                                  wl, sens, _ptr(self._ws), f, h, w, st), "fm_procrustes_moments")
             with torch.cuda.stream(self._side_stream if early_moments else cur):
-                sst = torch.cuda.current_stream().cuda_stream
-                idx = self.injected_indices
-                if idx is None:
-                    if update:  # seeded by the step clock (replayable); intrinsics_softmin.py:90
-                        idx = ops.random_subset_clock(self._clock, h * w, self._idx_buf)
-                    else:
-                        idx = ops.random_subset(h * w, min(c.softmin_points, h * w), dev)
-                idx = idx.contiguous()
-                if rag:
-                    check(L.fm_softmin_sweep_fwd_videos(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                                        idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                                        P(self._sw_rt), P(self._sw_ws), self._layout_ref, h, w, sst),
-                          "fm_softmin_sweep_fwd_videos")
-                else:
-                    check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                                 idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                                 P(self._sw_rt), P(self._sw_ws), b, f, h, w, sst),
-                          "fm_softmin_sweep_fwd")
-                check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, b, P(self._sw_sm),
-                                         P(self._sw_focal), sst), "fm_softmin_focal")
+                idx = self._sweep_indices(clocked=update)
+                self._sweep_forward(idx, torch.cuda.current_stream().cuda_stream)
             if early_moments:
                 cur.wait_stream(self._side_stream)
-            a.moments_k4 = P(self._k4_base) if early_moments else None
+            a.moments_k4 = _ptr(self._k4_base) if early_moments else None
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
             # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
             fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and not rag
-            a.focal = P(self._sw_focal)
+            a.focal = _ptr(self._sw_focal)
             a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
             a.defer_adam = 1 if fuse else 0
             try:
@@ -580,21 +641,7 @@ class FusedOverfitter(Overfitter):
                 side.wait_stream(cur)
                 with torch.cuda.stream(side):
                     self._adam_frames(0, 2, f)
-            check(L.fm_softmin_focal_bwd(P(self._sw_sm), P(self._cand_f), P(self._sw_focal),
-                                         P(self._g_focal), n, b, P(self._sw_gerr), st),
-                  "fm_softmin_focal_bwd")
-            if rag:
-                check(L.fm_softmin_sweep_bwd_videos(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                                    idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
-                                                    P(self._sw_gerr), P(self._g_depth), P(self._g_w) if wl else None,
-                                                    P(self._sw_ws), self._layout_ref, h, w, st),
-                      "fm_softmin_sweep_bwd_videos")
-            else:
-                check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                             idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
-                                             P(self._sw_gerr), P(self._g_depth),
-                                             P(self._g_w) if wl else None, P(self._sw_ws), b, f, h, w, st),
-                      "fm_softmin_sweep_bwd")
+            self._sweep_backward(idx, st)
         if update:
             self._adam_frames(0, 0, 2)
             if c.use_correspondence_weights:
@@ -604,12 +651,6 @@ class FusedOverfitter(Overfitter):
 
     # ---- split step: the two halves of one iteration WITHOUT the parameter update, for callers that
     # need the loss values before they decide on the backward (torch.autograd: flowmap_b200.fused)
-    def _window(self):
-        """The hand-over window of the softmin stage (intrinsics_softmin.py:133-139): the bound
-        model's own list when there is one (drop-in surface), else this optimiser's."""
-        intr = self.model.intrinsics
-        return intr.window if hasattr(intr, "window") and self.optimizer is None else self.window
-
     def forward_phase(self, global_step: int, training: bool = True, depth: Optional[Tensor] = None,
                       weights: Optional[Tensor] = None):
         """Poses + flow loss with its direct gradients (fm_overfit_step, FM_STEP_FORWARD; the
@@ -619,48 +660,28 @@ class FusedOverfitter(Overfitter):
         they stay referenced until the next call (backward_phase reads them)."""
         from ._lib import check
         self._refuse_videos("the split-step surface")
-        c, a, L = self.cfg, self._args, self._lib
+        a, L = self._args, self._lib
         _, f, _, h, w = self.batch.videos.shape
         if self._network:
             self._bind_inputs(depth, weights, f, h, w)
         elif depth is not None or weights is not None:
             raise ValueError("flowmap_b200: an explicit-depth optimiser reads its own depth and weights")
-        dev = self.rt.device
         st = torch.cuda.current_stream().cuda_stream
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         self.global_step = global_step
-        if c.procrustes_randomize:
-            self._indices = self.model.extrinsics.select_indices(h, w, dev)
-        a.indices = None if self._indices is None else self._indices.data_ptr()
-        a.num_indices = 0 if self._indices is None else self._indices.numel()
-        a.flow_weight = c.flow_weight if global_step >= c.flow_enable_after else 0.0
+        self._begin_step()
         a.tracks, a.step, a.defer_adam = None, 0, 0
         self._sweep_idx = None
-        with torch.cuda.device(dev):
+        with torch.cuda.device(self.rt.device):
             if self._softmin_stage():
-                idx = self.injected_indices
-                if idx is None:
-                    idx = getattr(self.model.intrinsics, "injected_indices", None)
-                if idx is None:
-                    idx = ops.random_subset(h * w, min(c.softmin_points, h * w), dev)
-                self._sweep_idx = idx = idx.contiguous()
-                n = c.softmin_candidates
-                wl = P(self._wlog) if c.use_correspondence_weights else None
-                sens = c.weight_sensitivity if c.use_correspondence_weights else 0.0
-                check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                             idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                             P(self._sw_rt), P(self._sw_ws), 1, f, h, w, st),
-                      "fm_softmin_sweep_fwd")
-                check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, 1, P(self._sw_sm),
-                                         P(self._sw_focal), st), "fm_softmin_focal")
-                a.focal = P(self._sw_focal)
-                if training and c.regression_after is not None and \
-                        global_step >= c.regression_after - c.regression_window:
-                    self._window().append(self._sw_focal[0].clone())
+                self._sweep_idx = self._sweep_indices(split=True)
+                self._sweep_forward(self._sweep_idx, st)
+                a.focal = _ptr(self._sw_focal)
+                if training:
+                    self._append_window(split=True)
             else:
-                if self._softmin and global_step == c.regression_after and training:
-                    self._focal.copy_(torch.stack(self._window()).mean())
-                a.focal = None if self._focal is None else self._focal.data_ptr()
+                if training:
+                    self._hand_over(split=True)
+                a.focal = _ptr(self._focal)
             a.phase = 1  # FM_STEP_FORWARD
             try:
                 check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (forward)")
@@ -686,16 +707,15 @@ class FusedOverfitter(Overfitter):
         Returns the weighted tracking loss (device scalar buffer)."""
         from ._lib import check
         self._refuse_videos("the split-step surface")
-        c, a, L, pk = self.cfg, self._args, self._lib, self._packed
+        c, L, pk = self.cfg, self._lib, self._packed
         _, f, _, h, w = self.batch.videos.shape
-        P = lambda t: t.data_ptr()  # noqa: E731
         st = torch.cuda.current_stream().cuda_stream
         with torch.cuda.device(self.rt.device):
-            check(L.fm_pose_chain(P(self.rt), P(self._ext), 1, f, st), "fm_pose_chain")
+            check(L.fm_pose_chain(_ptr(self.rt), _ptr(self._ext), 1, f, st), "fm_pose_chain")
             check(L.fm_track_loss_fwd_sharded(
-                P(self._depth), P(self._k4), P(self._ext), P(pk.seg), pk.num_segments, pk.max_rows,
-                pk.max_points, P(pk.xy), P(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta,
-                c.tracking_weight, P(self._track_loss), P(self._tws), f, h, w, 0, 0, f, 1, st),
+                _ptr(self._depth), _ptr(self._k4), _ptr(self._ext), _ptr(pk.seg), pk.num_segments, pk.max_rows,
+                pk.max_points, _ptr(pk.xy), _ptr(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta,
+                c.tracking_weight, _ptr(self._track_loss), _ptr(self._tws), f, h, w, 0, 0, f, 1, st),
                 "fm_track_loss_fwd")
         return self._track_loss
 
@@ -705,12 +725,10 @@ class FusedOverfitter(Overfitter):
         Leaves the gradients in gradients()."""
         from ._lib import check
         self._refuse_videos("the split-step surface")
-        c, a, L = self.cfg, self._args, self._lib
-        _, f, _, h, w = self.batch.videos.shape
+        a, L = self._args, self._lib
         st = torch.cuda.current_stream().cuda_stream
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         a.tracks = self._ctypes.pointer(self._pk_c) if with_tracking else None
-        a.flow_grad_scale, a.track_grad_scale = P(flow_scale), P(track_scale)
+        a.flow_grad_scale, a.track_grad_scale = _ptr(flow_scale), _ptr(track_scale)
         a.phase, a.step, a.defer_adam = 2, 0, 0  # FM_STEP_BACKWARD
         # Without tracks this phase adds g_rt / track_g_k4 as a caller's pose / intrinsics gradient: a step
         # whose tracking loss is not enabled yet (loss.py:40-41) has none, whatever those buffers hold.
@@ -724,17 +742,7 @@ class FusedOverfitter(Overfitter):
                 a.phase, a.tracks, a.flow_grad_scale, a.track_grad_scale = 0, None, None, None
                 a.g_rt, a.track_g_k4 = kept
             if self._sweep_idx is not None:
-                idx, n = self._sweep_idx, c.softmin_candidates
-                wl = P(self._wlog) if c.use_correspondence_weights else None
-                sens = c.weight_sensitivity if c.use_correspondence_weights else 0.0
-                check(L.fm_softmin_focal_bwd(P(self._sw_sm), P(self._cand_f), P(self._sw_focal),
-                                             P(self._g_focal), n, 1, P(self._sw_gerr), st),
-                      "fm_softmin_focal_bwd")
-                check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                             idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
-                                             P(self._sw_gerr), P(self._g_depth),
-                                             P(self._g_w) if wl else None, P(self._sw_ws), 1, f, h, w, st),
-                      "fm_softmin_sweep_bwd")
+                self._sweep_backward(self._sweep_idx, st)
 
     def _refuse_videos(self, what: str):
         if self._layout is not None:
@@ -743,18 +751,17 @@ class FusedOverfitter(Overfitter):
     def _step_body(self, update: bool, track_on: bool, sweep: bool):
         """One step as a fixed launch sequence (no host-side step numbers: see ops.StepClock)."""
         from ._lib import check
-        c, a = self.cfg, self._args
+        a = self._args
         if update:
             self._clock.tick(tick_focal=not sweep and not self._gt)
         a.tracks = self._ctypes.pointer(self._pk_c) if track_on else None
-        a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
         # the metrics row is indexed by the step clock, which only update steps advance
         a.metrics_log = self._mlog.data_ptr() if (update and self._mlog is not None) else None
         try:
             if sweep:
                 self._step_softmin(update)
             else:
-                a.focal = None if self._focal is None else self._focal.data_ptr()
+                a.focal = _ptr(self._focal)
                 a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
                 with torch.cuda.device(self.rt.device):
                     self._call_step()
@@ -789,31 +796,24 @@ class FusedOverfitter(Overfitter):
     def training_step(self, update: bool = True):
         """Returns (total loss (device tensor: a scalar, or the (B,) per-video totals), relative poses
         rt (B, F-1, 3, 4), or a list of (F_b - 1, 3, 4) for videos of different lengths)."""
-        c, a = self.cfg, self._args
+        c = self.cfg
         if self._network:
             raise ValueError("flowmap_b200: a network backbone's step runs through the model's losses "
                              "(forward_phase / backward_phase), not training_step")
-        if c.procrustes_randomize:
-            self._indices = self.model.extrinsics.select_indices(*self._hw, self.rt.device)
-        a.indices = None if self._indices is None else self._indices.data_ptr()
-        a.num_indices = 0 if self._indices is None else self._indices.numel()
+        self._begin_step()
         track_on = c.use_tracking and self.global_step >= c.tracking_enable_after
         sweep = self._softmin_stage()
         if update:
             self._clock.set(self.optimizer_steps, self.focal_steps)
-            if self._softmin and not sweep and self.global_step == c.regression_after:
-                # hand-over: seed the regressed focal length (each video's) once
-                self._focal.copy_(torch.stack(self.window).mean(0))
-        window_on = sweep and c.regression_after is not None and \
-            self.global_step >= c.regression_after - c.regression_window
+            self._hand_over()
+        window_on = self._window_open()
         key = (track_on, sweep, self.global_step >= c.flow_enable_after)
         graphable = (update and self.use_cuda_graph and not c.procrustes_randomize and not window_on and
                      getattr(self, "injected_indices", None) is None)
         ticks_focal = not sweep and not self._gt
         self._run_body(key, graphable, lambda upd=update: self._step_body(upd, track_on, sweep), ticks_focal)
         if update:
-            if window_on:
-                self.window.append(self._window_entry())
+            self._append_window()
             self.global_step += 1
             self.optimizer_steps += 1
             self.focal_steps += int(ticks_focal)
@@ -1026,26 +1026,25 @@ class ShardedFusedOverfitter(FusedOverfitter):
         from ._lib import check
         c, L, pk, F = self.cfg, self._lib, self._packed, self._F
         a0, b0 = self.plan.pair_range
-        P = lambda t: t.data_ptr()  # noqa: E731
         st = torch.cuda.current_stream().cuda_stream
         parallel.gather_pairs(self.plan, self.rt, self._rt_all, self.group)
         k4_all = self._k4[0].expand(F, 4).contiguous()  # one shared focal length
-        args = (P(k4_all), P(self._ext_all), P(pk.seg), pk.num_segments, pk.max_rows, pk.max_points, P(pk.xy),
-                P(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta, c.tracking_weight)
+        args = (_ptr(k4_all), _ptr(self._ext_all), _ptr(pk.seg), pk.num_segments, pk.max_rows, pk.max_points,
+                _ptr(pk.xy), _ptr(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta, c.tracking_weight)
         tail = (F, h, w, a0, self._src_range[0], self._src_range[1])
         with torch.cuda.device(self.rt.device):
-            check(L.fm_pose_chain(P(self._rt_all), P(self._ext_all), 1, F, st), "fm_pose_chain")
-            check(L.fm_track_loss_fwd_sharded(P(self._depth), *args, None, P(self._tws), *tail, 1, st),
+            check(L.fm_pose_chain(_ptr(self._rt_all), _ptr(self._ext_all), 1, F, st), "fm_pose_chain")
+            check(L.fm_track_loss_fwd_sharded(_ptr(self._depth), *args, None, _ptr(self._tws), *tail, 1, st),
                   "fm_track_loss_fwd_sharded")  # shared focal: only the summed K gradient is used
             if self.plan.world > 1:
                 dist.all_reduce(self._treduce, group=self.group)
-            check(L.fm_track_loss_value(P(self._tws), c.tracking_weight, P(self._track_loss), st),
+            check(L.fm_track_loss_value(_ptr(self._tws), c.tracking_weight, _ptr(self._track_loss), st),
                   "fm_track_loss_value")
-            check(L.fm_track_loss_bwd_sharded(P(self._depth), *args, None, P(self._g_depth), P(self._g_ext_all),
-                                              P(self._tg_k4_all), P(self._tws), *tail, st),
+            check(L.fm_track_loss_bwd_sharded(_ptr(self._depth), *args, None, _ptr(self._g_depth),
+                                              _ptr(self._g_ext_all), _ptr(self._tg_k4_all), _ptr(self._tws), *tail, st),
                   "fm_track_loss_bwd_sharded")
-            check(L.fm_pose_chain_bwd(P(self._rt_all), P(self._ext_all), P(self._g_ext_all),
-                                      P(self._g_rt_all), 1, F, st), "fm_pose_chain_bwd")
+            check(L.fm_pose_chain_bwd(_ptr(self._rt_all), _ptr(self._ext_all), _ptr(self._g_ext_all),
+                                      _ptr(self._g_rt_all), 1, F, st), "fm_pose_chain_bwd")
         self._g_rt_local.copy_(self._g_rt_all[:, a0:b0])
         scale = (h * w) ** 0.5
         return (self._tg_k4_all[:, 0].double().sum() * (scale / w) +
@@ -1057,11 +1056,10 @@ class ShardedFusedOverfitter(FusedOverfitter):
         boundary frames and the two scalars travel, then the boundary frames and the focal length."""
         from ._lib import check
         c, a, p, r = self.cfg, self._args, self.plan, self.reducer
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         clk = self._clock
         clk.tick(tick_focal=True)
         a.clock, a.tracks, a.step, a.focal_step, a.defer_adam, a.phase = clk.ptr, None, 1, 1, 2, 0
-        a.focal = P(self._focal)
+        a.focal = _ptr(self._focal)
         # the step writes its two scalars (loss, d focal) straight into the all-reduce buffer
         loss_ptr, gf_ptr = a.loss, a.g_focal
         a.loss, a.g_focal = r.scal[0:1].data_ptr(), r.scal[1:2].data_ptr()
@@ -1090,12 +1088,11 @@ class ShardedFusedOverfitter(FusedOverfitter):
         import torch.distributed as dist
         from ._lib import check
         c, a, p, L = self.cfg, self._args, self.plan, self._lib
-        _, _, _, h_, w_ = self.batch.videos.shape
+        _, _, _, h, w = self.batch.videos.shape
+        self._begin_step()
         if (update and not self._softmin and not c.procrustes_randomize and self._indices is None and
-                c.use_correspondence_weights and w_ % 4 == 0 and
+                c.use_correspondence_weights and w % 4 == 0 and
                 not (c.use_tracking and self.global_step >= c.tracking_enable_after)):
-            a.indices, a.num_indices = None, 0
-            a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
             self._clock.set(self.optimizer_steps, self.focal_steps)
             self._run_body(("flow", self.global_step >= c.flow_enable_after), self.use_cuda_graph,
                            self._flow_only_body, True)
@@ -1103,15 +1100,8 @@ class ShardedFusedOverfitter(FusedOverfitter):
             self.optimizer_steps += 1
             self.focal_steps += 1
             return self._total.clone(), self.rt
-        _, _, _, h, w = self.batch.videos.shape
-        P = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         st = torch.cuda.current_stream().cuda_stream
         dev = self.rt.device
-        if c.procrustes_randomize:
-            self._indices = self.model.extrinsics.select_indices(h, w, dev)
-        a.indices = None if self._indices is None else self._indices.data_ptr()
-        a.num_indices = 0 if self._indices is None else self._indices.numel()
-        a.flow_weight = c.flow_weight if self.global_step >= c.flow_enable_after else 0.0
         track_on = c.use_tracking and self.global_step >= c.tracking_enable_after
         sweep = self._softmin_stage()
         own_sweep = sweep and p.rank == 0
@@ -1123,36 +1113,24 @@ class ShardedFusedOverfitter(FusedOverfitter):
         a.step = self.optimizer_steps + 1 if fuse_w else 0
         a.defer_adam = (1 if own_sweep else 2) if fuse_w else 0
         if sweep:
-            n = c.softmin_candidates
-            wl = P(self._wlog) if c.use_correspondence_weights else None
-            sens = c.weight_sensitivity if c.use_correspondence_weights else 0.0
             if own_sweep:
-                idx = self.injected_indices
-                if idx is None:
-                    idx = ops.random_subset(h * w, min(c.softmin_points, h * w), dev)
-                idx = idx.contiguous()
-                f_local = self._depth.shape[0]
+                idx = self._sweep_indices()
                 with torch.cuda.device(dev):
-                    check(L.fm_softmin_sweep_fwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                                 idx.numel(), P(self._cand_k4), n, P(self._sw_err),
-                                                 P(self._sw_rt), P(self._sw_ws), 1, f_local, h, w, st),
-                          "fm_softmin_sweep_fwd")
-                    check(L.fm_softmin_focal(P(self._sw_err), P(self._cand_f), n, 1, P(self._sw_sm),
-                                             P(self._sw_focal), st), "fm_softmin_focal")
+                    self._sweep_forward(idx, st)
             if p.world > 1:
                 dist.broadcast(self._sw_focal, src=self._first_rank(), group=self.group)
-            a.focal = P(self._sw_focal)
+            a.focal = _ptr(self._sw_focal)
         else:
-            a.focal = P(self._focal)
-            if self._softmin and self.global_step == c.regression_after and update:
-                self._focal.copy_(torch.stack(self.window).mean())  # hand-over, identical on all ranks
+            a.focal = _ptr(self._focal)
+            if update:
+                self._hand_over()  # identical on all ranks
         extra_focal = None
         with torch.cuda.device(dev):
             if track_on:
                 a.phase = 1  # FM_STEP_FORWARD
                 check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (forward)")
                 extra_focal = self._tracking_exchange(h, w)
-                a.phase, a.g_rt, a.track_g_k4 = 2, P(self._g_rt_local), None  # FM_STEP_BACKWARD
+                a.phase, a.g_rt, a.track_g_k4 = 2, _ptr(self._g_rt_local), None  # FM_STEP_BACKWARD
                 check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (backward)")
                 a.phase, a.g_rt = 0, None
             else:
@@ -1164,16 +1142,8 @@ class ShardedFusedOverfitter(FusedOverfitter):
         red = self.reducer.reduce(torch.stack((self._loss.reshape(()), g_focal)), self._g_depth)
         self._g_focal.copy_(red[1])
         if own_sweep:  # backward of the sweep with the summed focal gradient: frames 0/1, pair 0
-            f_local = self._depth.shape[0]
             with torch.cuda.device(dev):
-                check(L.fm_softmin_focal_bwd(P(self._sw_sm), P(self._cand_f), P(self._sw_focal),
-                                             P(self._g_focal), n, 1, P(self._sw_gerr), st),
-                      "fm_softmin_focal_bwd")
-                check(L.fm_softmin_sweep_bwd(P(self._depth), wl, sens, P(self.flows.backward), P(idx),
-                                             idx.numel(), P(self._cand_k4), n, P(self._sw_rt),
-                                             P(self._sw_gerr), P(self._g_depth),
-                                             P(self._g_w) if wl else None, P(self._sw_ws), 1, f_local, h, w, st),
-                      "fm_softmin_sweep_bwd")
+                self._sweep_backward(idx, st)
         if update:
             s_ = self.optimizer_steps + 1
             stt = self._state
@@ -1181,10 +1151,8 @@ class ShardedFusedOverfitter(FusedOverfitter):
             if c.use_correspondence_weights and (not fuse_w or own_sweep):
                 k = 1 if fuse_w else self._wlog.shape[0]  # pair 0 only when the rest was fused
                 ops.adam_step(self._wlog[:k], self._g_w[:k], stt[2][:k], stt[3][:k], s_, c.lr)
-            if sweep:
-                if c.regression_after is not None and self.global_step >= c.regression_after - c.regression_window:
-                    self.window.append(self._sw_focal[0].clone())
-            else:
+            self._append_window()
+            if not sweep:
                 self.focal_steps += 1
                 ops.adam_step(self._focal.reshape(1), self._g_focal.reshape(1), stt[4].reshape(1),
                               stt[5].reshape(1), self.focal_steps, c.lr)
@@ -1193,36 +1161,3 @@ class ShardedFusedOverfitter(FusedOverfitter):
         total = red[0] + self._track_loss if track_on else red[0]
         return total, self.rt
 
-
-class ShardedOverfitter(Overfitter):
-    """Pair-sharded optimisation (flowmap_b200.parallel): this rank holds the frames and
-    pairs of its ShardPlan; one all-reduce per step carries the loss, the focal-length
-    gradient and the boundary depth-gradient frames."""
-
-    def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, plan, device="cuda",
-                 group=None):
-        from . import parallel
-        if cfg.use_tracking or cfg.intrinsics != "regressed":
-            raise NotImplementedError("pair sharding currently covers the flow loss with a "
-                                      "regressed focal length (BASELINE config 4)")
-        super().__init__(cfg, batch, flows, None, device)
-        self.plan, self.group = plan, group
-        _, _, _, h, w = batch.videos.shape
-        self.reducer = parallel.StepReducer(plan, (h, w), self.flows.forward.device, 2, group)
-        local = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
-        self.losses[0].set_global_mask_sum(parallel.global_mask_sum(local, group))
-
-    def training_step(self):
-        self.optimizer.zero_grad()
-        out = self.model(self.batch, self.flows, self.global_step)
-        total = 0
-        for loss_fn in self.losses:
-            total = total + loss_fn.forward(self.batch, self.flows, None, out, self.global_step)
-        total.backward()
-        focal = self.model.intrinsics.focal_length
-        scalars = torch.stack((total.detach(), focal.grad.reshape(())))
-        red = self.reducer.reduce(scalars, self.model.backbone.depth.grad)
-        focal.grad.copy_(red[1])
-        self.optimizer.step()
-        self.global_step += 1
-        return red[0], out

@@ -50,7 +50,7 @@ def _worker(rank, world, port, f, h, w, out_dir):
             st.depth.copy_(d_l)
             st.weights.copy_(w_l)
         out = st.forward(fl_l, 0)
-        # local loss normalised by the GLOBAL mask sum (what LossFlow does with set_global_mask_sum)
+        # local loss normalised by the GLOBAL mask sum (what the pair-sharded step does with global_mask_sum)
         local_den = fl_l.forward_mask.sum() + fl_l.backward_mask.sum()
         den = parallel.global_mask_sum(local_den.reshape(()).clone())
         loss = 1000.0 * O.flow_loss(out.surfaces, out.extrinsics, out.intrinsics, fl_l) * local_den / den
