@@ -101,8 +101,9 @@ Workspace carve(void* base, int B, int F) { return carve_rows(base, B, (size_t)B
 // frame_offset[b + 1] - b - 1) of the (P, ...) ones, P = T - B.  Pair p of video b joins frames p + b and
 // p + b + 1, so no pair crosses two videos.  The per-frame and per-video kernels are templated on the video
 // layout: Videos, or Uniform below, and find a frame's or a pair's video through these accessors.
-// Scale: how a layout's kernels take d total / d loss.  Packed videos run only whole steps, so their loss
-// gradients are never scaled (NoScale); one video also runs split phases, which pass it as a device scalar.
+// Scale: how a layout's kernels take d total / d loss.  Whole steps of packed videos never scale their loss
+// gradients (NoScale); one video also runs split phases, which pass it as a device scalar, and so does the
+// split backward of packed videos through VideosScaled (its focal gradient only).
 struct NoScale {
   __host__ __device__ NoScale(const float*) {}
 };
@@ -117,6 +118,12 @@ struct Videos {
   __device__ __forceinline__ int of_pair(int p) const { return __ldg(pair_video + p); }
   __device__ __forceinline__ int first(int b) const { return __ldg(frame_offset + b); }
   __device__ __forceinline__ int frames(int b) const { return __ldg(frame_offset + b + 1) - __ldg(frame_offset + b); }
+};
+// Packed videos in the backward phase of a split step: one d total / d flow loss for the whole batch (the
+// pooled flow loss of a pretraining batch), a device scalar.  A layout of its own, so that the whole-step
+// Videos instances keep their code.
+struct VideosScaled : Videos {
+  using Scale = const float* __restrict__;
 };
 // B videos of F frames each in the (B F, ...) and (B (F - 1), ...) buffers: one video (B = 1) and the
 // standalone (B, F) entry points.  Pair p of video b joins frames p + b and p + b + 1, as in Videos.
@@ -3779,7 +3786,15 @@ const char* step_refusal(const fm_overfit_step_args* a, const Uniform&) {
                   : nullptr;
 }
 const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
-  if (a->phase != FM_STEP_ALL || a->splat_plan) return "fm_overfit_step_videos: serves whole steps without a splat plan";
+  if (a->splat_plan) return "fm_overfit_step_videos: serves steps without a splat plan";
+  // The split phases serve a network backbone's batch (pretraining): the caller owns the update, and the
+  // tracking kernels of packed videos take no d total / d tracking loss (TrackVideos::Scale is NoScale).
+  if (a->phase != FM_STEP_ALL) {
+    if (a->tracks) return "fm_overfit_step_videos: a split step (FM_STEP_FORWARD / FM_STEP_BACKWARD) takes no tracks";
+    if (a->step != 0 || a->defer_adam != 0)
+      return "fm_overfit_step_videos: a split step updates no parameter (pass step = 0 and defer_adam = 0)";
+    if (a->metrics_log) return "fm_overfit_step_videos: a split step writes no metrics log";
+  }
   if (a->defer_adam == 1 && a->step > 0 && a->weight_logits)
     return "fm_overfit_step_videos: does not fuse the logit update of a deferred step (pass step = 0)";
   if (a->metrics_log && !a->gt_fxfy) return "fm_overfit_step_videos: metrics need gt_fxfy";
@@ -3793,6 +3808,19 @@ TrackOneVideo track_layout(const Uniform&) { return TrackOneVideo{}; }
 TrackVideos track_layout(const Videos& v) { return TrackVideos{v.frame_video}; }
 double* step_track_sums(const Uniform&, const Workspace&, void* track_ws) { return (double*)track_ws; }
 double* step_track_sums(const Videos&, const Workspace& w, void*) { return w.track_sums; }
+
+// d loss / d focal of every video (k_focal_grad), the flow part scaled by fscale (NULL = 1).  Packed videos
+// see a scale only in the backward phase of a split step: that takes the VideosScaled instance, whole steps
+// keep the NoScale one.
+void launch_focal_grad(const Workspace& w, const float* track_g_k4, float* g_focal, int B, int H, int W,
+                       const Uniform& u, const float* fscale, cudaStream_t s) {
+  k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, u, fscale);
+}
+void launch_focal_grad(const Workspace& w, const float* track_g_k4, float* g_focal, int B, int H, int W,
+                       const Videos& v, const float* fscale, cudaStream_t s) {
+  if (fscale) k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, VideosScaled{v}, fscale);
+  else k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, v, NoScale(nullptr));
+}
 
 // The metrics row: one video reads the scalar gt_fx / gt_fy through k_trajectory_ate's row mode, packed
 // videos the (B, 2) gt_fxfy.
@@ -3991,7 +4019,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       return rc;
   }
   if (a->focal) {  // d loss / d focal, then (update steps) its Adam
-    k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, a->g_focal, H, W, lay, fscale);
+    launch_focal_grad(w, track_g_k4, a->g_focal, B, H, W, lay, fscale, s);
     FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
     if (a->step > 0 && !defer) {
       const int fstep = a->focal_step > 0 ? a->focal_step : a->step;

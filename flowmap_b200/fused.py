@@ -23,9 +23,16 @@ root's backward hands d loss / d depths and d loss / d weights to autograd, whic
 the network.  Outputs read before or after the losses reuse the stored BackboneOutput: the backbone
 never runs twice in one step.
 
+A network backbone's batch of several videos (the pretraining step, pretrain.py) runs on the packed layout
+of fm_overfit_step_videos when its intrinsics are softmin without a regression stage and no tracks come
+with it: one candidate sweep and one focal length per video, and LossFlow's one pooled mask sum for the
+whole batch (loss_flow.py:31-70), written into every video's slot, so that the step's (B,) losses sum to
+the loss autograd sees and one grad_output scales them all.
+
 Anything the fused step does not cover (a consumer that reads `model_output.extrinsics` under
-autograd, a batch of several videos, per-frame intrinsics, different mappings for the two losses)
-makes the LazyModelOutput materialise itself through the per-op autograd Functions of
+autograd, several explicit-depth videos, a batch of several videos with a regressed focal length, a
+regression stage, ground-truth intrinsics or tracks, per-frame intrinsics, different mappings for the two
+losses) makes the LazyModelOutput materialise itself through the per-op autograd Functions of
 flowmap_b200.ops: same results, the former speed.
 """
 from __future__ import annotations
@@ -107,6 +114,8 @@ class FusedStep:
                                   weights=inputs[1].detach() if inputs is not None and len(inputs) > 1 else None)
         self.token = _StepRoot.apply(self, *params)
         self.flow_done = True
+        if value.dim():  # a batch of videos: each normalised by the pooled mask sum, their sum is LossFlow's value
+            value = value.sum()
         return _LossNode.apply(self.token, self, "flow", value)
 
     def track_loss(self, loss_mod, tracks) -> Optional[Tensor]:
@@ -147,11 +156,11 @@ class FusedStep:
         """Detached ModelOutput of the step the forward half evaluated (for logging / visualisers
         that read the output after the losses): poses and intrinsics come from the engine's buffers."""
         eng, model = self.engine, self.model
-        _, f, _, h, w = self.batch.videos.shape
+        b, f = self.batch.videos.shape[:2]
         with torch.no_grad():
-            k4 = eng.intrinsics_k4()[None].clone()
-            rt = eng.rt.clone()
-            k = torch.zeros(1, f, 3, 3, device=k4.device)
+            k4 = eng.intrinsics_k4().reshape(b, f, 4).clone()
+            rt = eng.rt.reshape(b, f - 1, 3, 4).clone()
+            k = torch.zeros(b, f, 3, 3, device=k4.device)
             k[..., 0, 0], k[..., 1, 1], k[..., 0, 2], k[..., 1, 2], k[..., 2, 2] = \
                 k4[..., 0], k4[..., 1], k4[..., 2], k4[..., 3], 1.0
             bo = self.backbone_out

@@ -272,21 +272,25 @@ class Model(nn.Module):
     def _fusable(self, batch: Batch, flows: Flows, backbone_out: Optional[BackboneOutput] = None) -> bool:
         """Whether the losses of this step can run on the fused halves.  A network backbone (any backbone
         but BackboneExplicitDepth, e.g. the reference's BackboneMidas) is judged on the BackboneOutput of
-        the step: one video of CUDA depths (1, F, H, W) and weights (1, F-1, H, W)."""
+        the step: CUDA depths (B, F, H, W) and weights (B, F-1, H, W).  B > 1 (pretraining) takes one focal
+        length per video: softmin intrinsics without a regression stage (the regressed focal length, and the
+        window of a regression stage, are one value for the whole batch in the reference)."""
+        b = batch.videos.shape[0]
         if not (self.fused_enabled and torch.is_grad_enabled() and self.training and
                 isinstance(self.extrinsics, ExtrinsicsProcrustes) and
-                isinstance(self.intrinsics, (IntrinsicsRegressed, IntrinsicsSoftmin)) and
-                batch.videos.shape[0] == 1 and flows.forward.is_cuda):
+                isinstance(self.intrinsics, (IntrinsicsRegressed, IntrinsicsSoftmin)) and flows.forward.is_cuda):
             return False
         if isinstance(self.backbone, BackboneExplicitDepth):
-            return self.backbone.depth.is_cuda
+            return b == 1 and self.backbone.depth.is_cuda
         if backbone_out is None:
+            return False
+        if b > 1 and not (isinstance(self.intrinsics, IntrinsicsSoftmin) and self.intrinsics.cfg.regression is None):
             return False
         _, f, _, h, w = batch.videos.shape
         d, wt = backbone_out.depths, backbone_out.weights
         return (isinstance(d, Tensor) and isinstance(wt, Tensor) and d.is_floating_point() and
                 wt.is_floating_point() and d.device == wt.device == flows.forward.device and
-                tuple(d.shape) == (1, f, h, w) and tuple(wt.shape) == (1, f - 1, h, w))
+                tuple(d.shape) == (b, f, h, w) and tuple(wt.shape) == (b, f - 1, h, w))
 
     def _fused_params(self, global_step: int, inputs=None):
         """Tensors that receive a gradient from the fused step, in the order of FusedStep's buffers:
@@ -307,7 +311,11 @@ class Model(nn.Module):
 
     def _fused_engine(self, batch: Batch, flows: Flows, tracks, flow_loss):
         """The FusedOverfitter bound to this model's parameters for (flows, tracks); built on first
-        use, re-pointed when the Flows tensors change, None if the configuration is not covered."""
+        use, re-pointed when the Flows tensors change, None if the configuration is not covered.  A batch of
+        several videos with tracks is not (loss_tracking.py serves one video): the whole step then runs per-op,
+        as the flow loss must not run fused while the tracking loss reads a detached snapshot."""
+        if batch.videos.shape[0] > 1 and tracks is not None:
+            return None
         from .overfit import FusedOverfitter, OverfitCfg
         mc, bc, ic, ec = self.cfg, self.cfg.backbone, self.cfg.intrinsics, self.cfg.extrinsics
         lm = flow_loss.cfg.mapping

@@ -176,7 +176,8 @@ class FusedOverfitter(Overfitter):
     (T, H, W) / (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs
     [fo_b - b, fo_b - b + F_b - 1); `models[b]` is video b's Model, whose parameters are views into them.
     `tracks` is then a list of B segment lists, and the metrics log holds (steps, B) values.  Several
-    videos do not serve the splat plan, pair sharding or the split-step surface.  Two forms:
+    videos do not serve the splat plan, pair sharding or the split-step surface (but for a network Model's
+    batch, below).  Two forms:
 
     - `batch.videos` of shape (B, F, 3, H, W) with B > 1 and Flows of shape (B, F-1, ...): videos of one
       length, whose packed buffers are the (B, F, ...) / (B, F-1, ...) tensors.  training_step(),
@@ -190,6 +191,12 @@ class FusedOverfitter(Overfitter):
     surface of flowmap_b200.fused), the optimiser owns no depth or weight buffers and no Adam state for
     them: every step's depths and weights come from the network, through forward_phase, and only the
     split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight).
+    Such a Model also takes a tensor batch of B > 1 videos of F frames (the reference's pretraining step:
+    softmin intrinsics without a regression stage, no tracks): the packed layout with F_b = F, whose rows are
+    the network's (B, F, H, W) depths and (B, F-1, H, W) weights and the caller's (B, F-1, ...) Flows, which
+    set_flows re-points to rather than copies.  Its mask_sum holds the pooled normaliser of LossFlow at b > 1
+    in every video's slot, so that the (B,) losses sum to the batch's loss, and backward_phase takes one
+    flow_scale for the whole batch.
 
     cfg.intrinsics "ground_truth" (intrinsics_ground_truth.py, calibrated data) takes K as given: from
     `batch.intrinsics` (1, F, 3, 3), (B, F, 3, 3) for a tensor batch, or each Batch's own for a list, normalised
@@ -205,6 +212,9 @@ class FusedOverfitter(Overfitter):
             raise ValueError("flowmap_b200: the splat plan does not serve ground-truth intrinsics")
         if isinstance(batch, (list, tuple)):
             self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
+        elif batch.videos.shape[0] > 1 and isinstance(model, Model) and \
+                not isinstance(model.backbone, BackboneExplicitDepth):
+            self._init_network_videos(cfg, batch, flows, tracks, use_splat_plan, model)
         elif batch.videos.shape[0] > 1:
             b, f = batch.videos.shape[:2]
             if model is not None:
@@ -226,7 +236,7 @@ class FusedOverfitter(Overfitter):
         if self._gt:
             self.set_intrinsics(self.batch.intrinsics if self._layout is None or self._tensor_batch
                                 else [bt.intrinsics for bt in self.batches])
-        if self._tensor_batch:  # the parameters as (B, F, ...) / (B, F-1, ...) views of the packed buffers
+        if self._tensor_batch and not self._network:  # the parameters as (B, F, ...) / (B, F-1, ...) views
             self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
 
     def _init_one(self, cfg, batch, flows, tracks, device, use_splat_plan, model):
@@ -338,6 +348,49 @@ class FusedOverfitter(Overfitter):
         self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
         self._msum = self._video_mask_sums(self.flows)
 
+    def _init_network_videos(self, cfg, batch, flows, tracks, use_splat_plan, model):
+        """A network Model's tensor batch of several videos (see the class docstring): no parameter buffers,
+        one focal length per video from the softmin sweep."""
+        from ._lib import VideoLayout, lib
+        import ctypes
+        if use_splat_plan:
+            raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
+        if tracks is not None or cfg.use_tracking:
+            raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
+        if cfg.intrinsics != "softmin" or cfg.regression_after is not None:
+            raise ValueError("flowmap_b200: a network backbone's batch of several videos needs softmin intrinsics "
+                             "without a regression stage (one focal length per video)")
+        B, f, _, h, w = batch.videos.shape
+        dev = flows.forward.device
+        self.cfg, self.model, self.models, self.losses, self.optimizer = cfg, model, [model], None, None
+        self.B, self.frames, self.T, self.P = B, [f] * B, B * f, B * (f - 1)
+        self._first = [i * f for i in range(B)]
+        self._hw, self._lead, self._track_frames = (h, w), ((self.T,), (self.P,), (B,)), self.frames
+        self.batch, self.tracks = batch, None
+        self.global_step = self.optimizer_steps = self.focal_steps = 0
+        self._network, self._tensor_batch, self._depth, self._wlog = True, True, None, None
+        self.flows = self._network_flows(flows, dev)
+        self._tables = video_tables(self.frames, dev)
+        self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
+        self._layout_ref = ctypes.byref(self._layout)
+        self._use_plan, self._plan = False, None
+        self._focal = torch.zeros(B, device=dev)
+        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
+        self._msum = self._mask_sum(self.flows).expand(B).contiguous()
+
+    def _network_flows(self, flows: Flows, device) -> Flows:
+        """A network batch's (B, F-1, ...) Flows as the packed (P, ...) rows: views of the caller's tensors
+        (copies only of tensors that are not contiguous)."""
+        want = (self.B, self.frames[0] - 1, *self._hw)
+        rows = []
+        for name in _FLOW_NAMES:
+            t = ops._canon(getattr(flows, name), name)
+            shape = want + (2,) if name in ("forward", "backward") else want
+            if tuple(t.shape) != shape or t.device != device:
+                raise ValueError(f"flowmap_b200: flows.{name} must be a {shape} tensor on {device}")
+            rows.append(t.flatten(0, 1))
+        return Flows(*rows)
+
     def _init_step(self, cfg):
         """What one video and packed videos wire alike: the softmin buffers, the Adam state, the gradient
         and output buffers, the args struct, the step clock and the tracking buffers."""
@@ -442,8 +495,10 @@ class FusedOverfitter(Overfitter):
         prefetching loader) without rebuilding parameters or optimiser state.  `mask_sum` is the
         flow-loss normaliser (loss_flow.py:70) if the caller already has it.  Several videos: the new
         flows are copied into the packed buffers, from one (B, F-1, ...) Flows for a tensor batch, else
-        from a list of one Flows per video."""
-        if self._layout is not None:
+        from a list of one Flows per video.  A network backbone's batch of several videos: the step reads the
+        new (B, F-1, ...) Flows themselves, and `mask_sum` (default: the pooled sum of all their masks) goes
+        to every video."""
+        if self._layout is not None and not self._network:
             if self._tensor_batch and isinstance(flows, Flows):
                 flows = [_video(flows, i) for i in range(flows.forward.shape[0])]
             if not isinstance(flows, (list, tuple)) or len(flows) != self.B:
@@ -458,13 +513,16 @@ class FusedOverfitter(Overfitter):
             self._msum.copy_(self._video_mask_sums(self.flows) if mask_sum is None else mask_sum)
             return
         old = self.flows
-        canon = {}
-        for name in _FLOW_NAMES:
-            t = ops._canon(getattr(flows, name), name)
-            if t.shape != getattr(old, name).shape or t.device != getattr(old, name).device:
-                raise ValueError(f"flowmap_b200: `{name}` does not match the optimiser's shapes / device")
-            canon[name] = t
-        flows = Flows(canon["forward"], canon["backward"], canon["forward_mask"], canon["backward_mask"])
+        if self._layout is not None:
+            flows = self._network_flows(flows, old.forward.device)
+        else:
+            canon = {}
+            for name in _FLOW_NAMES:
+                t = ops._canon(getattr(flows, name), name)
+                if t.shape != getattr(old, name).shape or t.device != getattr(old, name).device:
+                    raise ValueError(f"flowmap_b200: `{name}` does not match the optimiser's shapes / device")
+                canon[name] = t
+            flows = Flows(canon["forward"], canon["backward"], canon["forward_mask"], canon["backward_mask"])
         self.flows = flows  # the canonical tensors stay referenced while the kernels hold their pointers
         a = self._args
         a.fflow, a.bflow = flows.forward.data_ptr(), flows.backward.data_ptr()
@@ -655,13 +713,14 @@ class FusedOverfitter(Overfitter):
                       weights: Optional[Tensor] = None):
         """Poses + flow loss with its direct gradients (fm_overfit_step, FM_STEP_FORWARD; the
         candidate sweep first in the softmin stage).  Returns the weighted flow loss (device scalar,
-        a buffer that the next call overwrites).  Bound to a network backbone, `depth` (1, F, H, W) and,
-        with correspondence weights, `weights` (1, F-1, H, W) are the step's contiguous float32 inputs;
-        they stay referenced until the next call (backward_phase reads them)."""
-        from ._lib import check
-        self._refuse_videos("the split-step surface")
-        a, L = self._args, self._lib
-        _, f, _, h, w = self.batch.videos.shape
+        a buffer that the next call overwrites; (B,) per-video losses for a network's batch of B videos).
+        Bound to a network backbone, `depth` (B, F, H, W) and, with correspondence weights, `weights`
+        (B, F-1, H, W) are the step's contiguous float32 inputs (B = 1 but for a network's batch); they stay
+        referenced until the next call (backward_phase reads them)."""
+        if not self._network:
+            self._refuse_videos("the split-step surface")
+        a = self._args
+        f, (h, w) = self.frames[0], self._hw
         if self._network:
             self._bind_inputs(depth, weights, f, h, w)
         elif depth is not None or weights is not None:
@@ -684,15 +743,15 @@ class FusedOverfitter(Overfitter):
                 a.focal = _ptr(self._focal)
             a.phase = 1  # FM_STEP_FORWARD
             try:
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (forward)")
+                self._call_step("fm_overfit_step (forward)")
             finally:
                 a.phase = 0
         return self._loss
 
     def _bind_inputs(self, depth, weights, f, h, w):
         """Point the step at a network backbone's depths / weights of this step."""
-        use_w = self.cfg.use_correspondence_weights
-        for name, t, shape in (("depth", depth, (1, f, h, w)), ("weights", weights if use_w else None, (1, f - 1, h, w))):
+        use_w, b = self.cfg.use_correspondence_weights, self.B
+        for name, t, shape in (("depth", depth, (b, f, h, w)), ("weights", weights if use_w else None, (b, f - 1, h, w))):
             if t is None and (name == "depth" or use_w):
                 raise ValueError(f"flowmap_b200: a network backbone's step needs its `{name}`")
             if t is not None and (tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()
@@ -721,11 +780,11 @@ class FusedOverfitter(Overfitter):
 
     def backward_phase(self, flow_scale=None, track_scale=None, with_tracking: bool = False):
         """Second half: [tracking backward,] Procrustes backward, focal gradient[, the sweep's
-        backward].  flow_scale / track_scale: device float scalars d total / d loss (None = 1).
-        Leaves the gradients in gradients()."""
-        from ._lib import check
-        self._refuse_videos("the split-step surface")
-        a, L = self._args, self._lib
+        backward].  flow_scale / track_scale: device float scalars d total / d loss (None = 1); a network's
+        batch of videos takes one flow_scale for all of them.  Leaves the gradients in gradients()."""
+        if not self._network:
+            self._refuse_videos("the split-step surface")
+        a = self._args
         st = torch.cuda.current_stream().cuda_stream
         a.tracks = self._ctypes.pointer(self._pk_c) if with_tracking else None
         a.flow_grad_scale, a.track_grad_scale = _ptr(flow_scale), _ptr(track_scale)
@@ -737,7 +796,7 @@ class FusedOverfitter(Overfitter):
             a.g_rt = a.track_g_k4 = None
         with torch.cuda.device(self.rt.device):
             try:
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (backward)")
+                self._call_step("fm_overfit_step (backward)")
             finally:
                 a.phase, a.tracks, a.flow_grad_scale, a.track_grad_scale = 0, None, None, None
                 a.g_rt, a.track_g_k4 = kept

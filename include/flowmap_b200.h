@@ -406,8 +406,15 @@ typedef struct {
  * segments of video b carry start frames frame_offset[b] + s (they never cross videos); track_ws is
  * fm_track_workspace_bytes(T, total_samples).  Metrics: gt_positions (T, 3), NaN first position of a
  * video = no ground truth; the ring is (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).
- * Needs phase FM_STEP_ALL and no splat plan, and refuses defer_adam = 1 together with step > 0 and weight
- * logits (the caller updates the logits after the sweep's backward). */
+ * Needs no splat plan, and refuses defer_adam = 1 together with step > 0 and weight logits (the caller
+ * updates the logits after the sweep's backward).
+ * Phases: FM_STEP_ALL, or the two halves of a split step, FM_STEP_FORWARD then FM_STEP_BACKWARD (a network
+ * backbone's batch, whose depths / weights come from the network and whose update the caller owns).  A
+ * split step needs step = 0, defer_adam = 0, tracks == NULL and metrics_log == NULL.  Its flow_grad_scale is
+ * ONE device scalar for the whole batch, d total / d loss_b for every video b: the sum of the B losses is the
+ * objective.  The reference's LossFlow at b > 1 (pretraining) is such a sum when every mask_sum[b] holds the
+ * pooled normaliser M = sum over all videos of their forward + backward mask sums ("or 1"): loss[b] is then
+ * weight * S_b / M and sum_b loss[b] the pooled loss. */
 int fm_overfit_step_videos(const fm_overfit_step_args* args, const fm_video_layout* layout, void* stream);
 size_t fm_workspace_bytes_videos(int B, int T);
 /* fm_procrustes_moments for packed videos (see fm_overfit_step_args.moments_k4). */
