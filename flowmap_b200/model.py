@@ -346,7 +346,10 @@ class Model(nn.Module):
             object.__setattr__(self, "_engine_key", key)
             object.__setattr__(self, "_engine_flows", None)
         cur = (flows.forward, flows.backward, flows.forward_mask, flows.backward_mask)
-        if self._engine_flows is None or any(a is not b for a, b in zip(cur, self._engine_flows)):
+        # the step reads contiguous Flows tensors themselves, and contiguous copies of the others: a copy is
+        # taken again every step, as a loader may have rewritten the tensor behind the same view
+        if (self._engine_flows is None or any(a is not b for a, b in zip(cur, self._engine_flows)) or
+                not all(t.is_contiguous() for t in cur)):
             eng.set_flows(flows, mask_sum=flow_loss._mask_total(flows))
             object.__setattr__(self, "_engine_flows", cur)
         return eng
