@@ -34,13 +34,6 @@ SIGNATURES = {
     "fm_procrustes_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "fm_procrustes_bwd": (c_int, [_P, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, _P, _P, _P,
                                   c_int, c_int, c_int, c_int, _P]),
-    "fm_splat_plan_bytes": (c_size_t, [c_int, c_int, c_int]),
-    "fm_splat_plan_build": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
-    "fm_splat_plan_info": (c_int, [_P, ctypes.POINTER(c_int), ctypes.POINTER(ctypes.c_uint),
-                                   ctypes.POINTER(ctypes.c_ulonglong), _P]),
-    "fm_procrustes_fwd_planned": (c_int, [_P, _P, _P, _P, c_float, _P, _P, _P, c_int, c_int, c_int, _P]),
-    "fm_procrustes_bwd_planned": (c_int, [_P, _P, _P, _P, c_float, _P, ctypes.c_uint, _P, c_int, _P, _P, _P, _P,
-                                          c_int, c_int, c_int, _P]),
     "fm_procrustes_moments": (c_int, [_P, _P, _P, _P, c_float, _P, c_int, c_int, c_int, _P]),
     "fm_mask_sum": (c_int, [_P, _P, _P, c_size_t, _P]),
     "fm_flow_loss_fwd_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_float, c_float, c_int,
@@ -104,7 +97,7 @@ class OverfitStepArgs(ctypes.Structure):
                 ("extrinsics", _P), ("g_extrinsics", _P), ("g_rt", _P), ("track_g_k4", _P),
                 ("track_loss", _P),
                 ("ws", _P), ("track_ws", _P), ("focal_step", c_int), ("defer_adam", c_int),
-                ("phase", c_int), ("splat_plan", _P), ("splat_overflow_max", ctypes.c_uint),
+                ("phase", c_int),
                 ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P),
                 ("gt_positions", _P), ("gt_fx", c_float), ("gt_fy", c_float), ("metrics_log", _P),
                 ("metrics_capacity", c_int), ("B", c_int), ("gt_fxfy", _P)]

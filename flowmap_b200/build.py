@@ -8,7 +8,7 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 SOURCES = ["fm_kernels.cu", "fm_io.cu"]
-HEADERS = ["fm_math.cuh", "fm_procrustes.cuh", "fm_ate.cuh", "fm_pixel.cuh", "fm_tiled.cuh", "fm_host.h"]
+HEADERS = ["fm_math.cuh", "fm_procrustes.cuh", "fm_ate.cuh", "fm_pixel.cuh", "fm_host.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 

@@ -255,13 +255,6 @@ __device__ __forceinline__ const float* opaque_ptr(const float* p) {
   return p;
 }
 
-// Same for a 32-bit value (a shared-space base address the compiler would otherwise re-derive from
-// %cluster_ctarank at every use).
-__device__ __forceinline__ unsigned opaque_u32(unsigned v) {
-  asm volatile("" : "+r"(v));
-  return v;
-}
-
 // Software prefetch into L2 (no register, no scoreboard): streaming operands are requested a couple
 // of chunks ahead so that the demand loads find them on chip.
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
@@ -931,16 +924,10 @@ __global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __r
 }
 
 // ================================================================== phase D1: adjoint solve
-// focal_moments != NULL (tiled path, all frames share one focal length): the pair's Procrustes part
-// of d loss / d focal is taken from the moment sums (fm_procrustes.cuh) and booked as the
-// equivalent d/dfx of the pair's earlier frame in k4acc -- the per-pixel kernels carry no
-// intrinsics accumulators at all.
 template <class Lay>
 __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* __restrict__ state,
                           const float* __restrict__ g_rt, int include_flow,
-                          const float* __restrict__ flow_scale, PairAdjoint* __restrict__ adj, int BP,
-                          Lay lay, const double* __restrict__ focal_moments = nullptr,
-                          const float* __restrict__ k4 = nullptr, double* __restrict__ k4acc = nullptr) {
+                          const float* __restrict__ flow_scale, PairAdjoint* __restrict__ adj, int BP, Lay lay) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   double g[12];
@@ -952,15 +939,7 @@ __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* _
   }
   if (g_rt) for (int k = 0; k < 12; ++k) g[k] += (double)g_rt[(size_t)pair * 12 + k];
   PairAdjoint out;
-  if (focal_moments) {
-    double dbl[15];
-    procrustes_adjoint(state[pair], g, out, dbl);
-    const int a = pair + lay.of_pair(pair);
-    const double fdf = procrustes_focal_log_grad(state[pair], focal_moments + (size_t)pair * kNumMoments, dbl);
-    k4acc[(size_t)a * 4] = fdf / (double)k4[(size_t)a * 4];  // f dL/df = fx dL/dfx
-  } else {
-    procrustes_adjoint(state[pair], g, out);
-  }
+  procrustes_adjoint(state[pair], g, out);
   adj[pair] = out;
 }
 
@@ -1320,8 +1299,6 @@ k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, i
   }
 }
 #undef FM_DISTRIBUTE_DENSE_PARAMS
-
-#include "fm_tiled.cuh"
 
 template <class Lay>
 __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
@@ -2821,112 +2798,6 @@ Uniform frames_of(const PairLayout& l) { return Uniform{l.F}; }
 const Videos& frames_of(const RaggedPairs& l) { return l.v; }
 PairLayout pairs_of(const Uniform& u, int H, int W) { return dense_layout(u.F, H, W); }
 RaggedPairs pairs_of(const Videos& v, int, int) { return RaggedPairs{v}; }
-}  // namespace
-
-// ---------------------------------------------------------------- tiled path: host side
-namespace {
-typedef CUresult (*TensorMapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                      CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                      CUtensorMapFloatOOBfill);
-TensorMapEncodeFn tensor_map_encoder() {
-  static const TensorMapEncodeFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    return (TensorMapEncodeFn)p;
-  }();
-  return fn;
-}
-
-// (W, H, frames) float32 tensor, box = one (kWX x kWY x 1) window; out-of-range parts read as 0.
-int make_window_map(CUtensorMap* m, const float* base, int W, int H, int frames) {
-  const TensorMapEncodeFn enc = tensor_map_encoder();
-  if (!enc) return fail_msg("tiled path: cuTensorMapEncodeTiled is not available from this driver");
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)frames};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4ull, (cuuint64_t)W * (cuuint64_t)H * 4ull};
-  const cuuint32_t box[3] = {(cuuint32_t)tiled::kWX, (cuuint32_t)tiled::kWY, 1u};
-  const cuuint32_t estr[3] = {1u, 1u, 1u};
-  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char msg[128];
-    snprintf(msg, sizeof(msg), "tiled path: cuTensorMapEncodeTiled failed (CUresult %d) for %d x %d x %d", (int)r, W, H, frames);
-    return fail_msg(msg);
-  }
-  return 0;
-}
-
-int sm_count() {
-  static const int n = [] {
-    int dev = 0, v = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1)
-      v = 132;
-    return v;
-  }();
-  return n;
-}
-
-bool tiled_shape_ok(int F, int H, int W) { return F >= 2 && W % 4 == 0 && H >= 1 && W < 32768 && H < 32768; }
-
-// Phase A through the plan: moments of all pairs (+ the step's correspondence weights into the
-// plan's scratch for phase D), then the solve.
-int launch_moments_tiled(const float* depth, const float* k4, const float* bflow, const float* weights, float wsens,
-                         const tiled::Plan& pl, double* moments, const float* zshift, int F, int H, int W,
-                         cudaStream_t s) {
-  CUtensorMap tm;
-  int rc = make_window_map(&tm, depth, W, H, F);
-  if (rc) return rc;
-  tiled::MomArgs b;
-  b.depth = depth; b.k4 = k4; b.bflow = bflow; b.weights = weights; b.wscratch = pl.wscratch; b.moments = moments;
-  b.zshift = zshift;
-  b.tinfo = pl.tiles; b.wsens = wsens; b.F = F; b.H = H; b.W = W; b.tiles_x = pl.tiles_x;
-  b.tiles = pl.tiles_x * pl.tiles_y; b.n_items = (F - 1) * b.tiles;
-  int grid = sm_count() * 3;
-  if (grid > b.n_items) grid = b.n_items;
-  static const cudaError_t at1 = cudaFuncSetAttribute(tiled::k_moments_tiled<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tiled::kMomSmem);
-  static const cudaError_t at0 = cudaFuncSetAttribute(tiled::k_moments_tiled<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tiled::kMomSmem);
-  if (at1 != cudaSuccess || at0 != cudaSuccess) return fail("k_moments_tiled: shared memory attribute", at1 != cudaSuccess ? at1 : at0);
-  if (weights) tiled::k_moments_tiled<true><<<grid, tiled::kT, tiled::kMomSmem, s>>>(tm, b);
-  else tiled::k_moments_tiled<false><<<grid, tiled::kT, tiled::kMomSmem, s>>>(tm, b);
-  FM_CHECK_LAUNCH("k_moments_tiled");
-  return 0;
-}
-
-// Phase D2 through the plan: transposed (gather-form) bilinear splat + per-pixel adjoints + final depth
-// gradient in one pass; flow outliers afterwards as REDs.
-int launch_backward_tiled(const float* depth, const float* k4, const float* bflow, float* weights, float wsens,
-                          const tiled::Plan& pl, unsigned ovf_max, const PairAdjoint* adj, float* g_depth,
-                          float* g_weights, const AdamFuse& af, int F, int H, int W, cudaStream_t s) {
-  CUtensorMap tm_d, tm_w;
-  int rc = make_window_map(&tm_d, depth, W, H, F);
-  if (rc) return rc;
-  if ((rc = make_window_map(&tm_w, pl.wscratch, W, H, F - 1))) return rc;
-  tiled::BwdArgs b;
-  b.depth = depth; b.k4 = k4; b.bflow = bflow; b.weights = weights; b.adj = adj; b.tinfo = pl.tiles;
-  b.perm = pl.perm; b.entries = pl.entries; b.g_depth = g_depth; b.g_weights = g_weights; b.adam = af;
-  b.wsens = wsens; b.F = F; b.H = H; b.W = W; b.tiles_x = pl.tiles_x; b.tiles = pl.tiles_x * pl.tiles_y;
-  b.n_items = F * b.tiles;
-  int grid = sm_count() * 2;
-  if (grid > b.n_items) grid = b.n_items;
-  static const cudaError_t at1 = cudaFuncSetAttribute(tiled::k_backward_tiled<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tiled::kBwdSmem);
-  static const cudaError_t at0 = cudaFuncSetAttribute(tiled::k_backward_tiled<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tiled::kBwdSmem);
-  if (at1 != cudaSuccess || at0 != cudaSuccess) return fail("k_backward_tiled: shared memory attribute", at1 != cudaSuccess ? at1 : at0);
-  if (weights) tiled::k_backward_tiled<true><<<grid, tiled::kT, tiled::kBwdSmem, s>>>(tm_d, tm_w, b);
-  else tiled::k_backward_tiled<false><<<grid, tiled::kT, tiled::kBwdSmem, s>>>(tm_d, tm_w, b);
-  FM_CHECK_LAUNCH("k_backward_tiled");
-  if (ovf_max > 0u) {
-    const unsigned n = ovf_max < (unsigned)pl.ovf_cap ? ovf_max : (unsigned)pl.ovf_cap;
-    dim3 g2((n + 255u) / 256u, F - 1);
-    tiled::k_backward_overflow<<<g2, 256, 0, s>>>(depth, k4, weights ? pl.wscratch : nullptr, adj, pl.ovf_count, pl.ovf,
-                                                  pl.ovf_cap, g_depth, H, W);
-    FM_CHECK_LAUNCH("k_backward_overflow");
-  }
-  return 0;
-}
 
 // The Procrustes forward of B videos with T frames (T - B pairs) in all, laid out as `lay`: dense_layout
 // for one video or a uniform batch, RaggedPairs for packed videos of different lengths.  Pair shift,
@@ -3023,61 +2894,6 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
   return 0;
 }
 
-// The splat plan's Procrustes forward and backward (fm_tiled.cuh): one video, all pixels, W % 4 == 0.
-int procrustes_fwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                           float wsens, void* plan, float* rt, void* ws, int F, int H, int W, cudaStream_t s) {
-  if (!depth || !k4 || !backward_flow || !rt || !ws || bad_dims(1, F, H, W))
-    return fail_msg("fm_procrustes_fwd: bad arguments");
-  if (!tiled_shape_ok(F, H, W))
-    return fail_msg("fm_procrustes_fwd: the splat plan serves the dense single-video path with W % 4 == 0");
-  const int BP = F - 1;
-  const PairLayout lay = dense_layout(F, H, W);
-  Workspace w = carve(ws, 1, F);
-  cudaError_t e = cudaMemsetAsync(w.moments, 0, (size_t)BP * kNumMoments * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_fwd: memset", e);
-  k_pair_shift<<<BP, kThreads, 0, s>>>(depth, weights, wsens, w.zshift, lay, H, W);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_pair_shift");
-  const int rc = launch_moments_tiled(depth, k4, backward_flow, weights, wsens, tiled::plan_carve(plan, F, H, W),
-                                      w.moments, w.zshift, F, H, W, s);
-  if (rc) return rc;
-  k_solve<<<(BP + 63) / 64, 64, 0, s>>>(w.moments, w.zshift, rt, w.state, BP, lay, H, W, nullptr, nullptr);
-  FM_CHECK_LAUNCH("fm_procrustes_fwd: k_solve");
-  return 0;
-}
-
-// The caller scales the direct depth gradient in g_depth: flow_scale only scales the flow loss's pose and
-// K gradients here.
-int procrustes_bwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                           float wsens, void* plan, unsigned plan_ovf_max, const float* g_rt, int include_flow_loss,
-                           const float* flow_scale, float* g_depth, float* g_weights, float* g_k4, void* ws, int F,
-                           int H, int W, cudaStream_t s, const AdamFuse* adam) {
-  if (!tiled_shape_ok(F, H, W))
-    return fail_msg("fm_procrustes_bwd: the splat plan serves the dense single-video path with W % 4 == 0");
-  if (!g_k4) return fail_msg("fm_procrustes_bwd: the splat plan always computes the intrinsics gradient (g_k4)");
-  if (!depth || !k4 || !backward_flow || !g_depth || !g_k4 || !ws || bad_dims(1, F, H, W))
-    return fail_msg("fm_procrustes_bwd: bad arguments");
-  if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
-  const int BP = F - 1;
-  Workspace w = carve(ws, 1, F);
-  cudaError_t e = cudaMemsetAsync(w.k4acc, 0, (size_t)F * 4 * sizeof(double), s);
-  if (e != cudaSuccess) return fail("fm_procrustes_bwd: memset", e);
-  AdamFuse af;
-  if (adam) af = *adam; else memset(&af, 0, sizeof(af));
-  // one focal length shared by all frames (or constant intrinsics): the Procrustes part of the
-  // intrinsics gradient comes from the moment sums, the pixel kernel carries no K accumulators
-  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP,
-                                          Uniform{F}, w.moments, k4, w.k4acc);
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
-  const int rc = launch_backward_tiled(depth, k4, backward_flow, const_cast<float*>(weights), wsens,
-                                       tiled::plan_carve(plan, F, H, W), plan_ovf_max, w.adj, g_depth, g_weights, af,
-                                       F, H, W, s);
-  if (rc) return rc;
-  k_k4_finalize<<<(F + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, F,
-                                                Uniform{F});
-  FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
-  return 0;
-}
-
 PairLayout sweep_layout(int F, int H, int W, int cand) {
   PairLayout l = dense_layout(F, H, W);  // strides of the REAL tensors
   l.F = 2;                               // the sweep only sees frames 0 and 1 (pair 0)
@@ -3170,7 +2986,7 @@ int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensit
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 105; }
+int fm_version(void) { return 106; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -3245,78 +3061,6 @@ int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward
   return procrustes_bwd(depth, k4, backward_flow, weights, 0.f, indices, num_indices, g_rt, include_flow_loss,
                         flow_scale, g_depth, g_weights, g_k4, ws, B, B * F, dense_layout(F, H, W), H, W,
                         (cudaStream_t)stream, nullptr, /*depth_prescaled=*/false);
-}
-
-size_t fm_splat_plan_bytes(int F, int H, int W) {
-  if (!tiled_shape_ok(F, H, W) || (long long)H * W > (1ll << 30)) return 0;
-  return tiled::plan_carve(nullptr, F, H, W).bytes;
-}
-
-int fm_splat_plan_build(const float* backward_flow, void* plan, int F, int H, int W, void* stream) {
-  if (!backward_flow || !plan || !tiled_shape_ok(F, H, W) || bad_dims(1, F, H, W))
-    return fail_msg("fm_splat_plan_build: bad arguments (needs F >= 2 and W % 4 == 0)");
-  cudaStream_t s = (cudaStream_t)stream;
-  const tiled::Plan pl = tiled::plan_carve(plan, F, H, W);
-  const int P = F - 1, tiles = pl.tiles_x * pl.tiles_y;
-  const size_t N = (size_t)H * W;
-  cudaError_t e;
-  if ((e = cudaMemsetAsync(pl.count, 0, (size_t)P * N * sizeof(unsigned), s)) != cudaSuccess ||
-      (e = cudaMemsetAsync(pl.tile_sum, 0, (size_t)P * tiles * sizeof(int4), s)) != cudaSuccess ||
-      (e = cudaMemsetAsync(pl.ovf_count, 0, (size_t)P * sizeof(unsigned), s)) != cudaSuccess)
-    return fail("fm_splat_plan_build: memset", e);
-  tiled::k_plan_init<<<1, 1, 0, s>>>(pl.hdr, F, H, W, pl.tiles_x, pl.tiles_y, pl.ovf_cap, (unsigned long long)pl.entry_capacity);
-  FM_CHECK_LAUNCH("k_plan_init");
-  int nb = (int)((N + 255) / 256);
-  if (nb > 1024) nb = 1024;
-  tiled::k_plan_count<<<dim3(nb, P), 256, 0, s>>>(backward_flow, pl.count, pl.tile_sum, H, W, pl.tiles_x, tiles);
-  FM_CHECK_LAUNCH("k_plan_count");
-  tiled::k_plan_sort<<<dim3(tiles, P), tiled::kT, 0, s>>>(backward_flow, pl.count, pl.tile_sum, pl.tiles, pl.perm, pl.slot_of,
-                                                           pl.tile_total, pl.hdr, H, W, pl.tiles_x, tiles);
-  FM_CHECK_LAUNCH("k_plan_sort");
-  tiled::k_plan_scan<<<1, 1024, 0, s>>>(pl.tile_total, pl.tiles, pl.hdr, P * tiles, (unsigned long long)pl.entry_capacity);
-  FM_CHECK_LAUNCH("k_plan_scan");
-  if ((e = cudaMemsetAsync(pl.count, 0, (size_t)P * N * sizeof(unsigned), s)) != cudaSuccess)
-    return fail("fm_splat_plan_build: memset", e);
-  tiled::k_plan_fill<<<dim3(nb, P), 256, 0, s>>>(backward_flow, pl.tiles, pl.slot_of, pl.count, pl.entries, pl.ovf_count, pl.ovf,
-                                                 pl.hdr, H, W, pl.tiles_x, tiles, (unsigned long long)pl.entry_capacity, pl.ovf_cap);
-  FM_CHECK_LAUNCH("k_plan_fill");
-  const size_t slots = (size_t)P * tiles * tiled::kCells;
-  tiled::k_plan_canon<<<(unsigned)((slots + 255) / 256), 256, 0, s>>>(pl.tiles, pl.perm, pl.count, pl.entries, pl.ovf_count, pl.hdr,
-                                                                     H, W, pl.tiles_x, tiles, P, (unsigned long long)pl.entry_capacity);
-  FM_CHECK_LAUNCH("k_plan_canon");
-  return 0;
-}
-
-int fm_splat_plan_info(const void* plan, int* status, unsigned* overflow_max, unsigned long long* total_entries,
-                       void* stream) {
-  if (!plan) return fail_msg("fm_splat_plan_info: bad arguments");
-  tiled::PlanHeader h;
-  cudaError_t e = cudaMemcpyAsync(&h, plan, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
-  if (e != cudaSuccess) return fail("fm_splat_plan_info", e);
-  if (h.magic != tiled::kPlanMagic) return fail_msg("fm_splat_plan_info: not a splat plan");
-  if (status) *status = h.status;
-  if (overflow_max) *overflow_max = h.ovf_max;
-  if (total_entries) *total_entries = h.total_entries;
-  return 0;
-}
-
-int fm_procrustes_fwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                              float weight_sensitivity, void* plan, float* rt, void* ws, int F, int H, int W,
-                              void* stream) {
-  if (!plan) return fail_msg("fm_procrustes_fwd_planned: plan missing");
-  return procrustes_fwd_planned(depth, k4, backward_flow, weights, weight_sensitivity, plan, rt, ws, F, H, W,
-                                (cudaStream_t)stream);
-}
-
-int fm_procrustes_bwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                              float weight_sensitivity, void* plan, unsigned plan_overflow_max, const float* g_rt,
-                              int include_flow_loss, float* g_depth, float* g_weights, float* g_k4, void* ws, int F,
-                              int H, int W, void* stream) {
-  if (!plan) return fail_msg("fm_procrustes_bwd_planned: plan missing");
-  return procrustes_bwd_planned(depth, k4, backward_flow, weights, weight_sensitivity, plan, plan_overflow_max, g_rt,
-                                include_flow_loss, nullptr, g_depth, g_weights, g_k4, ws, F, H, W,
-                                (cudaStream_t)stream, nullptr);
 }
 
 int fm_mask_sum(const float* forward_mask, const float* backward_mask, double* out, size_t count, void* stream) {
@@ -3786,7 +3530,6 @@ const char* step_refusal(const fm_overfit_step_args* a, const Uniform&) {
                   : nullptr;
 }
 const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
-  if (a->splat_plan) return "fm_overfit_step_videos: serves steps without a splat plan";
   // The split phases serve a network backbone's batch (pretraining): the caller owns the update, and the
   // tracking kernels of packed videos take no d total / d tracking loss (TrackVideos::Scale is NoScale).
   if (a->phase != FM_STEP_ALL) {
@@ -3862,13 +3605,10 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   int rc;
   cudaError_t e;
   if (a->phase < FM_STEP_ALL || a->phase > FM_STEP_BACKWARD) return fail_msg("fm_overfit_step: unknown phase");
-  // the splat plan of this video's backward flows serves the dense path (all-pixel Procrustes)
-  void* plan = (a->splat_plan && !a->indices && tiled_shape_ok(T, H, W)) ? a->splat_plan : nullptr;
   // g_k4 == NULL: constant intrinsics (ground truth), the backward computes no intrinsics gradient
   const bool kgrad = a->g_k4 != nullptr;
   if (!kgrad && (a->focal || a->track_g_k4))
     return fail_msg("fm_overfit_step: g_k4 == NULL (constant intrinsics) needs focal == NULL and track_g_k4 == NULL");
-  if (!kgrad && plan) return fail_msg("fm_overfit_step: the splat plan does not serve constant intrinsics (g_k4 == NULL)");
   // intrinsics from the focal parameter (regressed stage) or as given
   float* k4 = a->k4;
   if (a->phase != FM_STEP_BACKWARD) {
@@ -3877,11 +3617,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       FM_CHECK_LAUNCH("fm_overfit_step: k_k4_from_focal");
     }
     // Model.forward: Procrustes poses (model.py:54-90)
-    if ((rc = plan ? procrustes_fwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
-                                            a->rt, a->ws, T, H, W, s)
-                   : procrustes_fwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
-                                    a->num_indices, a->rt, a->ws, B, T, pairs, H, W, s,
-                                    a->indices ? nullptr : a->moments_k4, /*solve=*/true)))
+    if ((rc = procrustes_fwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                             a->num_indices, a->rt, a->ws, B, T, pairs, H, W, s,
+                             a->indices ? nullptr : a->moments_k4, /*solve=*/true)))
       return rc;
     // The flow loss and the tracking sweep both need only the poses: with tracking on they run as
     // two branches of the step (the tracking sweep is issue-bound, the flow kernel waits on memory:
@@ -3958,9 +3696,8 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   SideLane* lane = nullptr;  // carries the tracking loss's depth scatter while the Procrustes backward runs
   if (a->tracks) {
     const fm_packed_tracks* t = a->tracks;
-    // REDs into g_depth commute with those of k_distribute; the splat-plan backward instead rewrites
-    // g_depth with plain stores, so there the scatter stays in stream order
-    if (!plan) lane = side_lane();
+    // REDs into g_depth commute with those of k_distribute
+    lane = side_lane();
     cudaStream_t apply_stream = s;
     if (lane) {
       if ((e = cudaEventRecord(lane->fork, s)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
@@ -3999,12 +3736,9 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
     af.bc2_sqrt = (float)sqrt(1.0 - pow(a->beta2, (double)a->step));
   }
   // g_depth was scaled by fscale above
-  if ((rc = plan ? procrustes_bwd_planned(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, plan,
-                                          a->splat_overflow_max, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4,
-                                          a->ws, T, H, W, s, fuse_w ? &af : nullptr)
-                 : procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
-                                  a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4, a->ws, B, T,
-                                  pairs, H, W, s, fuse_w ? &af : nullptr, /*depth_prescaled=*/true)))
+  if ((rc = procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
+                           a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4, a->ws, B, T, pairs,
+                           H, W, s, fuse_w ? &af : nullptr, /*depth_prescaled=*/true)))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   // Adam (model_wrapper_overfit.py:104-105)

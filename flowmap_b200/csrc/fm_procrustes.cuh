@@ -162,9 +162,8 @@ FM_HD void procrustes_solve(const double* m, const double* shift, float* rt_out,
   }
 }
 
-// Adjoint of the solve.  g_rt is dL/d[R | t] (3x4 row-major, float64).  `dbl` (optional, 15
-// values) receives the float64 originals of out.cbar, out.pb, out.qb.
-FM_HD void procrustes_adjoint(const PairState& st, const double* g_rt, PairAdjoint& out, double* dbl = nullptr) {
+// Adjoint of the solve.  g_rt is dL/d[R | t] (3x4 row-major, float64).
+FM_HD void procrustes_adjoint(const PairState& st, const double* g_rt, PairAdjoint& out) {
   double gt[3] = {g_rt[3], g_rt[7], g_rt[11]};
   double G[9];
   double ptrue[3] = {st.pbar[0] + st.shift[0], st.pbar[1] + st.shift[1], st.pbar[2] + st.shift[2]};
@@ -220,30 +219,6 @@ FM_HD void procrustes_adjoint(const PairState& st, const double* g_rt, PairAdjoi
     out.shift[i] = (float)st.shift[i];
   }
   out.wconst = 0.0f;
-  if (dbl) {
-    for (int i = 0; i < 9; ++i) dbl[i] = Cb[i];
-    for (int i = 0; i < 3; ++i) { dbl[9 + i] = pbar_bar[i] * st.inv; dbl[12 + i] = qbar_bar[i] * st.inv; }
-  }
-}
-
-// d loss / d ln(focal) of one pair THROUGH the Procrustes inputs when both frames share one focal
-// length with a fixed principal point: p_xy and q_xy scale with 1 / f, so the per-point sum
-//   - sum_j (g_p_j . p_j + g_q_j . q_j)_{xy}
-// collapses onto the moment sums the forward pass already has (m: the 16 shifted moments,
-// M[a][b] = sum w q_a p_b at m[7 + 3 a + b]; the shift is along z and does not touch xy):
-//   sum_j g_p_j,a p_ja = sum_r Cb[r][a] (M[r][a] - qbar_r mp_a) + pb_a mp_a
-//   sum_j g_q_j,a q_ja = sum_c Cb[a][c] (M[a][c] - pbar_c mq_a) + qb_a mq_a        (a in {x, y})
-// with g_p = w (Cb^T dq + pb), g_q = w (Cb dp + qb) as in point_adjoint.
-FM_HD double procrustes_focal_log_grad(const PairState& st, const double* m, const double* dbl) {
-  const double* Cb = dbl; const double* pb = dbl + 9; const double* qb = dbl + 12;
-  double s = 0.0;
-  for (int a = 0; a < 2; ++a) {
-    for (int r = 0; r < 3; ++r) s += Cb[r * 3 + a] * (m[7 + r * 3 + a] - st.qbar[r] * st.mp[a]);
-    s += pb[a] * st.mp[a];
-    for (int c = 0; c < 3; ++c) s += Cb[a * 3 + c] * (m[7 + a * 3 + c] - st.pbar[c] * st.mq[a]);
-    s += qb[a] * st.mq[a];
-  }
-  return -s;
 }
 
 // Per-point adjoints given the pair constants: dp' = p' - pbar', dq' = q' - qbar'.

@@ -38,47 +38,6 @@ def workspace(B: int, F: int, H: int, W: int, device) -> Tensor:
     return torch.empty(n, dtype=torch.uint8, device=device)
 
 
-class SplatPlan:
-    """Static transpose of align_surfaces' bilinear gather for ONE video's backward flows
-    (projection.py:235-242; csrc/fm_tiled.cuh): built once per Flows, it turns the backward's
-    4-tap scatter into an atomic-free gather.  `ptr` is None when the shape is not served
-    (W % 4 != 0) or the flow field is too degenerate for the plan's capacity: the step then takes
-    the global-RED kernels."""
-
-    def __init__(self, backward_flow: Tensor):
-        bf = _canon(backward_flow, "backward_flow")
-        if bf.dim() != 5 or bf.shape[0] != 1 or bf.shape[-1] != 2:
-            raise ValueError("flowmap_b200: SplatPlan needs backward flows of shape (1, F-1, H, W, 2)")
-        _, p, h, w, _ = bf.shape
-        self.shape = (p + 1, h, w)
-        self.status, self.overflow_max, self.entries = 0, 0, 0
-        nbytes = lib().fm_splat_plan_bytes(p + 1, h, w)
-        self.buf = torch.empty(nbytes, dtype=torch.uint8, device=bf.device) if nbytes else None
-        if self.buf is not None:
-            self.rebuild(bf)
-
-    def rebuild(self, backward_flow: Tensor) -> None:
-        import ctypes
-        bf = _canon(backward_flow, "backward_flow")
-        f, h, w = self.shape
-        if self.buf is None or tuple(bf.shape) != (1, f - 1, h, w, 2):
-            raise ValueError("flowmap_b200: backward flows do not match the plan's shape")
-        st, ov, tot = ctypes.c_int(0), ctypes.c_uint(0), ctypes.c_ulonglong(0)
-        with torch.cuda.device(bf.device):
-            check(lib().fm_splat_plan_build(_ptr(bf), _ptr(self.buf), f, h, w, _stream()), "fm_splat_plan_build")
-            check(lib().fm_splat_plan_info(_ptr(self.buf), ctypes.byref(st), ctypes.byref(ov), ctypes.byref(tot),
-                                           _stream()), "fm_splat_plan_info")
-        self.status, self.overflow_max, self.entries = st.value, ov.value, tot.value
-
-    @property
-    def ok(self) -> bool:
-        return self.buf is not None and self.status == 1
-
-    @property
-    def ptr(self):
-        return self.buf.data_ptr() if self.ok else None
-
-
 def intrinsics_to_k4(intrinsics: Tensor) -> Tensor:
     """(..., 3, 3) normalised intrinsics -> (..., 4) = (fx, fy, cx, cy); differentiable."""
     return torch.stack((intrinsics[..., 0, 0], intrinsics[..., 1, 1], intrinsics[..., 0, 2],

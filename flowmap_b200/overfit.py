@@ -160,12 +160,6 @@ class FusedOverfitter(Overfitter):
     logits and its chain rule evaluated inside the kernels, gradients accumulated into a
     single buffer per parameter.
 
-    use_splat_plan=True selects the DETERMINISTIC backward (ops.SplatPlan, csrc/fm_tiled.cuh): the
-    bilinear scatter of the Procrustes adjoint is transposed once per Flows into a static plan and
-    evaluated as a gather with TMA-staged windows -- no atomics, bit-reproducible gradients.  It is
-    parity-green but has been slower per backward than the default global-RED kernel
-    (tools/ab_tiled.py compares the two), hence opt-in.
-
     Several videos run B INDEPENDENT overfits in one step (fm_overfit_step_videos).  Video b gets what a
     one-video FusedOverfitter on video b with the same cfg and step clock seed gets: its flow loss is
     normalised by its own mask sum, its tracking loss by its own valid count, and its gradients, Adam
@@ -176,8 +170,8 @@ class FusedOverfitter(Overfitter):
     (T, H, W) / (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs
     [fo_b - b, fo_b - b + F_b - 1); `models[b]` is video b's Model, whose parameters are views into them.
     `tracks` is then a list of B segment lists, and the metrics log holds (steps, B) values.  Several
-    videos do not serve the splat plan, pair sharding or the split-step surface (but for a network Model's
-    batch, below).  Two forms:
+    videos do not serve pair sharding or the split-step surface (but for a network Model's batch, below).
+    Two forms:
 
     - `batch.videos` of shape (B, F, 3, H, W) with B > 1 and Flows of shape (B, F-1, ...): videos of one
       length, whose packed buffers are the (B, F, ...) / (B, F-1, ...) tensors.  training_step(),
@@ -202,25 +196,20 @@ class FusedOverfitter(Overfitter):
     `batch.intrinsics` (1, F, 3, 3), (B, F, 3, 3) for a tensor batch, or each Batch's own for a list, normalised
     as in the reference and possibly different for every frame.  There is no focal parameter and the step
     computes no intrinsics gradient (fm_overfit_step with focal = g_k4 = track_g_k4 = NULL); set_intrinsics
-    swaps K in place.  The splat plan and pair sharding do not serve it."""
+    swaps K in place.  Pair sharding does not serve it."""
 
-    def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda",
-                 use_splat_plan: bool = False, model=None):
+    def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda", model=None):
         self._layout, self._tensor_batch, self._network = None, False, False
         self._gt = cfg.intrinsics == "ground_truth"
-        if self._gt and use_splat_plan:
-            raise ValueError("flowmap_b200: the splat plan does not serve ground-truth intrinsics")
         if isinstance(batch, (list, tuple)):
-            self._init_videos(cfg, list(batch), flows, tracks, device, use_splat_plan, model)
+            self._init_videos(cfg, list(batch), flows, tracks, device, model)
         elif batch.videos.shape[0] > 1 and isinstance(model, Model) and \
                 not isinstance(model.backbone, BackboneExplicitDepth):
-            self._init_network_videos(cfg, batch, flows, tracks, use_splat_plan, model)
+            self._init_network_videos(cfg, batch, flows, tracks, model)
         elif batch.videos.shape[0] > 1:
             b, f = batch.videos.shape[:2]
             if model is not None:
                 raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
-            if use_splat_plan:
-                raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
             if tracks is not None and len(tracks) != b:
                 raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({b})")
             for name in _FLOW_NAMES:
@@ -228,10 +217,10 @@ class FusedOverfitter(Overfitter):
                     raise ValueError(f"flowmap_b200: flows.{name} must hold (B, F-1) = ({b}, {f - 1}) pairs")
             batch = batch.to(device)
             self._init_videos(cfg, [_video(batch, i) for i in range(b)], [_video(flows, i) for i in range(b)],
-                              tracks, device, False, None)
+                              tracks, device, None)
             self._tensor_batch, self.batch = True, batch
         else:
-            self._init_one(cfg, batch, flows, tracks, device, use_splat_plan, model)
+            self._init_one(cfg, batch, flows, tracks, device, model)
         self._init_step(cfg)
         if self._gt:
             self.set_intrinsics(self.batch.intrinsics if self._layout is None or self._tensor_batch
@@ -239,7 +228,7 @@ class FusedOverfitter(Overfitter):
         if self._tensor_batch and not self._network:  # the parameters as (B, F, ...) / (B, F-1, ...) views
             self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
 
-    def _init_one(self, cfg, batch, flows, tracks, device, use_splat_plan, model):
+    def _init_one(self, cfg, batch, flows, tracks, device, model):
         """The one-video optimiser: its parameters are the Model's own tensors."""
         if model is not None and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
             raise ValueError(f"flowmap_b200: the bound model's intrinsics ({type(model.intrinsics).__name__}) do not "
@@ -253,8 +242,6 @@ class FusedOverfitter(Overfitter):
         self.B, self.frames, self.T, self._hw = 1, [f], f, (h, w)
         self._lead = ((1, f), (1, f - 1), ())  # leading dims of the per-frame, per-pair and per-video buffers
         self._track_frames = None
-        self._use_plan = use_splat_plan and cfg.procrustes_points is None and not cfg.procrustes_randomize
-        self._plan = ops.SplatPlan(self.flows.backward) if self._use_plan else None
         self.models = [self.model]
         if isinstance(self.model.backbone, BackboneExplicitDepth):
             self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
@@ -272,14 +259,12 @@ class FusedOverfitter(Overfitter):
         self._ws = ops.workspace(1, f, h, w, dev)
         self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
 
-    def _init_videos(self, cfg, batches, flows, tracks, device, use_splat_plan, model):
+    def _init_videos(self, cfg, batches, flows, tracks, device, model):
         """The packed optimiser of several videos (see the class docstring)."""
         from ._lib import VideoLayout, lib
         import ctypes
         if model is not None:
             raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
-        if use_splat_plan:
-            raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
         if not batches or not isinstance(flows, (list, tuple)) or len(flows) != len(batches):
             raise ValueError("flowmap_b200: videos of different lengths need one Flows per Batch")
         B = len(batches)
@@ -320,7 +305,6 @@ class FusedOverfitter(Overfitter):
         self._tables = video_tables(frames, dev)
         self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
         self._layout_ref = ctypes.byref(self._layout)
-        self._use_plan, self._plan = False, None
 
         def pack(params):
             buf = torch.cat([p.data for p in params]).contiguous()
@@ -348,13 +332,11 @@ class FusedOverfitter(Overfitter):
         self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
         self._msum = self._video_mask_sums(self.flows)
 
-    def _init_network_videos(self, cfg, batch, flows, tracks, use_splat_plan, model):
+    def _init_network_videos(self, cfg, batch, flows, tracks, model):
         """A network Model's tensor batch of several videos (see the class docstring): no parameter buffers,
         one focal length per video from the softmin sweep."""
         from ._lib import VideoLayout, lib
         import ctypes
-        if use_splat_plan:
-            raise ValueError("flowmap_b200: the splat plan serves one video; use_splat_plan needs B = 1")
         if tracks is not None or cfg.use_tracking:
             raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
         if cfg.intrinsics != "softmin" or cfg.regression_after is not None:
@@ -373,7 +355,6 @@ class FusedOverfitter(Overfitter):
         self._tables = video_tables(self.frames, dev)
         self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
         self._layout_ref = ctypes.byref(self._layout)
-        self._use_plan, self._plan = False, None
         self._focal = torch.zeros(B, device=dev)
         self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
         self._msum = self._mask_sum(self.flows).expand(B).contiguous()
@@ -449,7 +430,6 @@ class FusedOverfitter(Overfitter):
             if self._softmin else None
         self.use_cuda_graph = False  # opt-in: replay the update step as ONE CUDA graph launch
         self._graphs, self._eager_runs = {}, {}
-        self._set_plan_args(a)
         self._packed = None
         if cfg.use_tracking:
             assert self.tracks is not None
@@ -484,11 +464,6 @@ class FusedOverfitter(Overfitter):
             check(self._lib.fm_overfit_step_videos(a, self._layout_ref, st), what)
         else:
             check(self._lib.fm_overfit_step(a, st), what)
-
-    def _set_plan_args(self, a):
-        pl = self._plan
-        a.splat_plan = pl.ptr if pl is not None else None
-        a.splat_overflow_max = pl.overflow_max if (pl is not None and pl.ok) else 0
 
     def set_flows(self, flows: Flows, mask_sum: Optional[Tensor] = None):
         """Point the step at another device-resident Flows of the same shape (the next batch of a
@@ -528,9 +503,6 @@ class FusedOverfitter(Overfitter):
         a.fflow, a.bflow = flows.forward.data_ptr(), flows.backward.data_ptr()
         a.fmask, a.bmask = flows.forward_mask.data_ptr(), flows.backward_mask.data_ptr()
         self._msum.copy_(self._mask_sum(flows) if mask_sum is None else mask_sum)
-        if self._plan is not None:  # new backward flows: new transpose
-            self._plan.rebuild(flows.backward)
-            self._set_plan_args(a)
         self._graphs.clear()  # captured launches hold the old pointers
         self._eager_runs.clear()
 
@@ -659,7 +631,7 @@ class FusedOverfitter(Overfitter):
         # All-pixel Procrustes: the moment pass of the step does not have to wait for the focal length
         # the sweep is about to produce -- the sums for one K follow exactly from the sums for another
         # (fm_overfit_step_args.moments_k4) -- so it runs beside the sweep, on the candidate-0 intrinsics.
-        early_moments = update and self._indices is None and self._plan is None
+        early_moments = update and self._indices is None
         cur = torch.cuda.current_stream()
         with torch.cuda.device(self.rt.device):
             if early_moments:

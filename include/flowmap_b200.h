@@ -101,41 +101,6 @@ int fm_procrustes_bwd(const float* depth, const float* k4, const float* backward
                       float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int F, int H,
                       int W, void* stream);
 
-/* ---- splat plan: the loop-invariant transpose of align_surfaces' bilinear gather ------------
- * projection.py:235-242 samples the earlier frame at xy + backward_flow; its backward scatters into
- * four taps per pixel.  The backward flows do not change during an overfit run
- * (flow/__init__.py:23, model_wrapper_overfit.py:44-49), so the scatter matrix is transposed ONCE
- * into a static plan (per 64 x 32 tile of the earlier frame: cells sorted by contributor count,
- * sliced-ELL entry lists = source pixel inside the tile's 128 x 60 window + unorm19 coefficient);
- * the per-step backward then gathers (no atomics, deterministic order) and stages its windows with
- * TMA.  `plan` is caller-provided device memory of fm_splat_plan_bytes(F, H, W) bytes (0 if the
- * shape is not served: needs W % 4 == 0); it also holds the per-step correspondence-weight scratch
- * that the planned forward hands to the planned backward.  fm_splat_plan_build is asynchronous;
- * fm_splat_plan_info SYNCHRONISES the stream and returns the build verdict: status 1 = usable,
- * otherwise the caller must pass plan = NULL to the step (degenerate flow fields whose lists exceed
- * the plan's capacity); overflow_max = largest number of flow outliers of any pair (sources outside
- * their tile's window; they take a small RED kernel), to be passed along with the plan. */
-size_t fm_splat_plan_bytes(int F, int H, int W);
-int fm_splat_plan_build(const float* backward_flow, void* plan, int F, int H, int W, void* stream);
-int fm_splat_plan_info(const void* plan, int* status, unsigned* overflow_max, unsigned long long* total_entries,
-                       void* stream);
-
-/* fm_procrustes_fwd / fm_procrustes_bwd for ONE video (B = 1), all pixels, through a splat plan
- * (projection.py:213-249 + procrustes.py:7-51 and their backward).  weights may be logits
- * (weight_sensitivity != 0: w = sigmoid(sens * logit), backbone_explicit_depth.py:40; g_weights is
- * then d/d logit) or NULL (all ones).  All frames must share their intrinsics up to the focal length
- * (intrinsics_regressed.py / intrinsics_softmin.py): g_k4 returns the intrinsics gradient as the
- * equivalent d/dfx of each frame, g_k4[:, 1:] = 0 (as fm_flow_loss_fwd_bwd does in
- * FM_K_SHARED_FOCAL mode).  g_depth holds the direct flow-loss gradient on entry (or zeros) and the
- * total gradient on return; every element is written exactly once (bit-reproducible). */
-int fm_procrustes_fwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                              float weight_sensitivity, void* plan, float* rt, void* ws, int F, int H, int W,
-                              void* stream);
-int fm_procrustes_bwd_planned(const float* depth, const float* k4, const float* backward_flow, const float* weights,
-                              float weight_sensitivity, void* plan, unsigned plan_overflow_max, const float* g_rt,
-                              int include_flow_loss, float* g_depth, float* g_weights, float* g_k4, void* ws, int F,
-                              int H, int W, void* stream);
-
 /* loss_flow.py:55-56,67-68 denominators: *out = sum(forward_mask) + sum(backward_mask)
  * (device float64 scalar). */
 int fm_mask_sum(const float* forward_mask, const float* backward_mask, double* out, size_t count,
@@ -298,8 +263,8 @@ typedef struct {
  * (no focal gradient).  focal == NULL together with g_k4 == NULL and track_g_k4 == NULL is the
  * constant-intrinsics step (intrinsics_ground_truth.py: K given per frame, e.g. calibrated data): it
  * computes no intrinsics gradient at all -- the Procrustes backward and the tracking sweep run without
- * their K accumulators -- and needs no splat plan; g_k4 == NULL with a focal parameter or a track_g_k4 is
- * refused.  step <= 0 computes loss and gradients but skips Adam.
+ * their K accumulators; g_k4 == NULL with a focal parameter or a track_g_k4 is refused.  step <= 0
+ * computes loss and gradients but skips Adam.
  * Gradients of the step are left in g_depth / g_weights / g_focal / g_k4. */
 typedef struct {
   int F, H, W;
@@ -342,9 +307,6 @@ typedef struct {
                                    g_rt (F-1,3,4) / intrinsics gradient track_g_k4 (F,4) (tracks == NULL,
                                    either may be NULL), then the Procrustes backward; step must be 0 in
                                    the two halves' common use (no parameter may change in between) */
-  void* splat_plan;             /* fm_splat_plan_build of `bflow` with status 1, or NULL (global-RED path);
-                                   used when indices == NULL */
-  unsigned splat_overflow_max;  /* overflow_max of fm_splat_plan_info */
   const float* flow_grad_scale;  /* FM_STEP_BACKWARD only: device scalars d total / d flow loss and     */
   const float* track_grad_scale; /* d total / d tracking loss (autograd's grad_output), or NULL (= 1) */
   const void* clock;             /* device step clock (fm_step_clock_tick) or NULL.  With a clock the Adam
@@ -406,8 +368,8 @@ typedef struct {
  * segments of video b carry start frames frame_offset[b] + s (they never cross videos); track_ws is
  * fm_track_workspace_bytes(T, total_samples).  Metrics: gt_positions (T, 3), NaN first position of a
  * video = no ground truth; the ring is (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).
- * Needs no splat plan, and refuses defer_adam = 1 together with step > 0 and weight logits (the caller
- * updates the logits after the sweep's backward).
+ * Refuses defer_adam = 1 together with step > 0 and weight logits (the caller updates the logits after
+ * the sweep's backward).
  * Phases: FM_STEP_ALL, or the two halves of a split step, FM_STEP_FORWARD then FM_STEP_BACKWARD (a network
  * backbone's batch, whose depths / weights come from the network and whose update the caller owns).  A
  * split step needs step = 0, defer_adam = 0, tracks == NULL and metrics_log == NULL.  Its flow_grad_scale is

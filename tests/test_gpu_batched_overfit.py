@@ -45,13 +45,10 @@ def _cpu_inputs(b, f=4, h=8, w=8):
 
 
 def test_batched_step_validates_its_inputs():
-    """Refused before anything reaches the device: the splat plan, a track list that is not one list per
-    video, a bound Model, flows whose batch does not match the videos, and pair sharding of several
-    videos."""
+    """Refused before anything reaches the device: a track list that is not one list per video, a bound
+    Model, flows whose batch does not match the videos, and pair sharding of several videos."""
     from flowmap_b200.overfit import FusedOverfitter, OverfitCfg, ShardedFusedOverfitter
     batch, flows, tracks = _cpu_inputs(2)
-    with pytest.raises(ValueError, match="splat plan"):
-        FusedOverfitter(OverfitCfg(), batch, flows, use_splat_plan=True)
     with pytest.raises(ValueError, match="one segment list per video"):
         FusedOverfitter(OverfitCfg(use_tracking=True), batch, flows, [tracks])
     with pytest.raises(ValueError, match="Model"):

@@ -10,8 +10,8 @@ through Procrustes with them.  These cases put the centre pixel at 1000 or 0.01,
 depth 200 with weight ~0, scale the whole depth by 1e-2 and 1e2, and move the weighted cloud into a
 corner.  Every path that forms the shift is covered: all-pixel Procrustes (k_moments_dense,
 k_distribute_window / _dense), subsampled Procrustes (k_moments / k_distribute), the softmin sweep
-(k_sweep_scale_solve), the fused step on both backwards (k_moments_tiled and the splat plan), and the
-explicit-points align_rigid (k_points_*).
+(k_sweep_scale_solve), the fused step with the tracking loss, and the explicit-points align_rigid
+(k_points_*).
 
 Gradients are checked per frame, per pair and on the border band against max(1e-4, 3x the float32
 oracle's own error); the loss within 1e-4 and the poses within 2e-5, or 3x the float32 oracle's error
@@ -188,12 +188,9 @@ def test_sweep_backward_in_depth_regimes_vs_float64_oracle(kind, b, f, h, w):
             assert got[key] <= max(1e-4, 3 * noise[key]), (label, key, got[key], noise[key])
 
 
-@pytest.mark.parametrize("use_plan", [False, True], ids=["red", "plan"])
-@pytest.mark.parametrize("kind", ["centre_far", "horizon"])
-def test_fused_step_with_tracking_in_depth_regimes_vs_float64_oracle(kind, use_plan):
-    """fm_overfit_step with the tracking loss on the global-RED and on the splat-plan backward (which
-    takes its moments from k_moments_tiled and its per-pair constants from the stored shift).  The
-    message says which path ran; with these few-pixel flows the plan must be taken."""
+@pytest.mark.parametrize("kind", ["centre_far", "horizon"], ids=lambda k: f"{k}-red")  # red: the global-RED backward
+def test_fused_step_with_tracking_in_depth_regimes_vs_float64_oracle(kind):
+    """fm_overfit_step with the tracking loss."""
     from oracle import flowmap_oracle as O
     from flowmap_b200.overfit import FusedOverfitter, OverfitCfg
     from flowmap_b200.types import Batch, Flows, Tracks
@@ -220,19 +217,15 @@ def test_fused_step_with_tracking_in_depth_regimes_vs_float64_oracle(kind, use_p
     batch = Batch(torch.zeros(1, 1, 1, 1, 1).expand(1, f, 3, h, w), torch.arange(f)[None], ["s"], ["d"])
     o = FusedOverfitter(OverfitCfg(initial_focal=focal, use_tracking=True, tracking_enable_after=0), batch,
                         Flows(*(t.float() for t in (fl.forward, fl.backward, fl.forward_mask, fl.backward_mask))),
-                        [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks], use_splat_plan=use_plan)
+                        [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks])
     with torch.no_grad():
         o.model.backbone.depth.copy_(depth.float())
         o.model.backbone.weights.copy_(wparam.float())
-    path = "splat plan" if o._plan is not None and o._plan.ok else "global RED"
-    if use_plan and o._plan is not None:
-        path += f" (plan status {o._plan.status}, overflow {o._plan.overflow_max})"
-    assert path.startswith("splat plan") == use_plan, path
     loss, _ = o.training_step(update=False)
     gr = o.gradients()
     out = dict(loss=float(loss), ext=o.extrinsics().cpu(), g_depth=gr["depth"].cpu(), g_w=gr["weights"].cpu(),
                g_focal=float(gr["focal"]))
-    label = f"fused {kind} {f}x{h}x{w} tracking, {path}"
+    label = f"fused {kind} {f}x{h}x{w} tracking"
     track_err = abs(float(o._track_loss) - ref["track"]) / abs(ref["track"])
     print(label, "tracking loss error", f"{track_err:.1e}")
     assert ref["track"] > 0 and track_err <= 1e-4, (label, track_err)

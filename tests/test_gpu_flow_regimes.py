@@ -4,8 +4,8 @@ outliers, zoom, and a rigid scene under large camera motion.  These reach what t
 flows of the other parity tests do not: bilinear_taps' clipping to the border and the pile-up of
 depth-gradient taps on the first and last rows and columns, the placement of k_distribute_window's
 scatter window (shifted by the tile's mean flow, clamped onto the image) and taps in its last
-column and pitch padding, the float RED fall-back for taps outside the window, the splat-plan
-backward, and the tracking sweep's predicted-target mask under large poses.
+column and pitch padding, the float RED fall-back for taps outside the window, and the tracking
+sweep's predicted-target mask under large poses.
 
 Every gradient is checked per frame (depth) or per frame pair (weights) and on the depth gradient's
 one-pixel border band, besides the whole tensor, against max(1e-4, 3x the float32 oracle's own
@@ -66,11 +66,9 @@ def _fused_case(kind, f, h, w):
     return depth[0], wparam, fl, focal, tracks
 
 
-@pytest.mark.parametrize("use_plan", [False, True], ids=["red", "plan"])
-@pytest.mark.parametrize("kind", ["scene", "zoom"])
-def test_fused_step_with_tracking_vs_float64_oracle(kind, use_plan):
-    """fm_overfit_step with the tracking loss, on the global-RED and on the splat-plan backward (a
-    plan that overflows leaves the step on the RED path; the message says which one ran)."""
+@pytest.mark.parametrize("kind", ["scene", "zoom"], ids=lambda k: f"{k}-red")  # red: the global-RED backward
+def test_fused_step_with_tracking_vs_float64_oracle(kind):
+    """fm_overfit_step with the tracking loss."""
     from oracle import flowmap_oracle as O
     from flowmap_b200.overfit import FusedOverfitter, OverfitCfg
     from flowmap_b200.types import Batch, Flows, Tracks
@@ -94,22 +92,15 @@ def test_fused_step_with_tracking_vs_float64_oracle(kind, use_plan):
     batch = Batch(torch.zeros(1, 1, 1, 1, 1).expand(1, f, 3, h, w), torch.arange(f)[None], ["s"], ["d"])
     o = FusedOverfitter(OverfitCfg(initial_focal=focal, use_tracking=True, tracking_enable_after=0), batch,
                         Flows(*(t.float() for t in (fl.forward, fl.backward, fl.forward_mask, fl.backward_mask))),
-                        [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks], use_splat_plan=use_plan)
+                        [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks])
     with torch.no_grad():
         o.model.backbone.depth.copy_(depth.float())
         o.model.backbone.weights.copy_(wparam.float())
-    path = "splat plan" if o._plan is not None and o._plan.ok else "global RED"
-    if use_plan and o._plan is not None:
-        path += f" (plan status {o._plan.status}, overflow {o._plan.overflow_max})"
-    # zoom spreads taps past the plan's overflow capacity and falls back to RED; the scene must take
-    # the plan, or no fused case would reach the planned backward with tracking
-    if use_plan and kind == "scene":
-        assert path.startswith("splat plan"), path
     loss, _ = o.training_step(update=False)
     gr = o.gradients()
     out = dict(loss=float(loss), ext=o.extrinsics().cpu(), g_depth=gr["depth"].cpu(), g_w=gr["weights"].cpu(),
                g_focal=float(gr["focal"]))
-    label = f"fused {kind} {f}x{h}x{w} tracking, {path}"
+    label = f"fused {kind} {f}x{h}x{w} tracking"
     track_err = abs(float(o._track_loss) - ref["track"]) / abs(ref["track"])
     print(label, "tracking loss error", f"{track_err:.1e}")
     assert ref["track"] > 0 and track_err <= 1e-4, (label, track_err)

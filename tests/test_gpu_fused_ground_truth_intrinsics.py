@@ -429,8 +429,6 @@ def test_refusals():
     with pytest.raises(ValueError, match="match"):
         FusedOverfitter(OverfitCfg(), _batch(f, h, w, k.to(DEV)), flows, device=DEV,
                         model=model(IntrinsicsGroundTruthCfg("ground_truth")))
-    with pytest.raises(ValueError, match="splat plan"):
-        FusedOverfitter(cfg, _batch(f, h, w, k.to(DEV)), flows, device=DEV, use_splat_plan=True)
     o = FusedOverfitter(cfg, _batch(f, h, w, k.to(DEV)), flows, device=DEV)
     with pytest.raises(ValueError, match="intrinsics"):
         o.set_intrinsics(k[:, :, :2].to(DEV))

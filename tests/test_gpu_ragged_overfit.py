@@ -43,7 +43,7 @@ def _cpu_video(f, h=8, w=8):
 
 def test_ragged_step_validates_its_inputs():
     """Refused before anything reaches the device: videos of different H x W, a video of one frame, Flows
-    that are not (1, F_b - 1, H, W, ...), the splat plan, a bound Model, and pair sharding."""
+    that are not (1, F_b - 1, H, W, ...), a bound Model, and pair sharding."""
     from flowmap_b200.overfit import FusedOverfitter, OverfitCfg, ShardedFusedOverfitter
     (b4, f4), (b6, f6) = _cpu_video(4), _cpu_video(6)
     cfg = OverfitCfg()
@@ -56,8 +56,6 @@ def test_ragged_step_validates_its_inputs():
         FusedOverfitter(cfg, [b4, b6], [f4, f4])
     with pytest.raises(ValueError, match="one Flows per Batch"):
         FusedOverfitter(cfg, [b4, b6], [f4])
-    with pytest.raises(ValueError, match="splat plan"):
-        FusedOverfitter(cfg, [b4, b6], [f4, f6], use_splat_plan=True)
     with pytest.raises(ValueError, match="Model"):
         FusedOverfitter(cfg, [b4, b6], [f4, f6], model=object())
     with pytest.raises(ValueError, match="one segment list per video"):

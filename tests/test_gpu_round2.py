@@ -1,77 +1,12 @@
-"""`-m gpu`: round-2 machinery around the hot path -- the deterministic splat-plan backward (TMA-staged
-tiled kernels) against the default global-RED kernels, the device step clock against by-value Adam,
-and CUDA-graph replay of the update step against eager execution."""
-import sys
-
+"""`-m gpu`: round-2 machinery around the hot path -- the device step clock against by-value Adam,
+CUDA-graph replay of the update step against eager execution, the early moment pass of a sweep step and
+the tracking sweep sharded by source frame."""
 import pytest
 import torch
 
-from conftest import ROOT, rel_l2
+from conftest import rel_l2
 
 pytestmark = pytest.mark.gpu
-sys.path.insert(0, str(ROOT / "tools"))
-
-
-@pytest.mark.parametrize("shape", [(3, 24, 32), (4, 36, 48), (3, 100, 64), (3, 136, 192)])
-@pytest.mark.parametrize("kind", ["iid", "smooth", "shift", "outliers"])
-def test_splat_plan_path_matches_the_red_path(shape, kind):
-    """fm_procrustes_{fwd,bwd}_planned vs fm_procrustes_{fwd,bwd}: poses, depth / weight / focal
-    gradients; the planned backward is bit-reproducible when no flow outlier needs the RED fall-back."""
-    import ab_tiled
-    r = ab_tiled.compare(*shape, kind)
-    assert r["plan_status"] == 1, r
-    assert r["ok"], r
-    if r["overflow_max"] == 0:
-        assert r["bitwise_repeatable"], r
-
-
-@pytest.mark.parametrize("kind", ["shift", "outliers"])
-def test_splat_plan_path_vs_float64_oracle(kind):
-    """The planned forward / backward on large coherent motion and on 5 % far outliers against the
-    float64 oracle itself, so that a bug shared with the RED path cannot hide behind the comparison
-    above: loss, poses, and the depth (whole, per frame, border band), weight-logit (whole, per pair)
-    and focal gradients within max(1e-4, 3x the float32 oracle's own error)."""
-    import ab_tiled
-    from oracle import flowmap_oracle as O
-    from flowmap_b200 import ops
-    from flow_regime_checks import check, errors, oracle_steps
-    f, h, w = 3, 136, 192
-    c = ab_tiled.make_case(f, h, w, kind)
-    plan = ops.SplatPlan(c["bwd"])
-    assert plan.status == 1, plan.status
-    r = ab_tiled.run_ops(c, f, h, w, plan)
-    cpu = {k: v.double().cpu() for k, v in c.items()}
-    refs = oracle_steps(cpu["depth"][None], cpu["wparam"][None],
-                        O.Flows(cpu["fwd"], cpu["bwd"], cpu["fmask"], cpu["bmask"]), 0.85)
-    out = dict(loss=r["loss"], ext=ops.pose_chain(r["rt"]).cpu(), g_depth=r["g_depth"].cpu(), g_w=r["g_w"].cpu(),
-               g_focal=r["g_focal"])
-    check(errors(out, refs[64]), errors(refs[32], refs[64]), f"splat plan {kind} {f}x{h}x{w}",
-          loss_tol=1e-4, pose_tol=2e-5, floor=1e-4)
-
-
-def test_degenerate_flows_fall_back_to_the_red_path():
-    """A flow field whose taps pile up far outside every tile window exceeds the plan's overflow
-    capacity: the plan reports it and FusedOverfitter silently keeps the global-RED kernels."""
-    import ab_tiled
-    import bench
-    from flowmap_b200 import ops
-    from flowmap_b200.overfit import FusedOverfitter, OverfitCfg
-    from flowmap_b200.types import Batch, Flows
-    f, h, w = 3, 360, 640
-    c = ab_tiled.make_case(f, h, w, "leave")
-    plan = ops.SplatPlan(c["bwd"])
-    assert plan.status != 1 and plan.ptr is None
-    dev = c["bwd"].device
-    batch = Batch(torch.zeros(1, 1, 1, 1, 1, device=dev).expand(1, f, 3, h, w), torch.arange(f, device=dev)[None], ["s"], ["d"])
-    flows = Flows(c["fwd"], c["bwd"], c["fmask"], c["bmask"])
-    outs = []
-    for use_plan in (False, True):
-        o = FusedOverfitter(OverfitCfg(), batch, flows, device=dev, use_splat_plan=use_plan)
-        with torch.no_grad():
-            o.model.backbone.depth.copy_(1.0 + c["depth"])
-            o.model.backbone.weights.copy_(c["wparam"])
-        outs.append(float(o.training_step(update=False)[0]))
-    assert outs[0] == outs[1]
 
 
 def test_step_clock_adam_equals_by_value_adam():

@@ -264,19 +264,19 @@ def test_subsampled_procrustes_vs_float64_oracle(kind, b, f, h, w, points):
             assert e <= max(1e-4, 3 * n), (label, "weight gradient at duplicated points", e, n)
 
 
-FUSED_CASES = [("scene", False, None), ("scene", True, None), ("leave", False, None), ("leave", True, None),
-               ("zoom", False, None), ("zoom", True, None), ("scene", False, 1000)]
+FUSED_CASES = [("scene", None), ("leave", None), ("zoom", None), ("scene", 1000)]
 
 
-@pytest.mark.parametrize("kind,use_plan,npts", FUSED_CASES,
-                         ids=[f"{k}-{'plan' if p else 'red'}{'' if n is None else f'-pts{n}'}" for k, p, n in FUSED_CASES])
-def test_fused_softmin_stage_vs_float64_oracle(kind, use_plan, npts):
+# red: the global-RED backward
+@pytest.mark.parametrize("kind,npts", FUSED_CASES,
+                         ids=[f"{k}-red{'' if n is None else f'-pts{n}'}" for k, n in FUSED_CASES])
+def test_fused_softmin_stage_vs_float64_oracle(kind, npts):
     """fm_overfit_step in the softmin stage with 8192 injected sweep points: one step without the update
     (loss, f_hat, poses, gradients per frame and pair), then 3 Adam steps against the oracle's
-    trajectory.  The update steps without the splat plan take the early moment pass (moments at the
-    candidate-0 intrinsics, rescaled inside the step); the all-pixel steps fuse the weight Adam of pairs
-    >= 1 into the step and leave pair 0 to the sweep's backward.  With 1000 Procrustes points the weight
-    gradient is sparse and its Adam runs on its own."""
+    trajectory.  The all-pixel update steps take the early moment pass (moments at the candidate-0
+    intrinsics, rescaled inside the step), fuse the weight Adam of pairs >= 1 into the step and leave pair 0
+    to the sweep's backward.  With 1000 Procrustes points the weight gradient is sparse and its Adam runs on
+    its own."""
     from oracle import flowmap_oracle as O
     from flowmap_b200.overfit import FusedOverfitter, OverfitCfg
     from flowmap_b200.types import Batch, Flows, Tracks
@@ -295,16 +295,12 @@ def test_fused_softmin_stage_vs_float64_oracle(kind, use_plan, npts):
     batch = Batch(torch.zeros(1, 1, 1, 1, 1).expand(1, f, 3, h, w), torch.arange(f)[None], ["s"], ["d"])
     o = FusedOverfitter(OverfitCfg(**kw), batch,
                         Flows(*(t.float() for t in (fl.forward, fl.backward, fl.forward_mask, fl.backward_mask))),
-                        None if tracks is None else [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks],
-                        use_splat_plan=use_plan)
+                        None if tracks is None else [Tracks(t.xy.float(), t.visibility, t.start_frame) for t in tracks])
     o.injected_indices = sweep_idx
     with torch.no_grad():
         o.model.backbone.depth.copy_(depth.float())
         o.model.backbone.weights.copy_(wparam.float())
     pts = None if o._indices is None else o._indices.cpu()
-    path = "splat plan" if o._plan is not None and o._plan.ok else "global RED"
-    if use_plan and o._plan is not None:
-        path += f" (plan status {o._plan.status}, overflow {o._plan.overflow_max})"
 
     def oracle(dt):
         st = O.OverfitOracle(O.OverfitConfig(**kw), f, h, w, dtype=dt)
@@ -325,7 +321,7 @@ def test_fused_softmin_stage_vs_float64_oracle(kind, use_plan, npts):
     ref32 = [as_out(step32()) for _ in range(3)]
     noise = errors(ref32[0], ref[0])
     label = f"fused softmin {kind} {f}x{h}x{w}{' tracking' if tracking else ''}, " \
-            f"{'all pixels' if npts is None else f'{npts} Procrustes points'}, {path}"
+            f"{'all pixels' if npts is None else f'{npts} Procrustes points'}"
 
     loss, _ = o.training_step(update=False)
     gr = o.gradients()

@@ -1,6 +1,6 @@
 """The fused engine of a network backbone's batch of several videos (the pretraining step) refuses what the
-packed split step does not serve before anything reaches the device: tracks, a regressed focal length, a
-softmin regression stage and the splat plan.  CPU only."""
+packed split step does not serve before anything reaches the device: tracks, a regressed focal length and a
+softmin regression stage.  CPU only."""
 import pytest
 import torch
 from torch import nn
@@ -43,8 +43,6 @@ def test_network_batch_engine_refusals():
                 OverfitCfg(intrinsics="ground_truth")):
         with pytest.raises(ValueError, match="softmin intrinsics without a regression stage"):
             FusedOverfitter(cfg, batch, flows, device="cpu", model=model)
-    with pytest.raises(ValueError, match="splat plan"):
-        FusedOverfitter(soft, batch, flows, device="cpu", use_splat_plan=True, model=model)
 
 
 def test_network_batch_engine_takes_cuda_flows_only():

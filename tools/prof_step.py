@@ -31,20 +31,6 @@ loss = torch.empty((), device=dev)
 P = lambda x: x.data_ptr()  # noqa: E731
 st = torch.cuda.current_stream().cuda_stream
 L = lib()
-PLANNED = len(sys.argv) >= 7 and sys.argv[6] == "plan"
-if PLANNED:  # the splat-plan path (weights as logits, as the fused step passes them)
-    plan = ops.SplatPlan(bwd)
-    assert plan.ok, plan.status
-    logits = 0.01 * torch.randn(1, F - 1, H, W, device=dev, generator=g)
-    for _ in range(REPS):
-        L.fm_procrustes_fwd_planned(P(depths), P(k4), P(bwd), P(logits), 100.0, plan.ptr, P(rt), P(ws), F, H, W, st)
-        L.fm_flow_loss_fwd_bwd(P(depths), P(k4), P(rt), P(fwd), P(bwd), P(fm), P(bm), P(msum), 0, 0.01,
-                               1000.0, KMODE, P(loss), P(g_depth), P(g_rt), P(g_k4), P(ws), 1, F, H, W, st)
-        L.fm_procrustes_bwd_planned(P(depths), P(k4), P(bwd), P(logits), 100.0, plan.ptr, plan.overflow_max, None, 1,
-                                    P(g_depth), P(g_w), P(g_k4), P(ws), F, H, W, st)
-    torch.cuda.synchronize()
-    print("loss", float(loss))
-    sys.exit(0)
 for _ in range(REPS):
     L.fm_procrustes_fwd(P(depths), P(k4), P(bwd), P(weights), None, 0, P(rt), P(ws), 1, F, H, W, st)
     L.fm_flow_loss_fwd_bwd(P(depths), P(k4), P(rt), P(fwd), P(bwd), P(fm), P(bm), P(msum), 0, 0.01,
