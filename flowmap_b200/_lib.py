@@ -51,6 +51,9 @@ SIGNATURES = {
     "fm_track_loss_fwd_sharded": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, ctypes.c_longlong,
                                           c_int, c_float, c_float, _P, _P, c_int, c_int, c_int, c_int, c_int,
                                           c_int, c_int, _P]),
+    "fm_track_loss_fwd_const_k": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, ctypes.c_longlong,
+                                          c_int, c_float, c_float, _P, _P, c_int, c_int, c_int, c_int, c_int,
+                                          c_int, _P]),
     "fm_track_loss_value": (c_int, [_P, c_float, _P, _P]),
     "fm_track_loss_bwd_sharded": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, ctypes.c_longlong,
                                           c_int, c_float, c_float, _P, _P, _P, _P, _P, c_int, c_int, c_int,

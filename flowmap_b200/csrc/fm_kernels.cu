@@ -3314,6 +3314,16 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
                         src_frame_hi, shared_intrinsics, stream, (double*)ws, 1, TrackOneVideo{}, true);
 }
 
+int fm_track_loss_fwd_const_k(const float* depth, const float* k4, const float* extrinsics, const int* segments,
+                              int num_segments, int max_rows, int max_points, const float* track_xy,
+                              const unsigned char* track_vis, long long total_samples, int mapping, float delta,
+                              float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
+                              int src_frame_lo, int src_frame_hi, void* stream) {
+  return track_fwd_impl(depth, k4, extrinsics, segments, num_segments, max_rows, max_points, track_xy, track_vis,
+                        total_samples, mapping, delta, loss_weight, loss, ws, F, H, W, depth_frame0, src_frame_lo,
+                        src_frame_hi, 1, stream, (double*)ws, 1, TrackOneVideo{}, false);
+}
+
 int fm_track_loss_fwd(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                       int num_segments, int max_rows, int max_points, const float* track_xy,
                       const unsigned char* track_vis, long long total_samples, int mapping, float delta,

@@ -5,7 +5,8 @@ flowmap/model/model_wrapper_overfit.py:51-73 drives.  Evaluated op by op it cost
 and several ATen launches per module; here the same surface runs on the two halves of the fused
 step (fm_overfit_step, FM_STEP_FORWARD / FM_STEP_BACKWARD):
 
-  * `Model.forward` launches nothing and returns a `LazyModelOutput`;
+  * `Model.forward` launches nothing and returns a `LazyModelOutput` (with ground-truth intrinsics an
+    ordinary ModelOutput that holds the batch's K: `fused_output`);
   * the first `LossFlow.forward` of the step runs the forward half (candidate sweep in the softmin
     stage, Procrustes poses, flow loss with its direct gradients) and returns the loss value as the
     output of an autograd node; `LossTracking.forward` adds the tracking sweep;
@@ -16,7 +17,7 @@ step (fm_overfit_step, FM_STEP_FORWARD / FM_STEP_BACKWARD):
 
 A network backbone (any backbone but BackboneExplicitDepth, e.g. the reference's BackboneMidas: a CNN
 for the depths, a per-pixel MLP or sigmoid(s * weights) for the correspondence weights) stays in
-torch.  `Model.forward` runs it once, under autograd, and the LazyModelOutput keeps its BackboneOutput.
+torch.  `Model.forward` runs it once, under autograd, and the step's output keeps its BackboneOutput.
 The root's inputs are then that step's depths and weights, converted to contiguous float32 inside the
 graph; the halves read them with weight sensitivity 0 (the weights themselves, not logits), and the
 root's backward hands d loss / d depths and d loss / d weights to autograd, which carries them on into
@@ -24,16 +25,22 @@ the network.  Outputs read before or after the losses reuse the stored BackboneO
 never runs twice in one step.
 
 A network backbone's batch of several videos (the pretraining step, pretrain.py) runs on the packed layout
-of fm_overfit_step_videos when its intrinsics are softmin without a regression stage and no tracks come
-with it: one candidate sweep and one focal length per video, and LossFlow's one pooled mask sum for the
-whole batch (loss_flow.py:31-70), written into every video's slot, so that the step's (B,) losses sum to
-the loss autograd sees and one grad_output scales them all.
+of fm_overfit_step_videos when its intrinsics are softmin without a regression stage, or ground truth, and no
+tracks come with it: one candidate sweep and one focal length per video (or each video's own per-frame K), and
+LossFlow's one pooled mask sum for the whole batch (loss_flow.py:31-70), written into every video's slot, so
+that the step's (B,) losses sum to the loss autograd sees and one grad_output scales them all.
+
+Ground-truth intrinsics (intrinsics_ground_truth.py) run the constant-intrinsics step for explicit depth, a
+network on one video and a network's batch alike, when `batch.intrinsics` is a floating (B, F, 3, 3) tensor on
+the flows' device: it is read into the step's k4 buffer before every forward half (a loader's new K, or the same
+tensor rewritten in place), without a host synchronisation or a check of its values, as in the reference; no
+focal length is learned and the snapshot reports k_mode "const".
 
 Anything the fused step does not cover (a consumer that reads `model_output.extrinsics` under
 autograd, several explicit-depth videos, a batch of several videos with a regressed focal length, a
-regression stage, ground-truth intrinsics or tracks, per-frame intrinsics, different mappings for the two
-losses) makes the LazyModelOutput materialise itself through the per-op autograd Functions of
-flowmap_b200.ops: same results, the former speed.
+regression stage or tracks, ground-truth intrinsics without a CUDA `batch.intrinsics`, eval mode, different
+mappings for the two losses) makes the step's output materialise itself through the per-op autograd
+Functions of flowmap_b200.ops: same results, the former speed.
 """
 from __future__ import annotations
 
@@ -98,6 +105,8 @@ class FusedStep:
         self.engine = eng
         eng.cfg.flow_weight, eng.cfg.flow_enable_after = loss_mod.cfg.weight, loss_mod.cfg.enable_after
         eng._msum.copy_(loss_mod._mask_total(self.flows))
+        if eng._gt:  # this step's K: a loader brings a new one with every batch, or rewrites it in place
+            eng._write_k4(self.batch.intrinsics)
         inputs = None
         if self.backbone_out is not None:  # the kernels read float32 rows; the casts stay in the graph
             bo = self.backbone_out
@@ -168,48 +177,60 @@ class FusedStep:
                 bo = model.backbone.forward(self.batch, self.flows)
             weights = bo.weights if model.cfg.use_correspondence_weights else torch.ones_like(bo.weights)
             return ModelOutput(bo.depths.detach(), None, k, ops.pose_chain(rt), weights.detach(), relative=rt, k4=k4,
-                               k_mode="shared_focal")
+                               k_mode="const" if eng._gt else "shared_focal")
+
+
+def _bind(out: ModelOutput, model, batch: Batch, flows: Flows, global_step: int,
+          backbone_out: Optional[BackboneOutput]):
+    """Make `out` the output of a fused step: `depths` is the parameter itself (explicit depth) or the network
+    backbone's output, as are a network backbone's `backward_correspondence_weights`; ModelOutput.__getattr__
+    takes every attribute that is not set from materialize(out)."""
+    d = out.__dict__
+    d["_fused"], d["_full"] = FusedStep(model, batch, flows, global_step, backbone_out), None
+    if backbone_out is None:
+        d["depths"] = model.backbone.depth[None]
+    else:
+        weights = backbone_out.weights
+        if not model.cfg.use_correspondence_weights:  # model.py:67-68
+            weights = torch.ones_like(weights)
+        d["depths"], d["backward_correspondence_weights"] = backbone_out.depths, weights
+
+
+def materialize(out: ModelOutput) -> ModelOutput:
+    """What the output of a fused step computes when it is read: before the losses the differentiable per-op
+    evaluation (which retires the fused step for this iteration), after them the detached snapshot of the step."""
+    d = out.__dict__
+    if d["_full"] is None:
+        fused = d["_fused"]
+        if fused.flow_done:  # the fused losses already consumed this output: values only
+            d["_full"] = fused.snapshot()
+        else:
+            fused.dead = True
+            d["_full"] = fused.model._forward_materialized(fused.batch, fused.flows, fused.global_step,
+                                                           fused.backbone_out)
+    return d["_full"]
 
 
 class LazyModelOutput(ModelOutput):
-    """ModelOutput of a fused step: `depths` is the parameter itself (explicit depth) or the network
-    backbone's output, as are a network backbone's `backward_correspondence_weights`; everything else is
-    computed when (and only if) somebody reads it: before the losses through the differentiable per-op
-    path (which retires the fused step for this iteration), after them as detached values of the step
-    the fused forward half evaluated."""
+    """ModelOutput of a fused step whose intrinsics come out of the step (a regressed focal length, or the softmin
+    sweep's): everything but `depths` (and a network backbone's weights) is computed when (and only if) somebody
+    reads it, through materialize()."""
 
     def __init__(self, model, batch: Batch, flows: Flows, global_step: int,
                  backbone_out: Optional[BackboneOutput] = None):
-        object.__setattr__(self, "_lazy", (model, batch, flows, global_step, backbone_out))
-        object.__setattr__(self, "_full", None)
-        object.__setattr__(self, "_fused", FusedStep(model, batch, flows, global_step, backbone_out))
-        if backbone_out is None:
-            object.__setattr__(self, "depths", model.backbone.depth[None])
-        else:
-            weights = backbone_out.weights
-            if not model.cfg.use_correspondence_weights:  # model.py:67-68
-                weights = torch.ones_like(weights)
-            object.__setattr__(self, "depths", backbone_out.depths)
-            object.__setattr__(self, "backward_correspondence_weights", weights)
+        _bind(self, model, batch, flows, global_step, backbone_out)
 
-    def _materialize(self) -> ModelOutput:
-        full = object.__getattribute__(self, "_full")
-        if full is None:
-            model, batch, flows, step, backbone_out = object.__getattribute__(self, "_lazy")
-            fused = object.__getattribute__(self, "_fused")
-            if fused.flow_done:  # the fused losses already consumed this output: values only
-                full = fused.snapshot()
-            else:
-                fused.dead = True
-                full = model._forward_materialized(batch, flows, step, backbone_out)
-            object.__setattr__(self, "_full", full)
-        return full
 
-    @property
-    def surfaces(self) -> Tensor:
-        return self._materialize().surfaces
-
-    def __getattr__(self, name):  # only reached for attributes not set in __init__
-        if name.startswith("__"):
-            raise AttributeError(name)
-        return getattr(self._materialize(), name)
+def fused_output(model, batch: Batch, flows: Flows, global_step: int,
+                 backbone_out: Optional[BackboneOutput] = None) -> ModelOutput:
+    """The output Model.forward returns for a step the losses evaluate on the fused halves.  With ground-truth
+    intrinsics the step does not change K: the output is an ordinary ModelOutput that holds the batch's intrinsics
+    and k_mode "const" (reading them keeps the step fused, as in the per-op path they are the batch's own), and
+    computes its poses, k4 and surfaces when they are read.  Otherwise a LazyModelOutput."""
+    from .model import IntrinsicsGroundTruth
+    if not isinstance(model.intrinsics, IntrinsicsGroundTruth):
+        return LazyModelOutput(model, batch, flows, global_step, backbone_out)
+    out = ModelOutput.__new__(ModelOutput)
+    _bind(out, model, batch, flows, global_step, backbone_out)
+    out.__dict__.update(intrinsics=batch.intrinsics, k_mode="const")
+    return out

@@ -92,7 +92,7 @@ class LossFlow(Loss):
 
     def compute_weighted_loss(self, batch, flows, tracks, model_output, global_step):
         out = model_output
-        fused = out.__dict__.get("_fused")  # flowmap_b200.fused.LazyModelOutput
+        fused = out.__dict__.get("_fused")  # the output of a fused step (flowmap_b200.fused)
         if fused is not None:
             value = fused.flow_loss(self, tracks)
             if value is not None:

@@ -274,19 +274,26 @@ class Model(nn.Module):
         but BackboneExplicitDepth, e.g. the reference's BackboneMidas) is judged on the BackboneOutput of
         the step: CUDA depths (B, F, H, W) and weights (B, F-1, H, W).  B > 1 (pretraining) takes one focal
         length per video: softmin intrinsics without a regression stage (the regressed focal length, and the
-        window of a regression stage, are one value for the whole batch in the reference)."""
-        b = batch.videos.shape[0]
+        window of a regression stage, are one value for the whole batch in the reference), or ground-truth K.
+        Ground-truth K must come as a floating (B, F, 3, 3) `batch.intrinsics` on the flows' device."""
+        b, f, _, h, w = batch.videos.shape
+        gt = isinstance(self.intrinsics, IntrinsicsGroundTruth)
         if not (self.fused_enabled and torch.is_grad_enabled() and self.training and
                 isinstance(self.extrinsics, ExtrinsicsProcrustes) and
-                isinstance(self.intrinsics, (IntrinsicsRegressed, IntrinsicsSoftmin)) and flows.forward.is_cuda):
+                isinstance(self.intrinsics, (IntrinsicsRegressed, IntrinsicsSoftmin, IntrinsicsGroundTruth)) and
+                flows.forward.is_cuda):
             return False
+        if gt:
+            k = batch.intrinsics
+            if not (isinstance(k, Tensor) and k.is_floating_point() and k.device == flows.forward.device and
+                    tuple(k.shape) == (b, f, 3, 3)):
+                return False
         if isinstance(self.backbone, BackboneExplicitDepth):
             return b == 1 and self.backbone.depth.is_cuda
         if backbone_out is None:
             return False
-        if b > 1 and not (isinstance(self.intrinsics, IntrinsicsSoftmin) and self.intrinsics.cfg.regression is None):
+        if b > 1 and not (gt or isinstance(self.intrinsics, IntrinsicsSoftmin) and self.intrinsics.cfg.regression is None):
             return False
-        _, f, _, h, w = batch.videos.shape
         d, wt = backbone_out.depths, backbone_out.weights
         return (isinstance(d, Tensor) and isinstance(wt, Tensor) and d.is_floating_point() and
                 wt.is_floating_point() and d.device == wt.device == flows.forward.device and
@@ -295,7 +302,7 @@ class Model(nn.Module):
     def _fused_params(self, global_step: int, inputs=None):
         """Tensors that receive a gradient from the fused step, in the order of FusedStep's buffers:
         the explicit-depth parameters, or a network backbone's float32 `inputs` (depths [, weights]) of
-        this step, then the focal length that is being learned."""
+        this step, then the focal length that is being learned (none for ground-truth K)."""
         if inputs is not None:
             params = list(inputs)
         else:
@@ -305,7 +312,8 @@ class Model(nn.Module):
         intr = self.intrinsics
         if isinstance(intr, IntrinsicsRegressed):
             params.append(intr.focal_length)
-        elif intr.cfg.regression is not None and global_step >= intr.cfg.regression.after_step:
+        elif (isinstance(intr, IntrinsicsSoftmin) and intr.cfg.regression is not None and
+              global_step >= intr.cfg.regression.after_step):
             params.append(intr.intrinsics_regressed.focal_length)
         return params
 
@@ -326,12 +334,14 @@ class Model(nn.Module):
             explicit = isinstance(self.backbone, BackboneExplicitDepth)
             soft = isinstance(self.intrinsics, IntrinsicsSoftmin)
             reg = ic.regression if soft else None
+            intrinsics = ("ground_truth" if isinstance(self.intrinsics, IntrinsicsGroundTruth) else
+                          "softmin" if soft else "regressed")
             # a network backbone's BackboneOutput holds the weights themselves: sensitivity 0 to the kernels
             cfg = OverfitCfg(
                 initial_depth=bc.initial_depth if explicit else 0.0,
                 weight_sensitivity=bc.weight_sensitivity if explicit else 0.0,
                 use_correspondence_weights=mc.use_correspondence_weights, procrustes_points=ec.num_points,
-                procrustes_randomize=ec.randomize_points, intrinsics="softmin" if soft else "regressed",
+                procrustes_randomize=ec.randomize_points, intrinsics=intrinsics,
                 softmin_points=ic.num_procrustes_points if soft else 8192,
                 softmin_min=ic.min_focal_length if soft else 0.5, softmin_max=ic.max_focal_length if soft else 2.0,
                 softmin_candidates=ic.num_candidates if soft else 60,
@@ -355,15 +365,15 @@ class Model(nn.Module):
         return eng
 
     def forward(self, batch: Batch, flows: Flows, global_step: int) -> ModelOutput:
-        from .fused import LazyModelOutput
+        from .fused import fused_output
         if isinstance(self.backbone, BackboneExplicitDepth):
             if self._fusable(batch, flows):
-                return LazyModelOutput(self, batch, flows, global_step)
+                return fused_output(self, batch, flows, global_step)
             return self._forward_materialized(batch, flows, global_step)
         # a network backbone runs once per step, under autograd as usual; the fused halves take its output
         backbone_out = self.backbone.forward(batch, flows)
         if self._fusable(batch, flows, backbone_out):
-            return LazyModelOutput(self, batch, flows, global_step, backbone_out)
+            return fused_output(self, batch, flows, global_step, backbone_out)
         return self._forward_materialized(batch, flows, global_step, backbone_out)
 
     def _forward_materialized(self, batch: Batch, flows: Flows, global_step: int,

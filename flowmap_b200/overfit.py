@@ -186,7 +186,7 @@ class FusedOverfitter(Overfitter):
     them: every step's depths and weights come from the network, through forward_phase, and only the
     split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight).
     Such a Model also takes a tensor batch of B > 1 videos of F frames (the reference's pretraining step:
-    softmin intrinsics without a regression stage, no tracks): the packed layout with F_b = F, whose rows are
+    softmin intrinsics without a regression stage, or ground-truth K, no tracks): the packed layout with F_b = F, whose rows are
     the network's (B, F, H, W) depths and (B, F-1, H, W) weights and the caller's (B, F-1, ...) Flows, which
     set_flows re-points to rather than copies.  Its mask_sum holds the pooled normaliser of LossFlow at b > 1
     in every video's slot, so that the (B,) losses sum to the batch's loss, and backward_phase takes one
@@ -195,8 +195,9 @@ class FusedOverfitter(Overfitter):
     cfg.intrinsics "ground_truth" (intrinsics_ground_truth.py, calibrated data) takes K as given: from
     `batch.intrinsics` (1, F, 3, 3), (B, F, 3, 3) for a tensor batch, or each Batch's own for a list, normalised
     as in the reference and possibly different for every frame.  There is no focal parameter and the step
-    computes no intrinsics gradient (fm_overfit_step with focal = g_k4 = track_g_k4 = NULL); set_intrinsics
-    swaps K in place.  Pair sharding does not serve it."""
+    computes no intrinsics gradient (fm_overfit_step with focal = g_k4 = track_g_k4 = NULL, and the split
+    forward's tracking sweep fm_track_loss_fwd_const_k); set_intrinsics swaps K in place.  Pair sharding does not
+    serve it."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda", model=None):
         self._layout, self._tensor_batch, self._network = None, False, False
@@ -223,8 +224,14 @@ class FusedOverfitter(Overfitter):
             self._init_one(cfg, batch, flows, tracks, device, model)
         self._init_step(cfg)
         if self._gt:
-            self.set_intrinsics(self.batch.intrinsics if self._layout is None or self._tensor_batch
-                                else [bt.intrinsics for bt in self.batches])
+            k = self.batch.intrinsics if self._layout is None or self._tensor_batch else \
+                [bt.intrinsics for bt in self.batches]
+            # a Model-bound optimiser serves the autograd surface, which rewrites K before every step and, like
+            # the reference, does not check its values
+            if model is None:
+                self.set_intrinsics(k)
+            else:
+                self._write_k4(k)
         if self._tensor_batch and not self._network:  # the parameters as (B, F, ...) / (B, F-1, ...) views
             self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
 
@@ -334,14 +341,17 @@ class FusedOverfitter(Overfitter):
 
     def _init_network_videos(self, cfg, batch, flows, tracks, model):
         """A network Model's tensor batch of several videos (see the class docstring): no parameter buffers,
-        one focal length per video from the softmin sweep."""
+        one focal length per video from the softmin sweep, or each video's own ground-truth K."""
         from ._lib import VideoLayout, lib
         import ctypes
         if tracks is not None or cfg.use_tracking:
             raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
-        if cfg.intrinsics != "softmin" or cfg.regression_after is not None:
+        if (self._gt != isinstance(model.intrinsics, IntrinsicsGroundTruth) or
+                not self._gt and (cfg.intrinsics != "softmin" or cfg.regression_after is not None)):
             raise ValueError("flowmap_b200: a network backbone's batch of several videos needs softmin intrinsics "
-                             "without a regression stage (one focal length per video)")
+                             "without a regression stage (one focal length per video), or ground-truth intrinsics, "
+                             f"in both cfg.intrinsics ({cfg.intrinsics!r}) and the bound model "
+                             f"({type(model.intrinsics).__name__})")
         B, f, _, h, w = batch.videos.shape
         dev = flows.forward.device
         self.cfg, self.model, self.models, self.losses, self.optimizer = cfg, model, [model], None, None
@@ -355,7 +365,7 @@ class FusedOverfitter(Overfitter):
         self._tables = video_tables(self.frames, dev)
         self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
         self._layout_ref = ctypes.byref(self._layout)
-        self._focal = torch.zeros(B, device=dev)
+        self._focal = None if self._gt else torch.zeros(B, device=dev)
         self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
         self._msum = self._mask_sum(self.flows).expand(B).contiguous()
 
@@ -741,13 +751,15 @@ class FusedOverfitter(Overfitter):
         c, L, pk = self.cfg, self._lib, self._packed
         _, f, _, h, w = self.batch.videos.shape
         st = torch.cuda.current_stream().cuda_stream
+        head = (_ptr(self._depth), _ptr(self._k4), _ptr(self._ext), _ptr(pk.seg), pk.num_segments, pk.max_rows,
+                pk.max_points, _ptr(pk.xy), _ptr(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta,
+                c.tracking_weight, _ptr(self._track_loss), _ptr(self._tws), f, h, w, 0, 0, f)
         with torch.cuda.device(self.rt.device):
             check(L.fm_pose_chain(_ptr(self.rt), _ptr(self._ext), 1, f, st), "fm_pose_chain")
-            check(L.fm_track_loss_fwd_sharded(
-                _ptr(self._depth), _ptr(self._k4), _ptr(self._ext), _ptr(pk.seg), pk.num_segments, pk.max_rows,
-                pk.max_points, _ptr(pk.xy), _ptr(pk.vis), pk.total, ops.MAPPINGS[c.mapping], c.delta,
-                c.tracking_weight, _ptr(self._track_loss), _ptr(self._tws), f, h, w, 0, 0, f, 1, st),
-                "fm_track_loss_fwd")
+            if self._gt:  # constant K: the sweep without intrinsics terms, as the backward half reads it
+                check(L.fm_track_loss_fwd_const_k(*head, st), "fm_track_loss_fwd_const_k")
+            else:
+                check(L.fm_track_loss_fwd_sharded(*head, 1, st), "fm_track_loss_fwd")
         return self._track_loss
 
     def backward_phase(self, flow_scale=None, track_scale=None, with_tracking: bool = False):
@@ -873,7 +885,18 @@ class FusedOverfitter(Overfitter):
         """Ground-truth intrinsics for the following steps, copied into the step's k4 buffer (captured CUDA
         graphs stay valid): (1, F, 3, 3) for one video, (B, F, 3, 3) for a tensor batch, a list of the videos'
         (1, F_b, 3, 3) for a list of Batches; normalised as in the reference.  ValueError on a missing, wrongly
-        shaped or non-finite K."""
+        shaped or non-finite K (the finiteness check synchronises with the host)."""
+        per = self._check_intrinsics(intrinsics)
+        finite = torch.isfinite(per.flatten(1)).all(1) if isinstance(per, Tensor) else \
+            torch.stack([torch.isfinite(k).all() for k in per])
+        bad = (~finite).nonzero()
+        if bad.numel():
+            raise ValueError(f"flowmap_b200: the intrinsics of video {int(bad[0, 0])} are not finite")
+        self._write_k4(intrinsics)
+
+    def _check_intrinsics(self, intrinsics):
+        """The shape checks of a ground-truth K (host only): the (B, F, 3, 3) tensor of one video or a tensor
+        batch, or the list of a list of Batches."""
         if not self._gt:
             raise ValueError("flowmap_b200: set_intrinsics needs cfg.intrinsics = 'ground_truth'")
         if intrinsics is None:
@@ -887,20 +910,25 @@ class FusedOverfitter(Overfitter):
                 raise ValueError(f"flowmap_b200: videos of different lengths need a list of {self.B} intrinsics")
             if intrinsics.dim() != 4:
                 raise ValueError(f"flowmap_b200: intrinsics must be (B, F, 3, 3), got {tuple(intrinsics.shape)}")
-            per = [intrinsics[i:i + 1] for i in range(intrinsics.shape[0])]
+            # a tensor holds videos of one length: video 0's shape stands for all of them
+            per = [intrinsics[:1]] * intrinsics.shape[0]
         if len(per) != self.B:
             raise ValueError(f"flowmap_b200: intrinsics for {len(per)} videos, the optimiser holds {self.B}")
-        rows = []
         for i, (k, f) in enumerate(zip(per, self.frames)):
             if k is None:
                 raise ValueError(f"flowmap_b200: video {i} carries no intrinsics (batch.intrinsics)")
             if tuple(k.shape) != (1, f, 3, 3):
                 raise ValueError(f"flowmap_b200: the intrinsics of video {i} must be (1, {f}, 3, 3), got "
                                  f"{tuple(k.shape)}")
-            if not bool(torch.isfinite(k).all()):
-                raise ValueError(f"flowmap_b200: the intrinsics of video {i} are not finite")
-            rows.append(ops.intrinsics_to_k4(k[0].to(device=self._k4.device, dtype=torch.float32)))
-        self._k4.copy_(torch.cat(rows))
+        return intrinsics if isinstance(intrinsics, Tensor) else per
+
+    def _write_k4(self, intrinsics):
+        """Copy a ground-truth K into the step's k4 buffer without synchronising the host: the shape checks of
+        set_intrinsics, no finiteness check (a non-finite K gives a non-finite loss, as in the reference).  A
+        tensor converts as one batched op."""
+        k = self._check_intrinsics(intrinsics)
+        k = k.reshape(-1, 3, 3) if isinstance(k, Tensor) else torch.cat([t[0].to(self._k4.device) for t in k])
+        self._k4.copy_(ops.intrinsics_to_k4(k))
 
     def intrinsics_k4(self) -> Tensor:
         """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for a (B, F) tensor batch; a list of

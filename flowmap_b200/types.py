@@ -73,11 +73,22 @@ class ModelOutput:
 
     @property
     def surfaces(self) -> Tensor:
+        if "_fused" in self.__dict__:  # the output of a fused step (flowmap_b200.fused): the step's own surfaces
+            from .fused import materialize
+            return materialize(self).surfaces
         if self._surfaces is None:
             from . import ops
             k4 = self.k4 if self.k4 is not None else ops.intrinsics_to_k4(self.intrinsics)
             self._surfaces = ops.unproject_depth(self.depths, k4)
         return self._surfaces
+
+    def __getattr__(self, name):
+        # only reached for attributes that are not set: those a fused step (flowmap_b200.fused) computes when they
+        # are read
+        if "_fused" not in self.__dict__ or name.startswith("__"):
+            raise AttributeError(name)
+        from .fused import materialize
+        return getattr(materialize(self), name)
 
 
 @dataclass

@@ -186,6 +186,15 @@ int fm_track_loss_fwd_sharded(const float* depth, const float* k4, const float* 
                               const unsigned char* track_vis, long long total_samples, int mapping, float delta,
                               float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
                               int src_frame_lo, int src_frame_hi, int shared_intrinsics, void* stream);
+/* fm_track_loss_fwd_sharded for constant intrinsics (ground truth): the sweep accumulates no intrinsics
+ * terms (6 values per target-row reduction instead of 10) and leaves in `ws` what the constant-intrinsics
+ * backward reads, fm_overfit_step's FM_STEP_BACKWARD with g_k4 == track_g_k4 == NULL.  k4 may differ from
+ * frame to frame.  Arguments as in fm_track_loss_fwd_sharded, which shared_intrinsics would not change. */
+int fm_track_loss_fwd_const_k(const float* depth, const float* k4, const float* extrinsics, const int* segments,
+                              int num_segments, int max_rows, int max_points, const float* track_xy,
+                              const unsigned char* track_vis, long long total_samples, int mapping, float delta,
+                              float loss_weight, float* loss, void* ws, int F, int H, int W, int depth_frame0,
+                              int src_frame_lo, int src_frame_hi, void* stream);
 int fm_track_loss_value(const void* ws, float loss_weight, float* loss, void* stream);
 int fm_track_loss_bwd_sharded(const float* depth, const float* k4, const float* extrinsics, const int* segments,
                               int num_segments, int max_rows, int max_points, const float* track_xy,
