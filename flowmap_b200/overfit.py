@@ -153,234 +153,201 @@ def _video(x, i: int):
     return replace(x, **{f.name: getattr(x, f.name)[i:i + 1] for f in fields(x) if getattr(x, f.name) is not None})
 
 
-class FusedOverfitter(Overfitter):
+class FusedOverfitter:
     """Same optimisation as :class:`Overfitter` (explicit-depth backbone, Procrustes poses,
     regressed focal length, flow [+ tracking] loss, Adam) but each step is ONE C-ABI call,
     fm_overfit_step: no autograd graph, no intermediate tensors, the sigmoid of the weight
     logits and its chain rule evaluated inside the kernels, gradients accumulated into a
     single buffer per parameter.
 
+    The constructor reads its inputs as B videos, each with its Batch, Flows, track segments and frame count
+    F_b, all of one H x W.  They come in one of three forms:
+
+    - one video: `batch.videos` (1, F, 3, H, W), Flows (1, F-1, ...), `tracks` a list of segments.  The
+      step is fm_overfit_step, whose buffers are the Model's own parameters, and which also serves the
+      split-step surface and pair sharding.
+    - a tensor batch: `batch.videos` (B, F, 3, H, W) with B > 1, Flows (B, F-1, ...): videos of one length.
+    - a list of B one-video Batches with a list of their Flows (1, F_b - 1, ...): videos of different lengths.
+
     Several videos run B INDEPENDENT overfits in one step (fm_overfit_step_videos).  Video b gets what a
     one-video FusedOverfitter on video b with the same cfg and step clock seed gets: its flow loss is
     normalised by its own mask sum, its tracking loss by its own valid count, and its gradients, Adam
-    moments, focal length, softmin window and poses are its own.  training_step() returns the (B,)
-    per-video totals, whose sum is the objective.  This differs on purpose from the reference's LossFlow
-    at b > 1 (pretraining), which normalises a batch by ONE pooled mask sum.  Shared by the batch: the
-    Procrustes point subset and the softmin point sample of each step.  The parameters live in packed
-    (T, H, W) / (T - B, H, W) / (B,) buffers, video b owning frames [fo_b, fo_b + F_b) and pairs
+    moments, focal length, softmin window and poses are its own.  This differs on purpose from the
+    reference's LossFlow at b > 1 (pretraining), which normalises a batch by ONE pooled mask sum.  Shared by
+    the batch: the Procrustes point subset and the softmin point sample of each step.  The parameters live
+    in buffers packed along the frame axis, video b owning frames [fo_b, fo_b + F_b) and pairs
     [fo_b - b, fo_b - b + F_b - 1); `models[b]` is video b's Model, whose parameters are views into them.
-    `tracks` is then a list of B segment lists, and the metrics log holds (steps, B) values.  Several
-    videos do not serve pair sharding or the split-step surface (but for a network Model's batch, below).
-    Two forms:
+    `tracks` is a list of B segment lists.  Several videos do not serve pair sharding or the split-step
+    surface (but for a network Model's batch, below).
 
-    - `batch.videos` of shape (B, F, 3, H, W) with B > 1 and Flows of shape (B, F-1, ...): videos of one
-      length, whose packed buffers are the (B, F, ...) / (B, F-1, ...) tensors.  training_step(),
-      extrinsics(), intrinsics_k4() and gradients() hand out (B, F [- 1], ...) views, and set_flows takes
-      one (B, F-1, ...) Flows.
-    - `batch` a list of B one-video Batches of the same H, W, `flows` a list of their Flows (1, F_b - 1, ...):
-      videos of different lengths.  training_step() returns the (B,) totals and a list of the videos'
-      relative poses; extrinsics(), intrinsics_k4() and gradients() hand out per-video lists.
+    Whatever takes or hands out one value per video follows the form: the buffer of one video, a
+    (B, F [- 1], ...) tensor for a tensor batch, a list for a list of Batches.  That holds for the totals
+    and poses of training_step(), extrinsics(), intrinsics_k4(), gradients(), set_flows, set_intrinsics
+    and the metrics log, whose rows are (steps,) for one video and (steps, B) for several.  `batches` holds
+    the videos' Batches in every form.
 
     Bound to a Model whose backbone is a network (any backbone but BackboneExplicitDepth, the drop-in
     surface of flowmap_b200.fused), the optimiser owns no depth or weight buffers and no Adam state for
     them: every step's depths and weights come from the network, through forward_phase, and only the
     split phases run (cfg.weight_sensitivity 0: the weights themselves, their gradient d loss / d weight).
-    Such a Model also takes a tensor batch of B > 1 videos of F frames (the reference's pretraining step:
-    softmin intrinsics without a regression stage, or ground-truth K, no tracks): the packed layout with F_b = F, whose rows are
-    the network's (B, F, H, W) depths and (B, F-1, H, W) weights and the caller's (B, F-1, ...) Flows, which
-    set_flows re-points to rather than copies.  Its mask_sum holds the pooled normaliser of LossFlow at b > 1
-    in every video's slot, so that the (B,) losses sum to the batch's loss, and backward_phase takes one
-    flow_scale for the whole batch.
+    Such a Model also takes a tensor batch (the reference's pretraining step: softmin intrinsics without a
+    regression stage, or ground-truth K, no tracks), whose rows are the network's depths and weights and
+    the caller's Flows, which set_flows re-points to rather than copies.  Its mask_sum holds the pooled
+    normaliser of LossFlow at b > 1 in every video's slot, so that the (B,) losses sum to the batch's loss,
+    and backward_phase takes one flow_scale for the whole batch.
 
     cfg.intrinsics "ground_truth" (intrinsics_ground_truth.py, calibrated data) takes K as given: from
-    `batch.intrinsics` (1, F, 3, 3), (B, F, 3, 3) for a tensor batch, or each Batch's own for a list, normalised
-    as in the reference and possibly different for every frame.  There is no focal parameter and the step
-    computes no intrinsics gradient (fm_overfit_step with focal = g_k4 = track_g_k4 = NULL, and the split
-    forward's tracking sweep fm_track_loss_fwd_const_k); set_intrinsics swaps K in place.  Pair sharding does not
-    serve it."""
+    each video's `batch.intrinsics`, normalised as in the reference and possibly different for every frame.
+    There is no focal parameter and the step computes no intrinsics gradient (fm_overfit_step with focal =
+    g_k4 = track_g_k4 = NULL, and the split forward's tracking sweep fm_track_loss_fwd_const_k);
+    set_intrinsics swaps K in place.  Pair sharding does not serve it."""
 
     def __init__(self, cfg: OverfitCfg, batch: Batch, flows: Flows, tracks=None, device="cuda", model=None):
-        self._layout, self._tensor_batch, self._network = None, False, False
-        self._gt = cfg.intrinsics == "ground_truth"
-        if isinstance(batch, (list, tuple)):
-            self._init_videos(cfg, list(batch), flows, tracks, device, model)
-        elif batch.videos.shape[0] > 1 and isinstance(model, Model) and \
-                not isinstance(model.backbone, BackboneExplicitDepth):
-            self._init_network_videos(cfg, batch, flows, tracks, model)
-        elif batch.videos.shape[0] > 1:
-            b, f = batch.videos.shape[:2]
-            if model is not None:
-                raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
-            if tracks is not None and len(tracks) != b:
-                raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({b})")
-            for name in _FLOW_NAMES:
-                if tuple(getattr(flows, name).shape[:2]) != (b, f - 1):
-                    raise ValueError(f"flowmap_b200: flows.{name} must hold (B, F-1) = ({b}, {f - 1}) pairs")
-            batch = batch.to(device)
-            self._init_videos(cfg, [_video(batch, i) for i in range(b)], [_video(flows, i) for i in range(b)],
-                              tracks, device, None)
-            self._tensor_batch, self.batch = True, batch
-        else:
-            self._init_one(cfg, batch, flows, tracks, device, model)
-        self._init_step(cfg)
-        if self._gt:
-            k = self.batch.intrinsics if self._layout is None or self._tensor_batch else \
-                [bt.intrinsics for bt in self.batches]
-            # a Model-bound optimiser serves the autograd surface, which rewrites K before every step and, like
-            # the reference, does not check its values
-            if model is None:
-                self.set_intrinsics(k)
-            else:
-                self._write_k4(k)
-        if self._tensor_batch and not self._network:  # the parameters as (B, F, ...) / (B, F-1, ...) views
-            self._depth, self._wlog = self._per_video(self._depth), self._per_video(self._wlog, pairs=True)
-
-    def _init_one(self, cfg, batch, flows, tracks, device, model):
-        """The one-video optimiser: its parameters are the Model's own tensors."""
-        if model is not None and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
-            raise ValueError(f"flowmap_b200: the bound model's intrinsics ({type(model.intrinsics).__name__}) do not "
-                             f"match cfg.intrinsics = {cfg.intrinsics!r}")
-        super().__init__(cfg, batch, flows, tracks, device, model=model)
-        _, f, _, h, w = batch.videos.shape
-        # the kernels read raw pointers: canonical (contiguous float32) copies, kept alive here
-        # (FlowPredictor.rescale_flow returns a permuted view, flow_predictor.py:40-49)
-        self.flows = Flows(*(ops._canon(getattr(self.flows, n), n) for n in _FLOW_NAMES))
-        dev = self.flows.forward.device
-        self.B, self.frames, self.T, self._hw = 1, [f], f, (h, w)
-        self._lead = ((1, f), (1, f - 1), ())  # leading dims of the per-frame, per-pair and per-video buffers
-        self._track_frames = None
-        self.models = [self.model]
-        if isinstance(self.model.backbone, BackboneExplicitDepth):
-            self._depth, self._wlog = self.model.backbone.depth.data, self.model.backbone.weights.data
-        else:  # a network backbone: the step's depths / weights arrive with forward_phase
-            self._network, self._depth, self._wlog = True, None, None
-        intr = self.model.intrinsics
-        if self._gt:
-            self._focal = None
-        elif cfg.intrinsics != "softmin":
-            self._focal = intr.focal_length.data
-        elif cfg.regression_after is not None:
-            self._focal = intr.intrinsics_regressed.focal_length.data
-        else:
-            self._focal = torch.zeros((), device=dev)
-        self._ws = ops.workspace(1, f, h, w, dev)
-        self._msum = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
-
-    def _init_videos(self, cfg, batches, flows, tracks, device, model):
-        """The packed optimiser of several videos (see the class docstring)."""
         from ._lib import VideoLayout, lib
         import ctypes
-        if model is not None:
+        listed = isinstance(batch, (list, tuple))
+        B = len(batch) if listed else batch.videos.shape[0]
+        one, tensor_batch = not listed and B == 1, not listed and B > 1
+        self.cfg, self._gt, self._tensor_batch = cfg, cfg.intrinsics == "ground_truth", tensor_batch
+        # bound to a caller's Model (the autograd drop-in surface, flowmap_b200.fused)
+        self._bound = model is not None
+        self._network = isinstance(model, Model) and not isinstance(model.backbone, BackboneExplicitDepth)
+
+        # ---- the videos: one (Batch, Flows) each, validated before anything reaches the device
+        if model is not None and (listed or tensor_batch and not self._network):
             raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
-        if not batches or not isinstance(flows, (list, tuple)) or len(flows) != len(batches):
+        if self._network and tensor_batch:
+            if tracks is not None or cfg.use_tracking:
+                raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
+            if (self._gt != isinstance(model.intrinsics, IntrinsicsGroundTruth) or
+                    not self._gt and (cfg.intrinsics != "softmin" or cfg.regression_after is not None)):
+                raise ValueError("flowmap_b200: a network backbone's batch of several videos needs softmin intrinsics "
+                                 "without a regression stage (one focal length per video), or ground-truth intrinsics, "
+                                 f"in both cfg.intrinsics ({cfg.intrinsics!r}) and the bound model "
+                                 f"({type(model.intrinsics).__name__})")
+        elif model is not None and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
+            raise ValueError(f"flowmap_b200: the bound model's intrinsics ({type(model.intrinsics).__name__}) do not "
+                             f"match cfg.intrinsics = {cfg.intrinsics!r}")
+        if listed and (not batch or not isinstance(flows, (list, tuple)) or len(flows) != B):
             raise ValueError("flowmap_b200: videos of different lengths need one Flows per Batch")
-        B = len(batches)
-        if cfg.use_tracking and (tracks is None or len(tracks) != B):
+        if not one and (cfg.use_tracking or tracks is not None) and (tracks is None or len(tracks) != B):
             raise ValueError(f"flowmap_b200: tracks must hold one segment list per video ({B})")
-        frames = []
-        for i, bt in enumerate(batches):
-            nb, f, _, h, w = bt.videos.shape
+        if tensor_batch:
+            for name in _FLOW_NAMES:
+                if tuple(getattr(flows, name).shape[:2]) != (B, batch.videos.shape[1] - 1):
+                    raise ValueError(f"flowmap_b200: flows.{name} must hold (B, F-1) = ({B}, "
+                                     f"{batch.videos.shape[1] - 1}) pairs")
+        videos = list(zip(batch, flows)) if listed else \
+            [(_video(batch, i), _video(flows, i)) for i in range(B)] if tensor_batch else [(batch, flows)]
+        h, w = videos[0][0].videos.shape[-2:]
+        for i, (bt, fl) in enumerate(videos):
+            nb, f = bt.videos.shape[:2]
             if nb != 1:
                 raise ValueError(f"flowmap_b200: video {i} must be a one-video Batch")
-            if (h, w) != tuple(batches[0].videos.shape[-2:]):
+            if tuple(bt.videos.shape[-2:]) != (h, w):
                 raise ValueError("flowmap_b200: the videos of one step need the same H x W")
             if f < 2:
                 raise ValueError(f"flowmap_b200: video {i} has {f} frame(s), a pair needs 2")
             for name in _FLOW_NAMES:
-                t = getattr(flows[i], name)
-                if tuple(t.shape[:4]) != (1, f - 1, h, w):
-                    raise ValueError(f"flowmap_b200: flows[{i}].{name} must hold (1, F_b-1, H, W) = (1, {f - 1}, {h}, {w})")
-            frames.append(f)
-        h, w = batches[0].videos.shape[-2:]
-        dev = torch.device(device)
-        self.cfg, self.B, self.frames = cfg, B, frames
-        self.T, self.P = sum(frames), sum(frames) - B
+                if tuple(getattr(fl, name).shape[:4]) != (1, f - 1, h, w):
+                    raise ValueError(f"flowmap_b200: flows[{i}].{name} must hold (1, F_b-1, H, W) = "
+                                     f"(1, {f - 1}, {h}, {w})")
+
+        # ---- one body for every form
+        if listed:
+            self.batches = [bt.to(device) for bt in batch]
+            self.batch = self.batches[0]
+        else:
+            self.batch = batch.to(device)
+            self.batches = [_video(self.batch, i) for i in range(B)] if tensor_batch else [self.batch]
+        frames = [bt.videos.shape[1] for bt in self.batches]
+        self.B, self.frames, self.T, self._hw = B, frames, sum(frames), (h, w)
         self._first = [sum(frames[:i]) for i in range(B)]
-        self._hw = (h, w)
-        self._lead = ((self.T,), (self.P,), (B,))
-        self._track_frames = frames
-        self.batches = [bt.to(device) for bt in batches]
-        self.batch = self.batches[0]
-        self.tracks = None if tracks is None else [[t.to(device) for t in v] for v in tracks]
-        self.global_step = self.optimizer_steps = self.focal_steps = 0
-        built = [build_model_and_losses(cfg, f, (h, w)) for f in frames]
-        self.models = [m.to(device) for m, _ in built]
-        self.model, self.losses, self.optimizer = self.models[0], built[0][1], None
-        # packed flows: the pairs of video b follow those of video b - 1
-        self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(dev), n)[0] for fl in flows]).contiguous()
-                             for n in _FLOW_NAMES))
-        self._tables = video_tables(frames, dev)
-        self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
-        self._layout_ref = ctypes.byref(self._layout)
+        T = self.T
+        # the kernels read raw pointers: canonical (contiguous float32) tensors, kept alive here
+        # (FlowPredictor.rescale_flow returns a permuted view, flow_predictor.py:40-49)
+        if one or self._network:  # the tensors given, or copies of those that are not contiguous
+            self.flows = self._canonical_flows(flows.to(device))
+        else:  # copies packed along the pair axis: the pairs of video b follow those of video b - 1
+            self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(device), n)[0] for _, fl in videos])
+                                 .contiguous() for n in _FLOW_NAMES))
+        dev = self.flows.forward.device
+        if one:  # the Uniform entry points, on the Model's own parameters
+            self._layout, self._track_frames = None, None
+            self._lead = ((1, T), (1, T - 1), ())  # leading dims of the per-frame, per-pair and per-video buffers
+            self.tracks = None if tracks is None else [t.to(device) for t in tracks]
+            self._ws = ops.workspace(1, T, h, w, dev)
+        else:  # the _videos entry points, on buffers packed along the frame axis
+            self._tables = video_tables(frames, dev)
+            self._layout = VideoLayout(B, T, *(t.data_ptr() for t in self._tables))
+            self._layout_ref = ctypes.byref(self._layout)
+            self._lead, self._track_frames = ((T,), (T - B,), (B,)), frames
+            self.tracks = None if tracks is None else [[t.to(device) for t in v] for v in tracks]
+            self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, T), dtype=torch.uint8, device=dev)
 
-        def pack(params):
-            buf = torch.cat([p.data for p in params]).contiguous()
-            o = 0
-            for p in params:
-                p.data = buf[o:o + p.shape[0]]
-                o += p.shape[0]
-            return buf
+        if model is None:
+            built = [build_model_and_losses(cfg, f, (h, w)) for f in frames]
+            self.models, self.losses = [m.to(device) for m, _ in built], built[0][1]
+        else:
+            self.models, self.losses = [model], None
+        self.model = self.models[0]
 
-        def stack(params):
-            buf = torch.stack([p.data for p in params]).contiguous()
-            for i, p in enumerate(params):
-                p.data = buf[i]
+        def gather(params, stack: bool):
+            """One buffer for the videos' `params`: the Model's own tensor for one video, else the videos' tensors
+            stacked or concatenated, which the parameters become views of."""
+            if one:
+                return params[0].data
+            buf = (torch.stack if stack else torch.cat)([p.data for p in params]).contiguous()
+            for p, part in zip(params, buf.unbind() if stack else buf.split([p.shape[0] for p in params])):
+                p.data = part
             return buf
-        self._depth = pack([m.backbone.depth for m in self.models])
-        self._wlog = pack([m.backbone.weights for m in self.models])
+        if self._network:  # the step's depths / weights arrive with forward_phase
+            self._depth = self._wlog = None
+        else:  # a tensor batch's are (B, F [- 1], H, W)
+            self._depth = gather([m.backbone.depth for m in self.models], tensor_batch)
+            self._wlog = gather([m.backbone.weights for m in self.models], tensor_batch)
         if self._gt:
             self._focal = None
         elif cfg.intrinsics != "softmin":
-            self._focal = stack([m.intrinsics.focal_length for m in self.models])
+            self._focal = gather([m.intrinsics.focal_length for m in self.models], True)
         elif cfg.regression_after is not None:
-            self._focal = stack([m.intrinsics.intrinsics_regressed.focal_length for m in self.models])
+            self._focal = gather([m.intrinsics.intrinsics_regressed.focal_length for m in self.models], True)
         else:
-            self._focal = torch.zeros(B, device=dev)
-        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
-        self._msum = self._video_mask_sums(self.flows)
+            self._focal = torch.zeros(self._lead[2], device=dev)
+        if self._network:  # LossFlow's pooled normaliser at b > 1, in every video's slot
+            pooled = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
+            self._msum = pooled.expand(self._lead[2]).contiguous()
+        else:
+            self._msum = self._video_mask_sums(self.flows)
+        self.global_step = 0
+        # torch.optim.Adam counts the updates each parameter has received, not the trainer's
+        # global_step (they differ when a run starts at global_step > 0 with a fresh optimiser, and
+        # for the focal length, which sees its first gradient at the softmin -> regressed hand-over)
+        self.optimizer_steps = self.focal_steps = 0
+        self._init_step(cfg)
+        if self._gt:
+            k = [bt.intrinsics for bt in self.batches] if listed else self.batch.intrinsics
+            # a Model-bound optimiser serves the autograd surface, which rewrites K before every step and, like
+            # the reference, does not check its values
+            if self._bound:
+                self._write_k4(k)
+            else:
+                self.set_intrinsics(k)
 
-    def _init_network_videos(self, cfg, batch, flows, tracks, model):
-        """A network Model's tensor batch of several videos (see the class docstring): no parameter buffers,
-        one focal length per video from the softmin sweep, or each video's own ground-truth K."""
-        from ._lib import VideoLayout, lib
-        import ctypes
-        if tracks is not None or cfg.use_tracking:
-            raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
-        if (self._gt != isinstance(model.intrinsics, IntrinsicsGroundTruth) or
-                not self._gt and (cfg.intrinsics != "softmin" or cfg.regression_after is not None)):
-            raise ValueError("flowmap_b200: a network backbone's batch of several videos needs softmin intrinsics "
-                             "without a regression stage (one focal length per video), or ground-truth intrinsics, "
-                             f"in both cfg.intrinsics ({cfg.intrinsics!r}) and the bound model "
-                             f"({type(model.intrinsics).__name__})")
-        B, f, _, h, w = batch.videos.shape
-        dev = flows.forward.device
-        self.cfg, self.model, self.models, self.losses, self.optimizer = cfg, model, [model], None, None
-        self.B, self.frames, self.T, self.P = B, [f] * B, B * f, B * (f - 1)
-        self._first = [i * f for i in range(B)]
-        self._hw, self._lead, self._track_frames = (h, w), ((self.T,), (self.P,), (B,)), self.frames
-        self.batch, self.tracks = batch, None
-        self.global_step = self.optimizer_steps = self.focal_steps = 0
-        self._network, self._tensor_batch, self._depth, self._wlog = True, True, None, None
-        self.flows = self._network_flows(flows, dev)
-        self._tables = video_tables(self.frames, dev)
-        self._layout = VideoLayout(B, self.T, *(t.data_ptr() for t in self._tables))
-        self._layout_ref = ctypes.byref(self._layout)
-        self._focal = None if self._gt else torch.zeros(B, device=dev)
-        self._ws = torch.empty(lib().fm_workspace_bytes_videos(B, self.T), dtype=torch.uint8, device=dev)
-        self._msum = self._mask_sum(self.flows).expand(B).contiguous()
-
-    def _network_flows(self, flows: Flows, device) -> Flows:
-        """A network batch's (B, F-1, ...) Flows as the packed (P, ...) rows: views of the caller's tensors
-        (copies only of tensors that are not contiguous)."""
+    def _canonical_flows(self, flows: Flows, device=None) -> Flows:
+        """Flows of this optimiser's (B, F-1, H, W, ...) shape on `device` (default: that of flows.forward), as
+        the contiguous float32 tensors the step reads: the tensors themselves, or copies of those that are not
+        contiguous."""
         want = (self.B, self.frames[0] - 1, *self._hw)
-        rows = []
+        canon = []
         for name in _FLOW_NAMES:
             t = ops._canon(getattr(flows, name), name)
+            device = device or t.device
             shape = want + (2,) if name in ("forward", "backward") else want
             if tuple(t.shape) != shape or t.device != device:
                 raise ValueError(f"flowmap_b200: flows.{name} must be a {shape} tensor on {device}")
-            rows.append(t.flatten(0, 1))
-        return Flows(*rows)
+            canon.append(t)
+        return Flows(*canon)
 
     def _init_step(self, cfg):
         """What one video and packed videos wire alike: the softmin buffers, the Adam state, the gradient
@@ -404,11 +371,10 @@ class FusedOverfitter(Overfitter):
             self.window = []
             self.injected_indices = None
         z = lambda t: None if t is None else torch.zeros_like(t)  # noqa: E731
-        self._state = [z(self._depth), z(self._depth), z(self._wlog), z(self._wlog), z(self._focal), z(self._focal)]
-        if self._network:
-            self._g_depth, self._g_w = torch.empty(T, h, w, device=dev), torch.empty(T - B, h, w, device=dev)
-        else:
-            self._g_depth, self._g_w = torch.empty_like(self._depth), torch.empty_like(self._wlog)
+        # the moments of the (T, H, W) depth and (T - B, H, W) logit rows: none for a network's depths and weights
+        rows = lambda n: None if self._network else torch.zeros(n, h, w, device=dev)  # noqa: E731
+        self._state = [rows(T), rows(T), rows(T - B), rows(T - B), z(self._focal), z(self._focal)]
+        self._g_depth, self._g_w = torch.empty(T, h, w, device=dev), torch.empty(T - B, h, w, device=dev)
         # ground-truth K: no focal parameter, and no intrinsics gradient buffers (the constant-intrinsics step)
         self._g_focal = z(self._focal)
         self._k4, self._g_k4 = torch.empty(T, 4, device=dev), None if self._gt else torch.empty(T, 4, device=dev)
@@ -460,8 +426,10 @@ class FusedOverfitter(Overfitter):
         self._mlog = None  # per-step metrics ring (enable_metrics_log)
 
     def _per_video(self, t: Tensor, pairs: bool = False):
-        """Views of a packed (T, ...) / (T - B, ...) buffer, one per video: a (B, F [- 1], ...) view for a
-        tensor batch, else a list."""
+        """Each video's rows of a (T, ...) frame buffer, or with `pairs` a (T - B, ...) pair buffer: the buffer
+        itself for one video, a (B, F [- 1], ...) view for a tensor batch, a list of views for a list of Batches."""
+        if self._layout is None:
+            return t
         if self._tensor_batch:
             return t.view(self.B, -1, *t.shape[1:])
         return [t[f0 - pairs * i:f0 - pairs * i + f - pairs] for i, (f0, f) in enumerate(zip(self._first, self.frames))]
@@ -480,9 +448,9 @@ class FusedOverfitter(Overfitter):
         prefetching loader) without rebuilding parameters or optimiser state.  `mask_sum` is the
         flow-loss normaliser (loss_flow.py:70) if the caller already has it.  Several videos: the new
         flows are copied into the packed buffers, from one (B, F-1, ...) Flows for a tensor batch, else
-        from a list of one Flows per video.  A network backbone's batch of several videos: the step reads the
-        new (B, F-1, ...) Flows themselves, and `mask_sum` (default: the pooled sum of all their masks) goes
-        to every video."""
+        from a list of one Flows per video.  One video, or a network backbone's batch of several: the step
+        reads the new Flows themselves, and `mask_sum` (default: the pooled sum of all their masks) goes to
+        every video."""
         if self._layout is not None and not self._network:
             if self._tensor_batch and isinstance(flows, Flows):
                 flows = [_video(flows, i) for i in range(flows.forward.shape[0])]
@@ -497,17 +465,7 @@ class FusedOverfitter(Overfitter):
                     dst[i].copy_(t[0])
             self._msum.copy_(self._video_mask_sums(self.flows) if mask_sum is None else mask_sum)
             return
-        old = self.flows
-        if self._layout is not None:
-            flows = self._network_flows(flows, old.forward.device)
-        else:
-            canon = {}
-            for name in _FLOW_NAMES:
-                t = ops._canon(getattr(flows, name), name)
-                if t.shape != getattr(old, name).shape or t.device != getattr(old, name).device:
-                    raise ValueError(f"flowmap_b200: `{name}` does not match the optimiser's shapes / device")
-                canon[name] = t
-            flows = Flows(canon["forward"], canon["backward"], canon["forward_mask"], canon["backward_mask"])
+        flows = self._canonical_flows(flows, self.flows.forward.device)
         self.flows = flows  # the canonical tensors stay referenced while the kernels hold their pointers
         a = self._args
         a.fflow, a.bflow = flows.forward.data_ptr(), flows.backward.data_ptr()
@@ -520,9 +478,9 @@ class FusedOverfitter(Overfitter):
         return ops.mask_sum(flows.forward_mask, flows.backward_mask)
 
     def _video_mask_sums(self, flows: Flows) -> Tensor:
-        """(B,) float64: each video's own flow-loss normaliser."""
+        """Each video's own flow-loss normaliser, float64: a scalar for one video, else (B,)."""
         fm, bm = self._per_video(flows.forward_mask, pairs=True), self._per_video(flows.backward_mask, pairs=True)
-        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(self.B)])
+        return torch.stack([ops.mask_sum(fm[i], bm[i]) for i in range(self.B)]).reshape(self._lead[2])
 
     def _adam_frames(self, i: int, lo: int, hi: int):
         """Adam (step clock) on frames lo <= f < hi of parameter i (0 depth, 1 weight logits); several videos:
@@ -607,11 +565,23 @@ class FusedOverfitter(Overfitter):
         else:
             check(L.fm_softmin_sweep_bwd(*head, 1, self.T, h, w, stream), "fm_softmin_sweep_bwd")
 
+    def _early_moments(self, stream):
+        """The step's Procrustes moment pass on the candidate-0 intrinsics (see _step_softmin), on the CUDA
+        stream handle `stream`."""
+        from ._lib import check
+        L, (h, w) = self._lib, self._hw
+        wl, sens = self._weight_args()
+        head = (_ptr(self._depth), _ptr(self._k4_base), _ptr(self.flows.backward), wl, sens, _ptr(self._ws))
+        if self._layout is not None:
+            check(L.fm_procrustes_moments_videos(*head, self._layout_ref, h, w, stream), "fm_procrustes_moments_videos")
+        else:
+            check(L.fm_procrustes_moments(*head, self.T, h, w, stream), "fm_procrustes_moments")
+
     def _window(self, split: bool = False):
         """The hand-over window of the softmin stage (intrinsics_softmin.py:133-139): on the split step
         of a bound model that has one, the model's own list (drop-in surface), else this optimiser's."""
         intr = self.model.intrinsics
-        return intr.window if split and hasattr(intr, "window") and self.optimizer is None else self.window
+        return intr.window if split and hasattr(intr, "window") and self._bound else self.window
 
     def _window_open(self) -> bool:
         """Whether this step's sweep estimate joins the hand-over window."""
@@ -633,11 +603,9 @@ class FusedOverfitter(Overfitter):
     def _step_softmin(self, update: bool):
         """Sweep stage (intrinsics_softmin.py:84-141): focal estimate from the candidate sweep,
         the step itself with that focal length, the sweep's backward, then Adam."""
-        from ._lib import check
-        c, a, L = self.cfg, self._args, self._lib
-        f, (h, w) = max(self.frames), self._hw
+        c, a = self.cfg, self._args
+        f, w = max(self.frames), self._hw[1]
         st = torch.cuda.current_stream().cuda_stream
-        rag = self._layout is not None
         # All-pixel Procrustes: the moment pass of the step does not have to wait for the focal length
         # the sweep is about to produce -- the sums for one K follow exactly from the sums for another
         # (fm_overfit_step_args.moments_k4) -- so it runs beside the sweep, on the candidate-0 intrinsics.
@@ -646,14 +614,7 @@ class FusedOverfitter(Overfitter):
         with torch.cuda.device(self.rt.device):
             if early_moments:
                 self._side_stream.wait_stream(cur)
-                wl, sens = self._weight_args()
-                if rag:
-                    check(L.fm_procrustes_moments_videos(_ptr(self._depth), _ptr(self._k4_base),
-                                                         _ptr(self.flows.backward), wl, sens, _ptr(self._ws),
-                                                         self._layout_ref, h, w, st), "fm_procrustes_moments_videos")
-                else:
-                    check(L.fm_procrustes_moments(_ptr(self._depth), _ptr(self._k4_base), _ptr(self.flows.backward),
-                                                  wl, sens, _ptr(self._ws), f, h, w, st), "fm_procrustes_moments")
+                self._early_moments(st)
             with torch.cuda.stream(self._side_stream if early_moments else cur):
                 idx = self._sweep_indices(clocked=update)
                 self._sweep_forward(idx, torch.cuda.current_stream().cuda_stream)
@@ -663,7 +624,8 @@ class FusedOverfitter(Overfitter):
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
             # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
-            fuse = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and not rag
+            fuse = (update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and
+                    self._layout is None)
             a.focal = _ptr(self._sw_focal)
             a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
             a.defer_adam = 1 if fuse else 0
@@ -860,26 +822,19 @@ class FusedOverfitter(Overfitter):
             self.global_step += 1
             self.optimizer_steps += 1
             self.focal_steps += int(ticks_focal)
-        if self._layout is not None:
-            return self._total.clone(), self._per_video(self.rt, pairs=True)
-        return self._total.clone(), self.rt
+        return self._total.clone(), self._per_video(self.rt, pairs=True)
 
     def extrinsics(self) -> Tensor:
         """Camera-to-world poses of the last step (projection.py:187-210): (B, F, 4, 4), or a list of
         (F_b, 4, 4) for videos of different lengths."""
-        if self._layout is None or self._tensor_batch:
-            return ops.pose_chain(self.rt if self._layout is None else self._per_video(self.rt, pairs=True))
-        return [ops.pose_chain(r[None])[0] for r in self._per_video(self.rt, pairs=True)]
+        rt = self._per_video(self.rt, pairs=True)
+        return ops.pose_chain(rt) if isinstance(rt, Tensor) else [ops.pose_chain(r[None])[0] for r in rt]
 
     def gradients(self):
         """d loss / d depth, weights and focal length of the last step; "focal" is None with ground-truth K."""
-        if self._layout is None:
-            return {"depth": self._g_depth, "weights": self._g_w, "focal": self._g_focal}
-        g_focal = self._g_focal
-        if g_focal is not None and not self._tensor_batch:
-            g_focal = list(g_focal.unbind())
-        return {"depth": self._per_video(self._g_depth), "weights": self._per_video(self._g_w, pairs=True),
-                "focal": g_focal}
+        depth, g_focal = self._per_video(self._g_depth), self._g_focal
+        return {"depth": depth, "weights": self._per_video(self._g_w, pairs=True),
+                "focal": g_focal if g_focal is None or isinstance(depth, Tensor) else list(g_focal.unbind())}
 
     def set_intrinsics(self, intrinsics):
         """Ground-truth intrinsics for the following steps, copied into the step's k4 buffer (captured CUDA
@@ -933,7 +888,7 @@ class FusedOverfitter(Overfitter):
     def intrinsics_k4(self) -> Tensor:
         """(F, 4) = (fx, fy, cx, cy) used by the last step; (B, F, 4) for a (B, F) tensor batch; a list of
         (F_b, 4) for videos of different lengths."""
-        return self._k4 if self._layout is None else self._per_video(self._k4)
+        return self._per_video(self._k4)
 
     METRIC_NAMES = ("train/loss/flow", "train/loss/tracking", "train/intrinsics/fx_error",
                     "train/intrinsics/fy_error", "metrics/ate")
@@ -953,37 +908,28 @@ class FusedOverfitter(Overfitter):
         val_check_interval: 1) evaluates the updated parameters: that is row k + 1."""
         if capacity < 1:
             raise ValueError("flowmap_b200: the metrics log needs a capacity >= 1")
-        b, dev, B = self.batch, self.rt.device, self.B
-        nan = float("nan")
-        one = self._layout is None
-        if not one:  # each video's own Batch; the camera centres packed like the frames
-            gts, fxfy = [], []
-            for bt, fb in zip(self.batches, self.frames):
-                gts.append(torch.full((fb, 3), nan, device=dev) if bt.extrinsics is None else
-                           bt.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32))
-                k = None if bt.intrinsics is None else bt.intrinsics[0].double()
-                fxfy.append(torch.tensor([nan, nan], dtype=torch.float64) if k is None else
-                            torch.stack((k[:, 0, 0].mean(), k[:, 1, 1].mean())).cpu())
-            self._mlog_gt = torch.cat(gts).contiguous()
-            self._mlog_fxfy = torch.stack(fxfy).to(device=dev, dtype=torch.float32).contiguous()
-            fx = fy = nan
-        else:
-            self._mlog_gt = None if b.extrinsics is None else \
-                b.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32).contiguous()
-            if b.intrinsics is None:
-                fx = fy = nan
-            else:
-                k = b.intrinsics[0].double()
-                fx, fy = float(k[:, 0, 0].mean()), float(k[:, 1, 1].mean())
+        dev, nan = self.rt.device, float("nan")
+        gts, fxfy = [], []  # each video's ground truth
+        for bt in self.batches:
+            gts.append(None if bt.extrinsics is None else
+                       bt.extrinsics[0, :, :3, 3].to(device=dev, dtype=torch.float32))
+            k = None if bt.intrinsics is None else bt.intrinsics[0].double()
+            fxfy.append(torch.tensor([nan, nan], dtype=torch.float64) if k is None else
+                        torch.stack((k[:, 0, 0].mean(), k[:, 1, 1].mean())).cpu())
+        # the camera centres packed like the frames, NaN for a video without them; none at all: no ATE
+        self._mlog_gt = None if all(g is None for g in gts) else torch.cat(
+            [torch.full((f, 3), nan, device=dev) if g is None else g for g, f in zip(gts, self.frames)]).contiguous()
+        fxfy = torch.stack(fxfy)
+        self._mlog_fxfy = fxfy.to(device=dev, dtype=torch.float32).contiguous()
         if getattr(self, "_ext", None) is None:  # flow-only steps chain the poses for the log
             self._ext = torch.empty(*self._lead[0], 4, 4, device=dev)
-        self._mlog = torch.full((capacity, 5) if one else (capacity, B, 5), nan, device=dev)
+        self._mlog = torch.full((capacity, *self._lead[2], 5), nan, device=dev)
         self._mlog_first = self.optimizer_steps
         a = self._args
         a.extrinsics = self._ext.data_ptr()
         a.gt_positions = None if self._mlog_gt is None else self._mlog_gt.data_ptr()
-        a.gt_fx, a.gt_fy, a.metrics_capacity = fx, fy, capacity
-        a.gt_fxfy = None if one else self._mlog_fxfy.data_ptr()
+        # the one-video step reads its video's fx / fy as scalars, packed videos the (B, 2) rows
+        (a.gt_fx, a.gt_fy), a.gt_fxfy, a.metrics_capacity = fxfy[0].tolist(), self._mlog_fxfy.data_ptr(), capacity
         self._graphs.clear()  # captured steps were recorded without the log
         self._eager_runs.clear()
 
