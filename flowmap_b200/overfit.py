@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 from torch import Tensor
 
-from . import ops
+from . import checkpoint, ops
 from .loss import (LossFlowCfg, LossTrackingCfg, MappingHuberCfg, MappingL1Cfg, MappingL2Cfg,
                    get_losses)
 from .model import (BackboneExplicitDepth, BackboneExplicitDepthCfg, ExtrinsicsProcrustesCfg, IntrinsicsGroundTruth,
@@ -944,6 +944,61 @@ class FusedOverfitter:
         rows = self._mlog[(steps % cap).to(self._mlog.device)].cpu()
         return {name: rows[..., i] for i, name in enumerate(self.METRIC_NAMES)}
 
+    # ---- checkpoints: the format and the interchange with torch.optim.Adam live in flowmap_b200.checkpoint
+    def _refuse_checkpoint(self):
+        if self._bound:
+            raise ValueError("flowmap_b200: an optimiser bound to a caller's Model (model=) keeps no Adam state: "
+                             "checkpoint the Model and the caller's torch optimiser")
+
+    def _adam_slots(self, b: int):
+        """Video b's Adam state as torch.optim.Adam holds it for models[b].parameters(): per parameter its
+        (exp_avg, exp_avg_sq) views of the packed moments and its update count."""
+        s, f0, f = self._state, self._first[b], self.frames[b]
+        rows = lambda t, p: t if self._layout is None else t[f0 - p * b:f0 - p * b + f - p]  # noqa: E731
+        moments = [(rows(s[0], 0), rows(s[1], 0)), (rows(s[2], 1), rows(s[3], 1))]
+        if s[4] is not None:  # softmin without a regression stage has a buffer here but no focal parameter
+            moments.append((s[4], s[5]) if self._layout is None else (s[4][b], s[5][b]))
+        steps = checkpoint.adam_steps(self.cfg, self.optimizer_steps, self.focal_steps)
+        return [(m, v, n) for (m, v), n in zip(moments, steps)]
+
+    def state_dict(self) -> dict:
+        """The run's state (flowmap_b200.checkpoint): each video's Model.state_dict() and torch.optim.Adam
+        state, the step counters, the softmin hand-over window and the step clock's seed; not the settings
+        use_cuda_graph and injected_indices, nor the metrics log.  No host synchronisation: the tensors are
+        clones on the optimiser's device, made on the current stream (Adam's `step` entries are CPU scalars,
+        as in torch).  A run under cfg.procrustes_randomize draws its point sets from torch's RNG, which is
+        not saved: its resumed point sets differ from those of the uninterrupted run."""
+        self._refuse_checkpoint()
+        videos = [checkpoint.video_entry(f, {k: t.clone() for k, t in m.state_dict().items()}, self._adam_slots(b),
+                                         self.cfg.lr) for b, (m, f) in enumerate(zip(self.models, self.frames))]
+        window = torch.stack(self.window) if self._softmin and self.window else None
+        return checkpoint.new_state(self.cfg, self.global_step, self.optimizer_steps, self.focal_steps,
+                                    self._clock.base_seed, window, videos)
+
+    def load_state_dict(self, state: dict) -> None:
+        """Continue the run of `state` on this optimiser, built on the same inputs: parameters and moments
+        are copied into the packed buffers in place (captured CUDA graphs stay valid), the counters, window
+        and seed replace this optimiser's.  ValueError naming the field when the format, cfg, number of
+        videos, frames per video, H x W or intrinsics mode differ; the Flows, tracks and ground-truth K are
+        inputs, not state."""
+        self._refuse_checkpoint()
+        checkpoint.check(state, self.cfg, self.frames, self._hw)
+        with torch.no_grad():
+            for b, (m, v) in enumerate(zip(self.models, state["videos"])):
+                m.load_state_dict(v["model"])  # copy_ into the parameters: views of the packed buffers
+                checkpoint.load_moments(v["optimizer"], self._adam_slots(b))
+        self.global_step, self.optimizer_steps, self.focal_steps = (
+            int(state[k]) for k in ("global_step", "optimizer_steps", "focal_steps"))
+        if self._softmin:
+            w = state["window"]
+            self.window = [] if w is None else list(w.to(self.rt.device).clone().unbind(0))
+        seed = int(state["base_seed"])
+        if seed != self._clock.base_seed:  # a captured step holds the seed as a launch argument of its tick
+            self._clock.base_seed = seed
+            self._graphs.clear()
+            self._eager_runs.clear()
+        self._clock.set(self.optimizer_steps, self.focal_steps)
+
 
 class ShardedFusedOverfitter(FusedOverfitter):
     """Pair-sharded :class:`FusedOverfitter` (flowmap_b200.parallel, SURVEY 8(e)).
@@ -1002,6 +1057,10 @@ class ShardedFusedOverfitter(FusedOverfitter):
     def enable_metrics_log(self, capacity: int):
         raise ValueError("flowmap_b200: the per-step metrics log covers the single-GPU FusedOverfitter; a "
                          "pair-sharded rank holds only part of the trajectory")
+
+    def _refuse_checkpoint(self):
+        raise ValueError("flowmap_b200: checkpoints cover the single-GPU FusedOverfitter; a pair-sharded rank "
+                         "holds only part of the video's state")
 
     def _mask_sum(self, flows: Flows) -> Tensor:
         from . import parallel
