@@ -103,7 +103,7 @@ class OverfitStepArgs(ctypes.Structure):
                 ("phase", c_int),
                 ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P),
                 ("gt_positions", _P), ("gt_fx", c_float), ("gt_fy", c_float), ("metrics_log", _P),
-                ("metrics_capacity", c_int), ("B", c_int), ("gt_fxfy", _P)]
+                ("metrics_capacity", c_int), ("video_grad_scales", c_int), ("B", c_int), ("gt_fxfy", _P)]
 
 
 class VideoLayout(ctypes.Structure):

@@ -27,6 +27,8 @@
 #include <string.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "../../include/flowmap_b200.h"
 #include "fm_ate.cuh"
 #include "fm_host.h"
@@ -107,8 +109,19 @@ Workspace carve(void* base, int B, int F) { return carve_rows(base, B, (size_t)B
 struct NoScale {
   __host__ __device__ NoScale(const float*) {}
 };
+// One d total / d loss_b for every video b, a device (B,) array (NULL = 1): the split backward of B networks'
+// videos (fm_overfit_step_args.video_grad_scales), where autograd hands every video its own grad_output.
+struct VideoScales {
+  __host__ __device__ VideoScales(const float* p) : s(p) {}
+  const float* s;
+};
+// The scale type of the Procrustes backward's flow-loss part: one device scalar, or VideoScales.
+using FlowScale = const float* __restrict__;
 __device__ __forceinline__ double scale_of(const float* s) { return s ? (double)*s : 1.0; }
-__device__ __forceinline__ double scale_of(NoScale) { return 1.0; }
+// ... of video b
+__device__ __forceinline__ double scale_of(const float* s, int) { return scale_of(s); }
+__device__ __forceinline__ double scale_of(NoScale, int) { return 1.0; }
+__device__ __forceinline__ double scale_of(VideoScales v, int b) { return v.s ? (double)__ldg(v.s + b) : 1.0; }
 struct Videos {
   using Scale = NoScale;
   const int* frame_offset;  // [B + 1]
@@ -124,6 +137,10 @@ struct Videos {
 // Videos instances keep their code.
 struct VideosScaled : Videos {
   using Scale = const float* __restrict__;
+};
+// ... and with one d total / d flow loss per video (VideoScales): the split backward of B networks' videos.
+struct VideosEachScaled : Videos {
+  using Scale = VideoScales;
 };
 // B videos of F frames each in the (B F, ...) and (B (F - 1), ...) buffers: one video (B = 1) and the
 // standalone (B, F) entry points.  Pair p of video b joins frames p + b and p + b + 1, as in Videos.
@@ -924,17 +941,25 @@ __global__ void k_flow_video_loss(const double* __restrict__ flowacc, float* __r
 }
 
 // ================================================================== phase D1: adjoint solve
+// d total / d flow loss of a pair: the one scalar, or (VideoScales) that of the pair's video
 template <class Lay>
+__device__ __forceinline__ double pair_scale(const float* s, const Lay&, int) { return s ? (double)*s : 1.0; }
+template <class Lay>
+__device__ __forceinline__ double pair_scale(VideoScales s, const Lay& lay, int pair) {
+  return scale_of(s, lay.of_pair(pair));
+}
+
+template <class Lay, class S = FlowScale>
 __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* __restrict__ state,
                           const float* __restrict__ g_rt, int include_flow,
-                          const float* __restrict__ flow_scale, PairAdjoint* __restrict__ adj, int BP, Lay lay) {
+                          S flow_scale, PairAdjoint* __restrict__ adj, int BP, Lay lay) {
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= BP) return;
   double g[12];
   for (int k = 0; k < 12; ++k) g[k] = 0.0;
   if (include_flow) {
     flow_pose_grad(flowacc, state, nullptr, pair, lay, g);
-    const double s = flow_scale ? (double)*flow_scale : 1.0;
+    const double s = pair_scale(flow_scale, lay, pair);
     for (int k = 0; k < 12; ++k) g[k] *= s;
   }
   if (g_rt) for (int k = 0; k < 12; ++k) g[k] += (double)g_rt[(size_t)pair * 12 + k];
@@ -1300,9 +1325,9 @@ k_distribute_window(FM_DISTRIBUTE_DENSE_PARAMS, Lay lay, AdamFuse adam, int H, i
 }
 #undef FM_DISTRIBUTE_DENSE_PARAMS
 
-template <class Lay>
+template <class Lay, class S = FlowScale>
 __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
-                              int include_flow, const float* __restrict__ flow_scale,
+                              int include_flow, S flow_scale,
                               float* __restrict__ g_k4, int T, Lay lay) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
@@ -1310,7 +1335,7 @@ __global__ void k_k4_finalize(const double* __restrict__ k4acc, const double* __
   if (include_flow) {  // flow_k4_grad on video b's own frames
     const int b = lay.of_frame(t), f0 = lay.first(b);
     flow_k4_grad(flowacc + (size_t)f0 * kFlowAcc, t - f0, lay.frames(b), g);
-    const double s = flow_scale ? (double)*flow_scale : 1.0;
+    const double s = scale_of(flow_scale, b);
     for (int k = 0; k < 4; ++k) g[k] *= s;
   }
   for (int k = 0; k < 4; ++k) g_k4[(size_t)t * 4 + k] = (float)(g[k] + k4acc[(size_t)t * 4 + k]);
@@ -1321,6 +1346,19 @@ __global__ void k_scale_inplace(float* __restrict__ buf, const float* __restrict
   if (s == 1.0f) return;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     buf[i] *= s;
+}
+
+// k_scale_inplace with one scale per video: frame row t of the (T, frame_elems) buffer times scale[video of t]
+// (NULL scale: nothing to do).  Row-major blocks: blockIdx.y strides the frames.
+__global__ void k_scale_videos(float* __restrict__ buf, const float* __restrict__ scale,
+                               const int* __restrict__ frame_video, size_t frame_elems, int T) {
+  for (int t = blockIdx.y; t < T; t += gridDim.y) {
+    const float s = __ldg(scale + __ldg(frame_video + t));
+    if (s == 1.0f) continue;
+    float* row = buf + (size_t)t * frame_elems;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < frame_elems; i += (size_t)gridDim.x * blockDim.x)
+      row[i] *= s;
+  }
 }
 
 // ================================================================== mask sum
@@ -1836,10 +1874,15 @@ __host__ __device__ constexpr size_t track_smem_bytes(int max_rows, int list_cap
 // go to, and how d total / d tracking loss comes (Scale, as for the video layouts).
 // kPerFrameK: whether the layout serves a per-frame intrinsics GRADIENT (k_track_src<false, true, TL>); every
 // layout reads each frame's own k4 row.
+// scale(): weight * d total / d loss / valid count of frame f's video (track_scale, defined below).
+__device__ __forceinline__ double track_scale(const double* sums, float loss_weight, const float* go);
 struct TrackOneVideo {  // one video, or the standalone op: the one pair at sums[0], sums[1]
   static constexpr bool kPerFrameK = true;  // per-frame intrinsics as well as one shared focal length
   using Scale = Uniform::Scale;
   template <class T> __device__ __forceinline__ T* sums_of(T* sums, int) const { return sums; }
+  __device__ __forceinline__ double scale(const double* sums, int f, float loss_weight, Scale go) const {
+    return track_scale(sums_of(sums, f), loss_weight, go);
+  }
 };
 struct TrackVideos {  // videos packed along the frame axis: frame f's video b has the pair sums[2 b], sums[2 b + 1]
   static constexpr bool kPerFrameK = false;  // one focal length per video, or constant intrinsics
@@ -1847,6 +1890,19 @@ struct TrackVideos {  // videos packed along the frame axis: frame f's video b h
   const int* frame_video;
   template <class T>
   __device__ __forceinline__ T* sums_of(T* sums, int f) const { return sums + 2 * __ldg(frame_video + f); }
+  __device__ __forceinline__ double scale(const double* sums, int f, float loss_weight, Scale) const {
+    return track_scale(sums_of(sums, f), loss_weight, nullptr);
+  }
+};
+// ... with one d total / d tracking loss per video (the split backward of B networks' videos)
+struct TrackVideosScaled : TrackVideos {
+  using Scale = VideoScales;
+  __device__ __forceinline__ double scale(const double* sums, int f, float loss_weight, Scale go) const {
+    const int b = __ldg(frame_video + f);
+    double cnt = sums[2 * b + 1];
+    if (cnt == 0.0) cnt = 1.0;  // as track_scale, in its order of operations
+    return (double)loss_weight * scale_of(go, b) / cnt;
+  }
 };
 
 template <bool SHARED_K, bool KGRAD, class TL>
@@ -2081,9 +2137,6 @@ __device__ __forceinline__ double track_scale(const double* sums, float loss_wei
   if (cnt == 0.0) cnt = 1.0;  // loss_tracking.py:61 "valid_sum or 1"
   return (double)loss_weight * (go ? (double)*go : 1.0) / cnt;
 }
-__device__ __forceinline__ double track_scale(const double* sums, float loss_weight, NoScale) {
-  return track_scale(sums, loss_weight, nullptr);
-}
 
 // The tracking losses of B videos: thread b reads video b's loss sum / valid count.
 __global__ void k_track_video_loss(const double* __restrict__ sums, float loss_weight, float* __restrict__ loss, int B) {
@@ -2105,7 +2158,7 @@ k_track_apply(const float* __restrict__ k4, const int* __restrict__ seg, const f
   if (row >= si.rows || p >= si.n || !sh.owns(si.start_frame + row)) return;
   const size_t sidx = (size_t)si.sample_start + (size_t)row * si.n + p;
   if (!flag[sidx]) return;
-  const float scale = (float)track_scale(tl.sums_of(sums, si.start_frame), loss_weight, go);
+  const float scale = (float)tl.scale(sums, si.start_frame, loss_weight, go);
   const int frame = si.start_frame + row;
   const GridDims grid = make_grid(H, W);
   const Cam ks = make_cam(load_k4(k4, frame));
@@ -2128,7 +2181,7 @@ __global__ void k_track_finalize(const double* __restrict__ trackacc, const doub
                                  float* __restrict__ g_ext, float* __restrict__ g_k4, int F, TL tl) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
-  const double sc = track_scale(tl.sums_of(sums, f), loss_weight, go);
+  const double sc = tl.scale(sums, f, loss_weight, go);
   const double* a = trackacc + (size_t)f * kTrackAcc;
   if (KGRAD)
     for (int k = 0; k < 4; ++k) g_k4[(size_t)f * 4 + k] = (float)(sc * a[k]);
@@ -2663,7 +2716,7 @@ template <class Lay>
 __global__ void k_focal_grad(const double* __restrict__ k4acc, const double* __restrict__ flowacc,
                              const float* __restrict__ extra_g_k4, float* __restrict__ g_focal, int H, int W,
                              Lay lay, typename Lay::Scale flow_scale) {
-  const double fs = scale_of(flow_scale);  // d total / d flow loss (the Procrustes part in k4acc carries it already)
+  const double fs = scale_of(flow_scale, blockIdx.x);  // d total / d flow loss (the Procrustes part in k4acc carries it already)
   const size_t f0 = lay.first(blockIdx.x);
   const int F = lay.frames(blockIdx.x);
   k4acc += f0 * 4;
@@ -2850,9 +2903,14 @@ template <class Lay>
 int procrustes_bwd(const float* depth, const float* k4, const float* backward_flow, const float* weights, float wsens,
                    const int64_t* indices, int num_indices, const float* g_rt, int include_flow_loss,
                    const float* flow_scale, float* g_depth, float* g_weights, float* g_k4, void* ws, int B, int T,
-                   const Lay& lay, int H, int W, cudaStream_t s, const AdamFuse* adam, bool depth_prescaled) {
+                   const Lay& lay, int H, int W, cudaStream_t s, const AdamFuse* adam, bool depth_prescaled,
+                   bool video_scales = false) {
   if (!depth || !k4 || !backward_flow || !g_depth || !ws || T < 2 * B || bad_dims(B, 2, H, W))
     return fail_msg("fm_procrustes_bwd: bad arguments");
+  using FL = std::decay_t<decltype(frames_of(lay))>;
+  constexpr bool kPacked = std::is_same<FL, Videos>::value;
+  if (video_scales && (!kPacked || !depth_prescaled))
+    return fail_msg("fm_procrustes_bwd: one flow scale per video needs packed videos and a prescaled depth gradient");
   if (!g_rt && !include_flow_loss) return fail_msg("fm_procrustes_bwd: no pose gradient given");
   const int BP = T - B;
   Workspace w = carve_rows(ws, B, T, BP);
@@ -2867,8 +2925,13 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
     k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(g_depth, flow_scale, (size_t)T * H * W);
     FM_CHECK_LAUNCH("fm_procrustes_bwd: k_scale_inplace");
   }
-  k_adjoint<<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale, w.adj, BP,
-                                          frames_of(lay));
+  // video_scales: flow_scale holds d total / d flow loss of every video (B,), else one scalar
+  if (!video_scales)
+    k_adjoint<FL, FlowScale><<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss, flow_scale,
+                                                          w.adj, BP, frames_of(lay));
+  else if constexpr (kPacked)
+    k_adjoint<Videos, VideoScales><<<(BP + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, include_flow_loss,
+                                                                VideoScales{flow_scale}, w.adj, BP, frames_of(lay));
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_adjoint");
   if (indices) {
     dim3 grid(blocks_for_points(num_indices), BP);
@@ -2888,8 +2951,12 @@ int procrustes_bwd(const float* depth, const float* k4, const float* backward_fl
   }
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_distribute");
   if (!kgrad) return 0;
-  k_k4_finalize<<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale, g_k4, T,
-                                                frames_of(lay));
+  if (!video_scales)
+    k_k4_finalize<FL, FlowScale><<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss, flow_scale,
+                                                                g_k4, T, frames_of(lay));
+  else if constexpr (kPacked)
+    k_k4_finalize<Videos, VideoScales><<<(T + 127) / 128, 128, 0, s>>>(w.k4acc, w.flowacc, include_flow_loss,
+                                                                      VideoScales{flow_scale}, g_k4, T, frames_of(lay));
   FM_CHECK_LAUNCH("fm_procrustes_bwd: k_k4_finalize");
   return 0;
 }
@@ -2968,7 +3035,7 @@ int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensit
   k_sweep_out<<<(items * 12 + 127) / 128, 128, 0, s>>>(w.flowacc, g_rt, items, 1, 12);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_out");
   // per-candidate adjoint constants, collapsed into one per batch element, then ONE distribution pass
-  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
+  k_adjoint<Uniform, FlowScale><<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_adjoint");
   k_sweep_aggregate<<<B, 32, 0, s>>>(w.adj, cand_k4, w.adj + items, B, num_candidates);
   FM_CHECK_LAUNCH("fm_softmin_sweep_bwd: k_sweep_aggregate");
@@ -3424,7 +3491,7 @@ int fm_align_rigid_bwd(const float* p, const float* q, const float* weights, con
   cudaStream_t s = (cudaStream_t)stream;
   Workspace w = carve(ws, items, 2);
   // items "pairs" of a 2-frame layout: k_adjoint indexes state / adj by pair
-  k_adjoint<<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
+  k_adjoint<Uniform, FlowScale><<<(items + 63) / 64, 64, 0, s>>>(w.flowacc, w.state, g_rt, 0, nullptr, w.adj, items, Uniform{2});
   FM_CHECK_LAUNCH("fm_align_rigid_bwd: k_adjoint");
   dim3 grid(blocks_for(n, 1), items);
   k_points_distribute<<<grid, kThreads, 0, s>>>(p, q, weights, w.adj, g_p, g_q, g_w, n);
@@ -3536,14 +3603,19 @@ static SideLane* side_lane(int which = 0) {
 extern "C++" {
 // What only one video supports: the packed step refuses it (nullptr: nothing to refuse).
 const char* step_refusal(const fm_overfit_step_args* a, const Uniform&) {
+  if (a->video_grad_scales) return "fm_overfit_step: one video takes scalar grad scales (video_grad_scales = 0)";
   return a->B > 1 ? "fm_overfit_step: one video per call (B = 0 or 1); several videos go to fm_overfit_step_videos"
                   : nullptr;
 }
 const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
-  // The split phases serve a network backbone's batch (pretraining): the caller owns the update, and the
-  // tracking kernels of packed videos take no d total / d tracking loss (TrackVideos::Scale is NoScale).
+  // The split phases serve networks' videos: a pretraining batch (one grad scale) or B networks' overfits
+  // (video_grad_scales).  The caller owns the update, and the tracking kernels of packed videos take a d total /
+  // d tracking loss only per video (TrackVideosScaled).
+  if (a->video_grad_scales && a->phase == FM_STEP_ALL)
+    return "fm_overfit_step_videos: video_grad_scales belongs to the split step (FM_STEP_FORWARD / FM_STEP_BACKWARD)";
   if (a->phase != FM_STEP_ALL) {
-    if (a->tracks) return "fm_overfit_step_videos: a split step (FM_STEP_FORWARD / FM_STEP_BACKWARD) takes no tracks";
+    if (a->tracks && !a->video_grad_scales)
+      return "fm_overfit_step_videos: a split step with one grad scale for the batch (video_grad_scales = 0) takes no tracks";
     if (a->step != 0 || a->defer_adam != 0)
       return "fm_overfit_step_videos: a split step updates no parameter (pass step = 0 and defer_adam = 0)";
     if (a->metrics_log) return "fm_overfit_step_videos: a split step writes no metrics log";
@@ -3559,19 +3631,21 @@ const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
 // videos.
 TrackOneVideo track_layout(const Uniform&) { return TrackOneVideo{}; }
 TrackVideos track_layout(const Videos& v) { return TrackVideos{v.frame_video}; }
+TrackVideosScaled track_layout_scaled(const Videos& v) { return TrackVideosScaled{{v.frame_video}}; }
 double* step_track_sums(const Uniform&, const Workspace&, void* track_ws) { return (double*)track_ws; }
 double* step_track_sums(const Videos&, const Workspace& w, void*) { return w.track_sums; }
 
 // d loss / d focal of every video (k_focal_grad), the flow part scaled by fscale (NULL = 1).  Packed videos
-// see a scale only in the backward phase of a split step: that takes the VideosScaled instance, whole steps
-// keep the NoScale one.
+// see a scale only in the backward phase of a split step: that takes the VideosScaled instance (one scale), or
+// with `each` the VideosEachScaled one (fscale holds B scales); whole steps keep the NoScale one.
 void launch_focal_grad(const Workspace& w, const float* track_g_k4, float* g_focal, int B, int H, int W,
-                       const Uniform& u, const float* fscale, cudaStream_t s) {
+                       const Uniform& u, const float* fscale, bool, cudaStream_t s) {
   k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, u, fscale);
 }
 void launch_focal_grad(const Workspace& w, const float* track_g_k4, float* g_focal, int B, int H, int W,
-                       const Videos& v, const float* fscale, cudaStream_t s) {
-  if (fscale) k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, VideosScaled{v}, fscale);
+                       const Videos& v, const float* fscale, bool each, cudaStream_t s) {
+  if (each) k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, VideosEachScaled{v}, fscale);
+  else if (fscale) k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, VideosScaled{v}, fscale);
   else k_focal_grad<<<B, 256, 0, s>>>(w.k4acc, w.flowacc, track_g_k4, g_focal, H, W, v, NoScale(nullptr));
 }
 
@@ -3696,9 +3770,17 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   // d total / d (flow loss) and d total / d (tracking loss) of a split step (device scalars, NULL = 1)
   const float* fscale = a->phase == FM_STEP_BACKWARD ? a->flow_grad_scale : nullptr;
   const float* tscale = a->phase == FM_STEP_BACKWARD ? a->track_grad_scale : nullptr;
+  // video_grad_scales (packed videos only, step_refusal): both scales hold one value per video
+  const bool each = a->phase == FM_STEP_BACKWARD && a->video_grad_scales != 0;
+  constexpr bool kPacked = std::is_same<Lay, Videos>::value;
   if (fscale) {  // the direct flow-loss gradient in g_depth was computed for scale 1; scale it before
     // the tracking loss adds its own (differently scaled) part
-    k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, TF * N);
+    if (!each) {
+      k_scale_inplace<<<sm_count_cached() * 4, kThreads, 0, s>>>(a->g_depth, fscale, TF * N);
+    } else if constexpr (kPacked) {
+      const unsigned nx = (unsigned)((N + kThreads * 4 - 1) / (kThreads * 4));
+      k_scale_videos<<<dim3(nx, T < 65535 ? T : 65535), kThreads, 0, s>>>(a->g_depth, fscale, lay.frame_video, N, T);
+    }
     FM_CHECK_LAUNCH("fm_overfit_step: k_scale_inplace");
   }
   const float* g_rt = a->phase == FM_STEP_BACKWARD ? a->g_rt : nullptr;           // the caller's
@@ -3714,11 +3796,19 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       if ((e = cudaStreamWaitEvent(lane->stream, lane->fork, 0)) != cudaSuccess) return fail("fm_overfit_step: fork", e);
       apply_stream = lane->stream;
     }
-    if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
-                             t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
-                             a->track_ws, T, H, W, 0, 0, T, s, apply_stream, step_track_sums(lay, w, a->track_ws),
-                             track_layout(lay))))
-      return rc;
+    if (!each) {
+      if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
+                               t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
+                               a->track_ws, T, H, W, 0, 0, T, s, apply_stream, step_track_sums(lay, w, a->track_ws),
+                               track_layout(lay))))
+        return rc;
+    } else if constexpr (kPacked) {
+      if ((rc = track_bwd_impl(k4, a->extrinsics, t->segments, t->num_segments, t->max_rows, t->max_points, t->xy,
+                               t->total_samples, a->track_weight, tscale, a->g_depth, a->g_extrinsics, a->track_g_k4,
+                               a->track_ws, T, H, W, 0, 0, T, s, apply_stream, step_track_sums(lay, w, a->track_ws),
+                               track_layout_scaled(lay))))
+        return rc;
+    }
     if (lane && (e = cudaEventRecord(lane->join, lane->stream)) != cudaSuccess) return fail("fm_overfit_step: join", e);
     if ((rc = pose_chain_bwd(a->rt, a->extrinsics, a->g_extrinsics, a->g_rt, B, lay, stream))) return rc;
     g_rt = a->g_rt;
@@ -3748,7 +3838,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   // g_depth was scaled by fscale above
   if ((rc = procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
                            a->num_indices, g_rt, 1, fscale, a->g_depth, a->g_weights, a->g_k4, a->ws, B, T, pairs,
-                           H, W, s, fuse_w ? &af : nullptr, /*depth_prescaled=*/true)))
+                           H, W, s, fuse_w ? &af : nullptr, /*depth_prescaled=*/true, each)))
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   // Adam (model_wrapper_overfit.py:104-105)
@@ -3763,7 +3853,7 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       return rc;
   }
   if (a->focal) {  // d loss / d focal, then (update steps) its Adam
-    launch_focal_grad(w, track_g_k4, a->g_focal, B, H, W, lay, fscale, s);
+    launch_focal_grad(w, track_g_k4, a->g_focal, B, H, W, lay, fscale, each, s);
     FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
     if (a->step > 0 && !defer) {
       const int fstep = a->focal_step > 0 ? a->focal_step : a->step;

@@ -69,7 +69,8 @@ class _StepRoot(torch.autograd.Function):
 
 
 class _LossNode(torch.autograd.Function):
-    """One loss of the step: value computed by the forward half, gradient deferred to the root."""
+    """One loss of the step (a scalar, or B networks' (B,) losses): value computed by the forward half, gradient
+    deferred to the root."""
 
     @staticmethod
     def forward(ctx, token, step, which, value):
@@ -78,7 +79,8 @@ class _LossNode(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        ctx.step.scales[ctx.which] = g.reshape(()).to(torch.float32).contiguous()
+        # one scalar, or (network_videos_step) one grad_output per video
+        ctx.step.scales[ctx.which] = g.to(torch.float32).contiguous()
         return g, None, None, None
 
 
@@ -234,3 +236,70 @@ def fused_output(model, batch: Batch, flows: Flows, global_step: int,
     _bind(out, model, batch, flows, global_step, backbone_out)
     out.__dict__.update(intrinsics=batch.intrinsics, k_mode="const")
     return out
+
+
+class _VideosStep:
+    """One step of B networks' overfits on the packed split halves (network_videos_step): the state that
+    _StepRoot and the two _LossNodes share.  Its scales are (B,) grad_outputs, one per video."""
+
+    def __init__(self, engine, params, focal_params):
+        self.engine, self._params, self._focal_params = engine, params, focal_params
+        self.scales = {}
+        self.track_done = False
+
+    def run_backward(self):
+        eng = self.engine
+        dev = eng.rt.device
+        zeros = torch.zeros(eng.B, dtype=torch.float32, device=dev)
+        # a loss that did not reach the objective has no grad_output: its gradient is 0, not 1
+        flow = self.scales.get("flow", zeros)
+        track = self.scales.get("tracking") if self.track_done else None
+        eng.backward_phase(flow, track, with_tracking=track is not None)
+        # the packed (T, H, W) / (T - B, H, W) buffers, as the step's inputs
+        out = [eng._g_depth.detach().view(self._params[0].shape)]
+        if len(self._params) > 1:
+            out.append(eng._g_w.detach().view(self._params[1].shape))
+        # each model's own d loss / d focal (copies: the buffer is rewritten by the next step)
+        out += [eng._g_focal[b].detach().clone().view(p.shape) for b, p in enumerate(self._focal_params)]
+        return tuple(out)
+
+
+def network_videos_step(engine, depths: Tensor, weights: Optional[Tensor], global_step: int,
+                        training: bool = True, intrinsics=None):
+    """One fused step of B networks' overfits, each network on its own video (a FusedOverfitter bound to a list of
+    B network Models).  `depths` (T, H, W) and, with correspondence weights, `weights` (T - B, H, W) are the step's
+    network outputs, packed along the frame axis (the caller concatenates its networks' outputs under autograd).
+    Returns the (B,) weighted flow losses and tracking losses (zeros while the tracking loss is off), outputs of
+    one root node: autograd calls its backward once, with one grad_output per video and loss, and it runs the
+    backward half and hands d loss / d depths, d loss / d weights and each model's d loss / d focal length to
+    autograd.  Video b gets what a one-video network-bound fused step on it gets, its gradients scaled by its own
+    grad_output.
+
+    Ground-truth intrinsics: the engine reads its videos' `batch.intrinsics` when it is built.  `intrinsics` (the
+    list of B (1, F_b, 3, 3) tensors, or a (B, F, 3, 3) tensor for a tensor batch) is this step's K, copied into the
+    step before its forward half without a host synchronisation, as the one-video surface reads `batch.intrinsics`
+    on every step (a loader's new K, or the same tensors rewritten in place); None keeps the K the step last read."""
+    eng = engine
+    if not getattr(eng, "_net_videos", False):
+        raise ValueError("flowmap_b200: network_videos_step needs a FusedOverfitter bound to a list of network Models")
+    cfg = eng.cfg
+    inputs = [depths.to(torch.float32).contiguous()]
+    if cfg.use_correspondence_weights:
+        if weights is None:
+            raise ValueError("flowmap_b200: a step with correspondence weights needs `weights`")
+        inputs.append(weights.to(torch.float32).contiguous())
+    if intrinsics is not None:
+        if not eng._gt:
+            raise ValueError("flowmap_b200: `intrinsics` serves ground-truth K (cfg.intrinsics = 'ground_truth')")
+        eng._write_k4(intrinsics)
+    # the focal gradients handed to autograd are copies (_VideosStep.run_backward): no .grad aliases the buffer
+    focal_params = [p for m in eng.models for p in m._fused_params(global_step, [])]
+    tracking = cfg.use_tracking and global_step >= cfg.tracking_enable_after
+    step = _VideosStep(eng, inputs, focal_params)
+    flow = eng.forward_phase(global_step, training=training, depth=inputs[0].detach(),
+                             weights=inputs[1].detach() if len(inputs) > 1 else None, tracking=tracking)
+    track = eng.track_losses() if tracking else torch.zeros_like(flow)
+    step.track_done = tracking
+    token = _StepRoot.apply(step, *inputs, *focal_params)
+    return (_LossNode.apply(token, step, "flow", flow),
+            _LossNode.apply(token, step, "tracking", track))

@@ -317,6 +317,26 @@ class Model(nn.Module):
             params.append(intr.intrinsics_regressed.focal_length)
         return params
 
+    def _overfit_fields(self) -> dict:
+        """The fields of an OverfitCfg that this model's configuration sets (a network backbone's BackboneOutput
+        holds the weights themselves: sensitivity 0 to the kernels)."""
+        mc, bc, ic, ec = self.cfg, self.cfg.backbone, self.cfg.intrinsics, self.cfg.extrinsics
+        explicit = isinstance(self.backbone, BackboneExplicitDepth)
+        soft = isinstance(self.intrinsics, IntrinsicsSoftmin)
+        reg = ic.regression if soft else None
+        intrinsics = ("ground_truth" if isinstance(self.intrinsics, IntrinsicsGroundTruth) else
+                      "softmin" if soft else "regressed")
+        return dict(
+            initial_depth=bc.initial_depth if explicit else 0.0,
+            weight_sensitivity=bc.weight_sensitivity if explicit else 0.0,
+            use_correspondence_weights=mc.use_correspondence_weights, procrustes_points=ec.num_points,
+            procrustes_randomize=ec.randomize_points, intrinsics=intrinsics,
+            softmin_points=ic.num_procrustes_points if soft else 8192,
+            softmin_min=ic.min_focal_length if soft else 0.5, softmin_max=ic.max_focal_length if soft else 2.0,
+            softmin_candidates=ic.num_candidates if soft else 60,
+            regression_after=reg.after_step if reg is not None else None,
+            regression_window=reg.window if reg is not None else 100)
+
     def _fused_engine(self, batch: Batch, flows: Flows, tracks, flow_loss):
         """The FusedOverfitter bound to this model's parameters for (flows, tracks); built on first
         use, re-pointed when the Flows tensors change, None if the configuration is not covered.  A batch of
@@ -325,28 +345,14 @@ class Model(nn.Module):
         if batch.videos.shape[0] > 1 and tracks is not None:
             return None
         from .overfit import FusedOverfitter, OverfitCfg
-        mc, bc, ic, ec = self.cfg, self.cfg.backbone, self.cfg.intrinsics, self.cfg.extrinsics
         lm = flow_loss.cfg.mapping
         key = (tuple(batch.videos.shape), None if tracks is None else tuple(id(t) for t in tracks),
                lm.name, getattr(lm, "delta", 0.01))
         eng = getattr(self, "_engine", None)
         if eng is None or self._engine_key != key:
             explicit = isinstance(self.backbone, BackboneExplicitDepth)
-            soft = isinstance(self.intrinsics, IntrinsicsSoftmin)
-            reg = ic.regression if soft else None
-            intrinsics = ("ground_truth" if isinstance(self.intrinsics, IntrinsicsGroundTruth) else
-                          "softmin" if soft else "regressed")
-            # a network backbone's BackboneOutput holds the weights themselves: sensitivity 0 to the kernels
             cfg = OverfitCfg(
-                initial_depth=bc.initial_depth if explicit else 0.0,
-                weight_sensitivity=bc.weight_sensitivity if explicit else 0.0,
-                use_correspondence_weights=mc.use_correspondence_weights, procrustes_points=ec.num_points,
-                procrustes_randomize=ec.randomize_points, intrinsics=intrinsics,
-                softmin_points=ic.num_procrustes_points if soft else 8192,
-                softmin_min=ic.min_focal_length if soft else 0.5, softmin_max=ic.max_focal_length if soft else 2.0,
-                softmin_candidates=ic.num_candidates if soft else 60,
-                regression_after=reg.after_step if reg is not None else None,
-                regression_window=reg.window if reg is not None else 100,
+                **self._overfit_fields(),
                 flow_weight=flow_loss.cfg.weight, flow_enable_after=flow_loss.cfg.enable_after,
                 use_tracking=tracks is not None, tracking_enable_after=0, mapping=lm.name,
                 delta=getattr(lm, "delta", 0.01))

@@ -207,16 +207,27 @@ class FusedOverfitter:
         import ctypes
         listed = isinstance(batch, (list, tuple))
         B = len(batch) if listed else batch.videos.shape[0]
-        one, tensor_batch = not listed and B == 1, not listed and B > 1
+        # a list of B network Models: B overfits in one packed split step (flowmap_b200.fused.network_videos_step)
+        self._net_videos = isinstance(model, (list, tuple))
+        one = not listed and B == 1 and not self._net_videos
+        tensor_batch = not listed and not one
         self.cfg, self._gt, self._tensor_batch = cfg, cfg.intrinsics == "ground_truth", tensor_batch
         # bound to a caller's Model (the autograd drop-in surface, flowmap_b200.fused)
         self._bound = model is not None
-        self._network = isinstance(model, Model) and not isinstance(model.backbone, BackboneExplicitDepth)
+        if self._net_videos:
+            self._check_network_models(cfg, list(model), B)
+            self._network = True
+        else:
+            self._network = isinstance(model, Model) and not isinstance(model.backbone, BackboneExplicitDepth)
+        # a network Model's tensor batch: the pretraining step, one pooled flow-loss normaliser
+        self._pooled = self._network and not self._net_videos and tensor_batch
 
         # ---- the videos: one (Batch, Flows) each, validated before anything reaches the device
-        if model is not None and (listed or tensor_batch and not self._network):
+        if self._net_videos:
+            pass
+        elif model is not None and (listed or tensor_batch and not self._network):
             raise ValueError("flowmap_b200: a bound Model holds one video (batch size 1)")
-        if self._network and tensor_batch:
+        if self._pooled:
             if tracks is not None or cfg.use_tracking:
                 raise ValueError("flowmap_b200: a network backbone's batch of several videos takes no tracks")
             if (self._gt != isinstance(model.intrinsics, IntrinsicsGroundTruth) or
@@ -225,7 +236,7 @@ class FusedOverfitter:
                                  "without a regression stage (one focal length per video), or ground-truth intrinsics, "
                                  f"in both cfg.intrinsics ({cfg.intrinsics!r}) and the bound model "
                                  f"({type(model.intrinsics).__name__})")
-        elif model is not None and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
+        elif model is not None and not self._net_videos and isinstance(model.intrinsics, IntrinsicsGroundTruth) != self._gt:
             raise ValueError(f"flowmap_b200: the bound model's intrinsics ({type(model.intrinsics).__name__}) do not "
                              f"match cfg.intrinsics = {cfg.intrinsics!r}")
         if listed and (not batch or not isinstance(flows, (list, tuple)) or len(flows) != B):
@@ -266,7 +277,7 @@ class FusedOverfitter:
         T = self.T
         # the kernels read raw pointers: canonical (contiguous float32) tensors, kept alive here
         # (FlowPredictor.rescale_flow returns a permuted view, flow_predictor.py:40-49)
-        if one or self._network:  # the tensors given, or copies of those that are not contiguous
+        if one or self._pooled:  # the tensors given, or copies of those that are not contiguous
             self.flows = self._canonical_flows(flows.to(device))
         else:  # copies packed along the pair axis: the pairs of video b follow those of video b - 1
             self.flows = Flows(*(torch.cat([ops._canon(getattr(fl, n).to(device), n)[0] for _, fl in videos])
@@ -288,6 +299,8 @@ class FusedOverfitter:
         if model is None:
             built = [build_model_and_losses(cfg, f, (h, w)) for f in frames]
             self.models, self.losses = [m.to(device) for m, _ in built], built[0][1]
+        elif self._net_videos:
+            self.models, self.losses = list(model), None
         else:
             self.models, self.losses = [model], None
         self.model = self.models[0]
@@ -314,7 +327,7 @@ class FusedOverfitter:
             self._focal = gather([m.intrinsics.intrinsics_regressed.focal_length for m in self.models], True)
         else:
             self._focal = torch.zeros(self._lead[2], device=dev)
-        if self._network:  # LossFlow's pooled normaliser at b > 1, in every video's slot
+        if self._pooled:  # LossFlow's pooled normaliser at b > 1, in every video's slot
             pooled = ops.mask_sum(self.flows.forward_mask, self.flows.backward_mask)
             self._msum = pooled.expand(self._lead[2]).contiguous()
         else:
@@ -333,6 +346,24 @@ class FusedOverfitter:
                 self._write_k4(k)
             else:
                 self.set_intrinsics(k)
+
+    @staticmethod
+    def _check_network_models(cfg: "OverfitCfg", models, B: int):
+        """The Models of B networks' overfits: one per video, each with a network backbone, all of one
+        configuration that `cfg` describes (the step runs one OverfitCfg and one step clock for all of them)."""
+        if len(models) != B:
+            raise ValueError(f"flowmap_b200: {len(models)} Models for {B} videos: one network Model per video")
+        for i, m in enumerate(models):
+            if not isinstance(m, Model) or isinstance(m.backbone, BackboneExplicitDepth):
+                raise ValueError(f"flowmap_b200: model {i} is not a Model with a network backbone (an explicit-depth "
+                                 "Model optimises its own depth: several of them go to a FusedOverfitter of their own)")
+            if m.cfg != models[0].cfg:
+                raise ValueError(f"flowmap_b200: model {i}'s cfg differs from model 0's: the videos of one step share "
+                                 "one configuration")
+        want = models[0]._overfit_fields()
+        diff = {k: (getattr(cfg, k), v) for k, v in want.items() if getattr(cfg, k) != v}
+        if diff:
+            raise ValueError(f"flowmap_b200: cfg does not describe the Models (cfg value, model value): {diff}")
 
     def _canonical_flows(self, flows: Flows, device=None) -> Flows:
         """Flows of this optimiser's (B, F-1, H, W, ...) shape on `device` (default: that of flows.forward), as
@@ -401,6 +432,7 @@ class FusedOverfitter:
         self._clock = ops.StepClock(dev, cfg.lr)
         self._side_stream = torch.cuda.Stream(device=dev)  # parallel branch of the step (see _step_softmin)
         a.clock = self._clock.ptr
+        a.video_grad_scales = int(self._net_videos)  # backward_phase's scales: one per video
         self._total = torch.zeros_like(self._loss)
         self._idx_buf = torch.empty(min(cfg.softmin_points, h * w), dtype=torch.int64, device=dev) \
             if self._softmin else None
@@ -451,7 +483,7 @@ class FusedOverfitter:
         from a list of one Flows per video.  One video, or a network backbone's batch of several: the step
         reads the new Flows themselves, and `mask_sum` (default: the pooled sum of all their masks) goes to
         every video."""
-        if self._layout is not None and not self._network:
+        if self._layout is not None and not self._pooled:
             if self._tensor_batch and isinstance(flows, Flows):
                 flows = [_video(flows, i) for i in range(flows.forward.shape[0])]
             if not isinstance(flows, (list, tuple)) or len(flows) != self.B:
@@ -590,14 +622,21 @@ class FusedOverfitter:
                 self.global_step >= c.regression_after - c.regression_window)
 
     def _append_window(self, split: bool = False):
-        """Append the sweep's focal estimate to the open window: a scalar, or (B,) for several videos."""
-        if self._window_open():
+        """Append the sweep's focal estimate to the open window: a scalar, or (B,) for several videos; B
+        networks' Models each keep their own video's scalars."""
+        if self._window_open() and self._net_videos:
+            for m, f in zip(self.models, self._sw_focal.clone().unbind()):
+                m.intrinsics.window.append(f)
+        elif self._window_open():
             self._window(split).append(self._sw_focal[0].clone() if self._layout is None else self._sw_focal.clone())
 
     def _hand_over(self, split: bool = False):
         """At global_step == regression_after, seed the regressed focal length (each video's) with the
         window's mean; the stacked window is (n,) for one video, (n, B) for several."""
-        if self._softmin and self.global_step == self.cfg.regression_after:
+        if self._softmin and self.global_step == self.cfg.regression_after and self._net_videos:
+            for b, m in enumerate(self.models):
+                self._focal[b].copy_(torch.stack(m.intrinsics.window).mean())
+        elif self._softmin and self.global_step == self.cfg.regression_after:
             self._focal.copy_(torch.stack(self._window(split)).mean(0))
 
     def _step_softmin(self, update: bool):
@@ -654,13 +693,15 @@ class FusedOverfitter:
     # ---- split step: the two halves of one iteration WITHOUT the parameter update, for callers that
     # need the loss values before they decide on the backward (torch.autograd: flowmap_b200.fused)
     def forward_phase(self, global_step: int, training: bool = True, depth: Optional[Tensor] = None,
-                      weights: Optional[Tensor] = None):
+                      weights: Optional[Tensor] = None, tracking: bool = False):
         """Poses + flow loss with its direct gradients (fm_overfit_step, FM_STEP_FORWARD; the
         candidate sweep first in the softmin stage).  Returns the weighted flow loss (device scalar,
         a buffer that the next call overwrites; (B,) per-video losses for a network's batch of B videos).
         Bound to a network backbone, `depth` (B, F, H, W) and, with correspondence weights, `weights`
         (B, F-1, H, W) are the step's contiguous float32 inputs (B = 1 but for a network's batch); they stay
-        referenced until the next call (backward_phase reads them)."""
+        referenced until the next call (backward_phase reads them).  B networks' videos (a list of Models):
+        `depth` (T, H, W) and `weights` (T - B, H, W) packed along the frame axis, and `tracking` adds the chained
+        poses and every video's tracking loss (track_losses()) to this half."""
         if not self._network:
             self._refuse_videos("the split-step surface")
         a = self._args
@@ -673,6 +714,10 @@ class FusedOverfitter:
         self.global_step = global_step
         self._begin_step()
         a.tracks, a.step, a.defer_adam = None, 0, 0
+        if tracking:
+            if not self._net_videos or self._packed is None:
+                raise ValueError("flowmap_b200: forward_phase(tracking=True) serves B networks' videos with tracks")
+            a.tracks = self._ctypes.pointer(self._pk_c)
         self._sweep_idx = None
         with torch.cuda.device(self.rt.device):
             if self._softmin_stage():
@@ -689,13 +734,19 @@ class FusedOverfitter:
             try:
                 self._call_step("fm_overfit_step (forward)")
             finally:
-                a.phase = 0
+                a.phase, a.tracks = 0, None
         return self._loss
+
+    def track_losses(self) -> Tensor:
+        """The (B,) weighted tracking losses of the last forward_phase(tracking=True) (a buffer that the next
+        call overwrites)."""
+        return self._track_loss
 
     def _bind_inputs(self, depth, weights, f, h, w):
         """Point the step at a network backbone's depths / weights of this step."""
         use_w, b = self.cfg.use_correspondence_weights, self.B
-        for name, t, shape in (("depth", depth, (b, f, h, w)), ("weights", weights if use_w else None, (b, f - 1, h, w))):
+        shapes = ((self.T, h, w), (self.T - b, h, w)) if self._net_videos else ((b, f, h, w), (b, f - 1, h, w))
+        for name, t, shape in (("depth", depth, shapes[0]), ("weights", weights if use_w else None, shapes[1])):
             if t is None and (name == "depth" or use_w):
                 raise ValueError(f"flowmap_b200: a network backbone's step needs its `{name}`")
             if t is not None and (tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()
@@ -727,7 +778,8 @@ class FusedOverfitter:
     def backward_phase(self, flow_scale=None, track_scale=None, with_tracking: bool = False):
         """Second half: [tracking backward,] Procrustes backward, focal gradient[, the sweep's
         backward].  flow_scale / track_scale: device float scalars d total / d loss (None = 1); a network's
-        batch of videos takes one flow_scale for all of them.  Leaves the gradients in gradients()."""
+        batch of videos takes one flow_scale for all of them, B networks' videos (B,) float32 tensors, one
+        d total / d loss_b per video.  Leaves the gradients in gradients()."""
         if not self._network:
             self._refuse_videos("the split-step surface")
         a = self._args
@@ -906,6 +958,8 @@ class FusedOverfitter:
         update evaluated, before its Adam step -- the values the reference's training_step logs at
         global_step k.  The reference's validation after update k (experiment/dump_ate.yaml's
         val_check_interval: 1) evaluates the updated parameters: that is row k + 1."""
+        if self._net_videos:
+            raise ValueError("flowmap_b200: B networks' overfits run the split step, which writes no metrics log")
         if capacity < 1:
             raise ValueError("flowmap_b200: the metrics log needs a capacity >= 1")
         dev, nan = self.rt.device, float("nan")

@@ -339,6 +339,11 @@ typedef struct {
   float gt_fx, gt_fy;            /* frame means of the normalised GT intrinsics, NaN: columns NaN */
   float* metrics_log;            /* (metrics_capacity, 5) ring, or NULL = off */
   int metrics_capacity;
+  /* fm_overfit_step_videos, split step only (FM_STEP_FORWARD / FM_STEP_BACKWARD; fm_overfit_step refuses it):
+     0 = flow_grad_scale is ONE device scalar for the whole batch (pretraining) and the step takes no tracks;
+     1 = B networks' overfits: flow_grad_scale and track_grad_scale are device (B,) arrays (NULL = all 1),
+     d total / d loss_b and d total / d track_loss_b of every video b, and the step may take tracks. */
+  int video_grad_scales;
   /* 0 or 1; fm_overfit_step_videos ignores it.  fm_overfit_step optimises one video and refuses B > 1:
      several videos go to fm_overfit_step_videos. */
   int B;
@@ -381,9 +386,13 @@ typedef struct {
  * the sweep's backward).
  * Phases: FM_STEP_ALL, or the two halves of a split step, FM_STEP_FORWARD then FM_STEP_BACKWARD (a network
  * backbone's batch, whose depths / weights come from the network and whose update the caller owns).  A
- * split step needs step = 0, defer_adam = 0, tracks == NULL and metrics_log == NULL.  Its flow_grad_scale is
- * ONE device scalar for the whole batch, d total / d loss_b for every video b: the sum of the B losses is the
- * objective.  The reference's LossFlow at b > 1 (pretraining) is such a sum when every mask_sum[b] holds the
+ * split step needs step = 0, defer_adam = 0 and metrics_log == NULL.  With video_grad_scales = 0 it takes no
+ * tracks and its flow_grad_scale is ONE device scalar for the whole batch, d total / d loss_b for every video b:
+ * the sum of the B losses is the objective.  With video_grad_scales = 1 (B networks, each overfitting its own
+ * video) it is B independent split steps: the forward computes each video's flow loss (by its own mask_sum[b])
+ * and, with tracks, the chained poses and each video's tracking loss into track_loss[b]; the backward scales
+ * video b's flow and tracking gradients, its focal gradient included, by flow_grad_scale[b] and
+ * track_grad_scale[b].  The reference's LossFlow at b > 1 (pretraining) is such a sum when every mask_sum[b] holds the
  * pooled normaliser M = sum over all videos of their forward + backward mask sums ("or 1"): loss[b] is then
  * weight * S_b / M and sum_b loss[b] the pooled loss. */
 int fm_overfit_step_videos(const fm_overfit_step_args* args, const fm_video_layout* layout, void* stream);
