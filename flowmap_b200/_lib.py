@@ -93,13 +93,13 @@ class OverfitStepArgs(ctypes.Structure):
                 ("tracks", ctypes.POINTER(PackedTracksC)), ("track_weight", c_float),
                 ("m_depth", _P), ("v_depth", _P), ("m_weights", _P), ("v_weights", _P),
                 ("m_focal", _P), ("v_focal", _P),
-                ("lr", c_double), ("beta1", c_double), ("beta2", c_double), ("eps", c_double),
+                ("beta1", c_double), ("beta2", c_double), ("eps", c_double),
                 ("step", c_int),
                 ("g_depth", _P), ("g_weights", _P), ("g_focal", _P), ("g_k4", _P),
                 ("rt", _P), ("loss", _P),
                 ("extrinsics", _P), ("g_extrinsics", _P), ("g_rt", _P), ("track_g_k4", _P),
                 ("track_loss", _P),
-                ("ws", _P), ("track_ws", _P), ("focal_step", c_int), ("defer_adam", c_int),
+                ("ws", _P), ("track_ws", _P), ("defer_adam", c_int),
                 ("phase", c_int),
                 ("flow_grad_scale", _P), ("track_grad_scale", _P), ("clock", _P), ("moments_k4", _P),
                 ("gt_positions", _P), ("gt_fx", c_float), ("gt_fy", c_float), ("metrics_log", _P),

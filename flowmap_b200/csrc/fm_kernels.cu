@@ -974,10 +974,10 @@ __global__ void k_adjoint(const double* __restrict__ flowacc, const PairState* _
 // Adam pass over the weights disappear into it.
 struct AdamFuse {
   float* m; float* v;
-  float beta1, beta2, omb1, omb2, eps, step_size, bc2_sqrt;
+  float beta1, beta2, omb1, omb2, eps;
   int on;
   int first_pair;  // pairs below this index are left to a later, separate Adam call
-  const float* consts;  // device {step_size, bc2_sqrt} of a step clock (CUDA-graph replays), or NULL
+  const float* consts;  // device {step_size, bc2_sqrt} of the step clock's current tick
 };
 
 // KGRAD (this kernel and the two dense ones): accumulate the intrinsics gradient into k4acc.  Without it
@@ -1000,7 +1000,6 @@ k_distribute(const float* __restrict__ depth, const float* __restrict__ k4, cons
   const PairAddr pa = pair_addr(lay, pair, N);
   const PairGeom g = pair_geom(k4, pa, H, W, ad.shift[2]);
   const int a = pa.k4_frame_a;
-  if (adam.on && adam.consts) { adam.step_size = __ldg(adam.consts); adam.bc2_sqrt = __ldg(adam.consts + 1); }
   const float* da = opaque_ptr(depth + pa.depth_a);
   const float* db = da + N;
   const float* fl = bflow + pa.flow;
@@ -1079,8 +1078,7 @@ __device__ __forceinline__ void distribute_pixels(const PairGeom& g, const PairA
     }
     if (VEC == 4 && fuse_adam) {  // torch.optim.Adam on the logits (k_adam's order)
       // the step clock's constants are re-read here (L1 hits) rather than held across the pixel loop
-      const float step_size = adam.consts ? __ldg(adam.consts) : adam.step_size;
-      const float bc2_sqrt = adam.consts ? __ldg(adam.consts + 1) : adam.bc2_sqrt;
+      const float step_size = __ldg(adam.consts), bc2_sqrt = __ldg(adam.consts + 1);
       float4 mm = *reinterpret_cast<float4*>(adam.m + wi);
       float4 vv = *reinterpret_cast<float4*>(adam.v + wi);
       float* mp = &mm.x; float* vp = &vv.x;
@@ -3053,7 +3051,7 @@ int sweep_bwd_impl(const float* depth, const float* weights, float weight_sensit
 // =================================================================== C ABI
 extern "C" {
 
-int fm_version(void) { return 106; }
+int fm_version(void) { return 107; }
 unsigned long long fm_launch_count(void) { return fm_host::launches(); }
 const char* fm_last_error(void) { return fm_host::last_error(); }
 
@@ -3620,7 +3618,7 @@ const char* step_refusal(const fm_overfit_step_args* a, const Videos&) {
       return "fm_overfit_step_videos: a split step updates no parameter (pass step = 0 and defer_adam = 0)";
     if (a->metrics_log) return "fm_overfit_step_videos: a split step writes no metrics log";
   }
-  if (a->defer_adam == 1 && a->step > 0 && a->weight_logits)
+  if (a->defer_adam == 1 && a->step && a->weight_logits)
     return "fm_overfit_step_videos: does not fuse the logit update of a deferred step (pass step = 0)";
   if (a->metrics_log && !a->gt_fxfy) return "fm_overfit_step_videos: metrics need gt_fxfy";
   return nullptr;
@@ -3674,6 +3672,8 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
       !a->g_depth || !a->rt || !a->loss || !a->ws || !a->k4 || T < 2 * B || bad_dims(B, 2, a->H, a->W))
     return fail_msg("fm_overfit_step: bad arguments");
   if (const char* why = step_refusal(a, lay)) return fail_msg(why);
+  if (a->step != 0 && a->step != 1) return fail_msg("fm_overfit_step: step switches the update off (0) or on (1)");
+  if (a->step && !a->clock) return fail_msg("fm_overfit_step: an update step (step = 1) needs the step clock");
   if (a->weight_logits && !a->g_weights) return fail_msg("fm_overfit_step: g_weights missing");
   if (a->tracks && (!a->extrinsics || !a->g_extrinsics || !a->track_ws || !a->track_loss))
     return fail_msg("fm_overfit_step: tracking needs extrinsics / g_extrinsics / track_ws / track_loss");
@@ -3824,16 +3824,14 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
   const bool defer = a->defer_adam != 0;  // softmin stage: the sweep's backward still adds gradients
   // (several videos with defer_adam = 1 would have to defer pair 0 of EVERY video, as first_pair counts pairs
   // of the whole batch: step_refusal leaves the logits of that step to the caller)
-  const bool fuse_w = a->step > 0 && a->weight_logits && !a->indices && W % 4 == 0;
+  const bool fuse_w = a->step && a->weight_logits && !a->indices && W % 4 == 0;
   const StepClock* clock = (const StepClock*)a->clock;
   if (fuse_w) {  // the weight gradient is final inside k_distribute: update the logits there
-    af.consts = clock ? &clock->step_size : nullptr;
+    af.consts = &clock->step_size;
     af.on = 1; af.m = a->m_weights; af.v = a->v_weights;
     af.first_pair = a->defer_adam == 1 ? 1 : 0;  // 1: the sweep still touches pair 0; 2: every pair is final
     af.beta1 = (float)a->beta1; af.beta2 = (float)a->beta2;
     af.omb1 = (float)(1.0 - a->beta1); af.omb2 = (float)(1.0 - a->beta2); af.eps = (float)a->eps;
-    af.step_size = (float)(a->lr / (1.0 - pow(a->beta1, (double)a->step)));
-    af.bc2_sqrt = (float)sqrt(1.0 - pow(a->beta2, (double)a->step));
   }
   // g_depth was scaled by fscale above
   if ((rc = procrustes_bwd(a->depth, k4, a->bflow, a->weight_logits, a->weight_sensitivity, a->indices,
@@ -3842,29 +3840,21 @@ static int overfit_step_impl(const fm_overfit_step_args* a, int B, int T, const 
     return rc;
   if (lane && (e = cudaStreamWaitEvent(s, lane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   // Adam (model_wrapper_overfit.py:104-105)
-  if (a->step > 0 && !defer) {
-    auto adam = [&](float* p, const float* g, float* m, float* v, size_t n, int step, int focal_clock) -> int {
-      return clock ? fm_adam_step_clock(p, g, m, v, n, clock, focal_clock, a->beta1, a->beta2, a->eps, stream)
-                   : fm_adam_step(p, g, m, v, n, a->lr, a->beta1, a->beta2, a->eps, step, stream);
-    };
-    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, TF * N, a->step, 0))) return rc;
+  auto adam = [&](float* p, const float* g, float* m, float* v, size_t n, int focal_clock) -> int {
+    return fm_adam_step_clock(p, g, m, v, n, clock, focal_clock, a->beta1, a->beta2, a->eps, stream);
+  };
+  if (a->step && !defer) {
+    if ((rc = adam(a->depth, a->g_depth, a->m_depth, a->v_depth, TF * N, 0))) return rc;
     if (a->weight_logits && !fuse_w &&
-        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, TP * N, a->step, 0)))
+        (rc = adam(a->weight_logits, a->g_weights, a->m_weights, a->v_weights, TP * N, 0)))
       return rc;
   }
   if (a->focal) {  // d loss / d focal, then (update steps) its Adam
     launch_focal_grad(w, track_g_k4, a->g_focal, B, H, W, lay, fscale, each, s);
     FM_CHECK_LAUNCH("fm_overfit_step: k_focal_grad");
-    if (a->step > 0 && !defer) {
-      const int fstep = a->focal_step > 0 ? a->focal_step : a->step;
-      if ((rc = clock ? fm_adam_step_clock(a->focal, a->g_focal, a->m_focal, a->v_focal, B, clock, 1, a->beta1,
-                                           a->beta2, a->eps, stream)
-                      : fm_adam_step(a->focal, a->g_focal, a->m_focal, a->v_focal, B, a->lr, a->beta1, a->beta2,
-                                     a->eps, fstep, stream)))
-        return rc;
-    }
+    if (a->step && !defer && (rc = adam(a->focal, a->g_focal, a->m_focal, a->v_focal, B, 1))) return rc;
   }
-  if (defer && a->step > 0 && a->weight_logits && !fuse_w) return fail_msg("fm_overfit_step: defer_adam needs the fused weight update");
+  if (defer && a->step && a->weight_logits && !fuse_w) return fail_msg("fm_overfit_step: defer_adam needs the fused weight update");
   if (mlane && (e = cudaStreamWaitEvent(s, mlane->join, 0)) != cudaSuccess) return fail("fm_overfit_step: join", e);
   return 0;
 }

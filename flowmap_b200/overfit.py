@@ -418,13 +418,13 @@ class FusedOverfitter:
         a.depth = _ptr(self._depth)
         a.weight_logits = _ptr(self._wlog) if cfg.use_correspondence_weights else None
         a.weight_sensitivity = cfg.weight_sensitivity
-        a.focal, a.k4 = _ptr(self._focal), _ptr(self._k4)
+        a.focal, a.k4 = _ptr(self._focal), _ptr(self._k4)  # a sweep step's calls pass the sweep's estimate
         a.fflow, a.bflow = _ptr(self.flows.forward), _ptr(self.flows.backward)
         a.fmask, a.bmask = _ptr(self.flows.forward_mask), _ptr(self.flows.backward_mask)
         a.mask_sum = _ptr(self._msum)
         a.mapping, a.delta, a.flow_weight = ops.MAPPINGS[cfg.mapping], cfg.delta, cfg.flow_weight
         (a.m_depth, a.v_depth, a.m_weights, a.v_weights, a.m_focal, a.v_focal) = [_ptr(t) for t in self._state]
-        a.lr, a.beta1, a.beta2, a.eps = cfg.lr, 0.9, 0.999, 1e-8
+        a.beta1, a.beta2, a.eps = 0.9, 0.999, 1e-8
         a.g_depth, a.g_weights = _ptr(self._g_depth), _ptr(self._g_w)
         a.g_focal, a.g_k4 = _ptr(self._g_focal), _ptr(self._g_k4)
         a.rt, a.loss, a.ws = _ptr(self.rt), _ptr(self._loss), _ptr(self._ws)
@@ -466,10 +466,15 @@ class FusedOverfitter:
             return t.view(self.B, -1, *t.shape[1:])
         return [t[f0 - pairs * i:f0 - pairs * i + f - pairs] for i, (f0, f) in enumerate(zip(self._first, self.frames))]
 
-    def _call_step(self, what: str = "fm_overfit_step"):
-        from ._lib import check
+    def _call_step(self, what: str = "fm_overfit_step", **fields):
+        """Run the step on a copy of _args with this call's `fields` (phase, tracks, step, defer_adam, focal, ...)
+        set: _args holds what every call shares, and no call leaves a field behind for the next one."""
+        from ._lib import OverfitStepArgs, check
+        args = OverfitStepArgs.from_buffer_copy(self._args)
+        for name, value in fields.items():
+            setattr(args, name, value)
         st = torch.cuda.current_stream().cuda_stream
-        a = self._ctypes.byref(self._args)
+        a = self._ctypes.byref(args)
         if self._layout is not None:
             check(self._lib.fm_overfit_step_videos(a, self._layout_ref, st), what)
         else:
@@ -639,10 +644,11 @@ class FusedOverfitter:
         elif self._softmin and self.global_step == self.cfg.regression_after:
             self._focal.copy_(torch.stack(self._window(split)).mean(0))
 
-    def _step_softmin(self, update: bool):
+    def _step_softmin(self, update: bool, **fields):
         """Sweep stage (intrinsics_softmin.py:84-141): focal estimate from the candidate sweep,
-        the step itself with that focal length, the sweep's backward, then Adam."""
-        c, a = self.cfg, self._args
+        the step itself with that focal length, the sweep's backward, then Adam.  `fields`: the step's
+        tracks and metrics_log."""
+        c = self.cfg
         f, w = max(self.frames), self._hw[1]
         st = torch.cuda.current_stream().cuda_stream
         # All-pixel Procrustes: the moment pass of the step does not have to wait for the focal length
@@ -659,20 +665,13 @@ class FusedOverfitter:
                 self._sweep_forward(idx, torch.cuda.current_stream().cuda_stream)
             if early_moments:
                 cur.wait_stream(self._side_stream)
-            a.moments_k4 = _ptr(self._k4_base) if early_moments else None
             # all-pixel dense path: the logits of pairs >= 1 are updated inside the step (their
             # gradient is final there); depth and pair 0 wait for the sweep's backward
             # (one video only: the fused update defers pair 0 of the batch, not pair 0 of every video)
             fuse = (update and c.use_correspondence_weights and self._indices is None and w % 4 == 0 and
                     self._layout is None)
-            a.focal = _ptr(self._sw_focal)
-            a.step = 1 if fuse else 0  # on / off: the bias corrections come from the step clock
-            a.defer_adam = 1 if fuse else 0
-            try:
-                self._call_step()
-            finally:
-                a.moments_k4 = None
-            a.defer_adam = 0
+            self._call_step(focal=_ptr(self._sw_focal), step=int(fuse), defer_adam=int(fuse),
+                            moments_k4=_ptr(self._k4_base) if early_moments else None, **fields)
             # The sweep's backward only touches the gradients of frames 0 / 1 (the candidate Procrustes
             # runs on the first pair): the depth update of every other frame runs beside it on a second
             # stream (a parallel branch of the captured step), frames 0 / 1 follow the sweep.
@@ -704,7 +703,6 @@ class FusedOverfitter:
         poses and every video's tracking loss (track_losses()) to this half."""
         if not self._network:
             self._refuse_videos("the split-step surface")
-        a = self._args
         f, (h, w) = self.frames[0], self._hw
         if self._network:
             self._bind_inputs(depth, weights, f, h, w)
@@ -713,28 +711,24 @@ class FusedOverfitter:
         st = torch.cuda.current_stream().cuda_stream
         self.global_step = global_step
         self._begin_step()
-        a.tracks, a.step, a.defer_adam = None, 0, 0
+        tracks = None
         if tracking:
             if not self._net_videos or self._packed is None:
                 raise ValueError("flowmap_b200: forward_phase(tracking=True) serves B networks' videos with tracks")
-            a.tracks = self._ctypes.pointer(self._pk_c)
+            tracks = self._ctypes.pointer(self._pk_c)
         self._sweep_idx = None
         with torch.cuda.device(self.rt.device):
             if self._softmin_stage():
                 self._sweep_idx = self._sweep_indices(split=True)
                 self._sweep_forward(self._sweep_idx, st)
-                a.focal = _ptr(self._sw_focal)
+                focal = self._sw_focal
                 if training:
                     self._append_window(split=True)
             else:
                 if training:
                     self._hand_over(split=True)
-                a.focal = _ptr(self._focal)
-            a.phase = 1  # FM_STEP_FORWARD
-            try:
-                self._call_step("fm_overfit_step (forward)")
-            finally:
-                a.phase, a.tracks = 0, None
+                focal = self._focal
+            self._call_step("fm_overfit_step (forward)", phase=1, tracks=tracks, focal=_ptr(focal))  # FM_STEP_FORWARD
         return self._loss
 
     def track_losses(self) -> Tensor:
@@ -782,22 +776,14 @@ class FusedOverfitter:
         d total / d loss_b per video.  Leaves the gradients in gradients()."""
         if not self._network:
             self._refuse_videos("the split-step surface")
-        a = self._args
         st = torch.cuda.current_stream().cuda_stream
-        a.tracks = self._ctypes.pointer(self._pk_c) if with_tracking else None
-        a.flow_grad_scale, a.track_grad_scale = _ptr(flow_scale), _ptr(track_scale)
-        a.phase, a.step, a.defer_adam = 2, 0, 0  # FM_STEP_BACKWARD
         # Without tracks this phase adds g_rt / track_g_k4 as a caller's pose / intrinsics gradient: a step
         # whose tracking loss is not enabled yet (loss.py:40-41) has none, whatever those buffers hold.
-        kept = a.g_rt, a.track_g_k4
-        if not with_tracking:
-            a.g_rt = a.track_g_k4 = None
+        tracking = (dict(tracks=self._ctypes.pointer(self._pk_c)) if with_tracking else
+                    dict(g_rt=None, track_g_k4=None))
         with torch.cuda.device(self.rt.device):
-            try:
-                self._call_step("fm_overfit_step (backward)")
-            finally:
-                a.phase, a.tracks, a.flow_grad_scale, a.track_grad_scale = 0, None, None, None
-                a.g_rt, a.track_g_k4 = kept
+            self._call_step("fm_overfit_step (backward)", phase=2,  # FM_STEP_BACKWARD
+                            flow_grad_scale=_ptr(flow_scale), track_grad_scale=_ptr(track_scale), **tracking)
             if self._sweep_idx is not None:
                 self._sweep_backward(self._sweep_idx, st)
 
@@ -807,23 +793,16 @@ class FusedOverfitter:
 
     def _step_body(self, update: bool, track_on: bool, sweep: bool):
         """One step as a fixed launch sequence (no host-side step numbers: see ops.StepClock)."""
-        from ._lib import check
-        a = self._args
         if update:
             self._clock.tick(tick_focal=not sweep and not self._gt)
-        a.tracks = self._ctypes.pointer(self._pk_c) if track_on else None
-        # the metrics row is indexed by the step clock, which only update steps advance
-        a.metrics_log = self._mlog.data_ptr() if (update and self._mlog is not None) else None
-        try:
-            if sweep:
-                self._step_softmin(update)
-            else:
-                a.focal = _ptr(self._focal)
-                a.step = a.focal_step = 1 if update else 0  # on / off: the step clock carries the counts
-                with torch.cuda.device(self.rt.device):
-                    self._call_step()
-        finally:
-            a.metrics_log = None
+        fields = dict(tracks=self._ctypes.pointer(self._pk_c) if track_on else None,
+                      # the metrics row is indexed by the step clock, which only update steps advance
+                      metrics_log=self._mlog.data_ptr() if (update and self._mlog is not None) else None)
+        if sweep:
+            self._step_softmin(update, **fields)
+        else:
+            with torch.cuda.device(self.rt.device):
+                self._call_step(step=int(update), **fields)
         if track_on:
             torch.add(self._loss, self._track_loss, out=self._total)
         else:
@@ -1084,7 +1063,6 @@ class ShardedFusedOverfitter(FusedOverfitter):
         super().__init__(replace(cfg, use_tracking=False), batch, flows, None, device)
         self.cfg = cfg
         self.plan, self.group = plan, group
-        self._args.clock = None  # this driver passes Adam's step numbers by value
         _, f_local, _, h, w = batch.videos.shape
         if f_local != plan.num_local_frames:
             raise ValueError("flowmap_b200: batch does not match the shard plan")
@@ -1172,22 +1150,12 @@ class ShardedFusedOverfitter(FusedOverfitter):
         """Flow loss with a regressed focal length, update step, as a fixed launch sequence: the step
         (weight-logit Adam fused in), the exchange started, Adam on the interior depth frames WHILE the
         boundary frames and the two scalars travel, then the boundary frames and the focal length."""
-        from ._lib import check
-        c, a, p, r = self.cfg, self._args, self.plan, self.reducer
+        p, r = self.plan, self.reducer
         clk = self._clock
         clk.tick(tick_focal=True)
-        a.clock, a.tracks, a.step, a.focal_step, a.defer_adam, a.phase = clk.ptr, None, 1, 1, 2, 0
-        a.focal = _ptr(self._focal)
-        # the step writes its two scalars (loss, d focal) straight into the all-reduce buffer
-        loss_ptr, gf_ptr = a.loss, a.g_focal
-        a.loss, a.g_focal = r.scal[0:1].data_ptr(), r.scal[1:2].data_ptr()
-        try:
-            with torch.cuda.device(self.rt.device):
-                check(self._lib.fm_overfit_step(self._ctypes.byref(a), torch.cuda.current_stream().cuda_stream),
-                      "fm_overfit_step")
-        finally:
-            a.clock, a.step, a.focal_step, a.defer_adam = None, 0, 0, 0
-            a.loss, a.g_focal = loss_ptr, gf_ptr
+        with torch.cuda.device(self.rt.device):
+            # the step writes its two scalars (loss, d focal) straight into the all-reduce buffer
+            self._call_step(step=1, defer_adam=2, loss=r.scal[0:1].data_ptr(), g_focal=r.scal[1:2].data_ptr())
         reqs = r.start(self._g_depth)
         stt, n = self._state, self._depth.shape[0]
         lo, hi = int(p.has_left and p.world > 1), n - int(p.has_right and p.world > 1)
@@ -1204,8 +1172,7 @@ class ShardedFusedOverfitter(FusedOverfitter):
 
     def training_step(self, update: bool = True):
         import torch.distributed as dist
-        from ._lib import check
-        c, a, p, L = self.cfg, self._args, self.plan, self._lib
+        c, p = self.cfg, self.plan
         _, _, _, h, w = self.batch.videos.shape
         self._begin_step()
         if (update and not self._softmin and not c.procrustes_randomize and self._indices is None and
@@ -1227,9 +1194,10 @@ class ShardedFusedOverfitter(FusedOverfitter):
         # (all pairs, or pairs >= 1 on the rank whose sweep still touches pair 0); depth and the
         # focal length wait for the exchange below
         fuse_w = update and c.use_correspondence_weights and self._indices is None and w % 4 == 0
-        a.tracks = None
-        a.step = self.optimizer_steps + 1 if fuse_w else 0
-        a.defer_adam = (1 if own_sweep else 2) if fuse_w else 0
+        if update:
+            self._clock.set(self.optimizer_steps, self.focal_steps)
+            self._clock.tick(tick_focal=not sweep)
+        fields = dict(step=int(fuse_w), defer_adam=(1 if own_sweep else 2) if fuse_w else 0)
         if sweep:
             if own_sweep:
                 idx = self._sweep_indices()
@@ -1237,23 +1205,18 @@ class ShardedFusedOverfitter(FusedOverfitter):
                     self._sweep_forward(idx, st)
             if p.world > 1:
                 dist.broadcast(self._sw_focal, src=self._first_rank(), group=self.group)
-            a.focal = _ptr(self._sw_focal)
-        else:
-            a.focal = _ptr(self._focal)
-            if update:
-                self._hand_over()  # identical on all ranks
+            fields["focal"] = _ptr(self._sw_focal)
+        elif update:
+            self._hand_over()  # identical on all ranks
         extra_focal = None
         with torch.cuda.device(dev):
             if track_on:
-                a.phase = 1  # FM_STEP_FORWARD
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (forward)")
+                self._call_step("fm_overfit_step (forward)", phase=1, **fields)  # FM_STEP_FORWARD
                 extra_focal = self._tracking_exchange(h, w)
-                a.phase, a.g_rt, a.track_g_k4 = 2, _ptr(self._g_rt_local), None  # FM_STEP_BACKWARD
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step (backward)")
-                a.phase, a.g_rt = 0, None
+                self._call_step("fm_overfit_step (backward)", phase=2, g_rt=_ptr(self._g_rt_local),  # FM_STEP_BACKWARD
+                                track_g_k4=None, **fields)
             else:
-                check(L.fm_overfit_step(self._ctypes.byref(a), st), "fm_overfit_step")
-        a.step, a.defer_adam = 0, 0
+                self._call_step(**fields)
         g_focal = self._g_focal.reshape(())
         if extra_focal is not None and p.rank == 0:  # global value, counted once
             g_focal = g_focal + extra_focal
@@ -1263,17 +1226,16 @@ class ShardedFusedOverfitter(FusedOverfitter):
             with torch.cuda.device(dev):
                 self._sweep_backward(idx, st)
         if update:
-            s_ = self.optimizer_steps + 1
-            stt = self._state
-            ops.adam_step(self._depth, self._g_depth, stt[0], stt[1], s_, c.lr)
+            stt, clk = self._state, self._clock
+            ops.adam_step_clock(self._depth, self._g_depth, stt[0], stt[1], clk)
             if c.use_correspondence_weights and (not fuse_w or own_sweep):
                 k = 1 if fuse_w else self._wlog.shape[0]  # pair 0 only when the rest was fused
-                ops.adam_step(self._wlog[:k], self._g_w[:k], stt[2][:k], stt[3][:k], s_, c.lr)
+                ops.adam_step_clock(self._wlog[:k], self._g_w[:k], stt[2][:k], stt[3][:k], clk)
             self._append_window()
             if not sweep:
                 self.focal_steps += 1
-                ops.adam_step(self._focal.reshape(1), self._g_focal.reshape(1), stt[4].reshape(1),
-                              stt[5].reshape(1), self.focal_steps, c.lr)
+                ops.adam_step_clock(self._focal.reshape(1), self._g_focal.reshape(1), stt[4].reshape(1),
+                                    stt[5].reshape(1), clk, focal_clock=True)
             self.global_step += 1
             self.optimizer_steps += 1
         total = red[0] + self._track_loss if track_on else red[0]

@@ -272,7 +272,7 @@ typedef struct {
  * (no focal gradient).  focal == NULL together with g_k4 == NULL and track_g_k4 == NULL is the
  * constant-intrinsics step (intrinsics_ground_truth.py: K given per frame, e.g. calibrated data): it
  * computes no intrinsics gradient at all -- the Procrustes backward and the tracking sweep run without
- * their K accumulators; g_k4 == NULL with a focal parameter or a track_g_k4 is refused.  step <= 0
+ * their K accumulators; g_k4 == NULL with a focal parameter or a track_g_k4 is refused.  step = 0
  * computes loss and gradients but skips Adam.
  * Gradients of the step are left in g_depth / g_weights / g_focal / g_k4. */
 typedef struct {
@@ -291,22 +291,20 @@ typedef struct {
   const fm_packed_tracks* tracks; /* host struct with device pointers, or NULL    */
   float track_weight;
   float *m_depth, *v_depth, *m_weights, *v_weights, *m_focal, *v_focal;
-  double lr, beta1, beta2, eps;
-  int step;                     /* 1-based Adam step number                        */
+  double beta1, beta2, eps;
+  int step;                     /* 1: update the parameters with Adam, on the bias corrections of `clock`'s
+                                   current tick (needs a clock); 0: no update.  Other values are refused. */
   float *g_depth, *g_weights, *g_focal, *g_k4;  /* gradient buffers (written)     */
   float *rt, *loss;             /* outputs: (F-1,3,4) poses, flow loss             */
   float *extrinsics, *g_extrinsics, *g_rt, *track_g_k4, *track_loss; /* tracking only */
   void *ws, *track_ws;
-  int focal_step;               /* Adam step number of the focal parameter (0: same as step);
-                                   differs after the softmin -> regressed hand-over, where the
-                                   focal length first receives a gradient at step after_step */
-  int defer_adam;               /* 0: Adam on everything inside the step.  1 (softmin stage): the sweep's
-                                   backward (fm_softmin_sweep_bwd) still has to add its gradients to depth
-                                   frames 0/1 and to the weights of pair 0, so only the weight logits of
-                                   pairs >= 1 are updated here (with `step`); the caller runs Adam on depth
-                                   and on pair 0's logits afterwards.  2 (pair sharding): the weight logits
-                                   of ALL pairs are updated here (their gradient is rank-local and final),
-                                   depth and focal length wait for the caller's collective */
+  int defer_adam;               /* With step = 1.  0: Adam on everything inside the step.  1 (softmin stage):
+                                   the sweep's backward (fm_softmin_sweep_bwd) still has to add its gradients
+                                   to depth frames 0/1 and to the weights of pair 0, so only the weight logits
+                                   of pairs >= 1 are updated here; the caller runs Adam on depth and on pair
+                                   0's logits afterwards.  2 (pair sharding): the weight logits of ALL pairs
+                                   are updated here (their gradient is rank-local and final), depth and focal
+                                   length wait for the caller's collective */
   int phase;                    /* FM_STEP_ALL, or a split step (pair sharding with a tracking loss; the
                                    autograd drop-in surface, where the losses' values are needed before
                                    backward() runs): FM_STEP_FORWARD computes rt, the flow loss with its
@@ -318,10 +316,11 @@ typedef struct {
                                    the two halves' common use (no parameter may change in between) */
   const float* flow_grad_scale;  /* FM_STEP_BACKWARD only: device scalars d total / d flow loss and     */
   const float* track_grad_scale; /* d total / d tracking loss (autograd's grad_output), or NULL (= 1) */
-  const void* clock;             /* device step clock (fm_step_clock_tick) or NULL.  With a clock the Adam
-                                    bias corrections come from it instead of `step` / `focal_step`
-                                    (which then only switch the update on), so that consecutive steps
-                                    are launches with identical arguments: a CUDA graph can replay them */
+  const void* clock;             /* device step clock (fm_step_clock_tick), the caller ticks it before an
+                                    update step; NULL only with step = 0.  Adam's bias corrections come from
+                                    its current tick (the focal length's from its own focal count), so that
+                                    consecutive steps are launches with identical arguments: a CUDA graph
+                                    can replay them */
   const float* moments_k4;       /* NULL, or the intrinsics (F,4) with which fm_procrustes_moments has ALREADY
                                     accumulated this step's moment sums into `ws` (all-pixel Procrustes only;
                                     same principal points as k4, any focal lengths): the step then starts at the
@@ -382,7 +381,7 @@ typedef struct {
  * segments of video b carry start frames frame_offset[b] + s (they never cross videos); track_ws is
  * fm_track_workspace_bytes(T, total_samples).  Metrics: gt_positions (T, 3), NaN first position of a
  * video = no ground truth; the ring is (metrics_capacity, B, 5).  ws: fm_workspace_bytes_videos(B, T).
- * Refuses defer_adam = 1 together with step > 0 and weight logits (the caller updates the logits after
+ * Refuses defer_adam = 1 together with step = 1 and weight logits (the caller updates the logits after
  * the sweep's backward).
  * Phases: FM_STEP_ALL, or the two halves of a split step, FM_STEP_FORWARD then FM_STEP_BACKWARD (a network
  * backbone's batch, whose depths / weights come from the network and whose update the caller owns).  A

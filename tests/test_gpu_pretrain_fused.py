@@ -9,7 +9,7 @@ the next, so that a per-video normaliser or a mix-up of videos shows.  Checked: 
 gradient of every network parameter and each video's d loss / d depths and d loss / d weights), those input
 gradients against the float64 oracle, the pooled loss against one-video fused steps, grad_output scales and
 accumulation, a six-step Adam run on a new batch every step, the per-op fall-backs and the refusals of the C
-ABI's packed split step."""
+ABI's packed split step and of its step switch."""
 import copy
 import ctypes
 
@@ -307,17 +307,31 @@ def test_packed_split_step_refusals():
     _, _, out, _ = _step(model, losses, batch, flows, fused=True)
     assert _is_fused(out, 2)
     eng = out.__dict__["_fused"].engine
-    a = eng._args
     tracks = PackedTracksC()
     log = torch.zeros(4, 2, 5, device="cuda:0")
     for phase in (1, 2):
         for field, value, match in (("tracks", ctypes.pointer(tracks), "takes no tracks"),
                                     ("step", 1, "updates no parameter"), ("defer_adam", 1, "updates no parameter"),
                                     ("metrics_log", log.data_ptr(), "no metrics log")):
-            a.phase = phase
-            setattr(a, field, value)
-            try:
-                with pytest.raises(FlowmapLibraryError, match=match):
-                    eng._call_step("fm_overfit_step_videos")
-            finally:  # what every split step of the engine passes
-                a.phase, a.tracks, a.step, a.defer_adam, a.metrics_log = 0, None, 0, 0, None
+            with pytest.raises(FlowmapLibraryError, match=match):
+                eng._call_step("fm_overfit_step_videos", phase=phase, **{field: value})
+
+
+def test_step_switch_refusals():
+    """The C ABI's `step` switches the update off (0) or on (1), and an update takes Adam's bias corrections
+    from the step clock: fm_overfit_step refuses step = 1 without a clock and step = 2, before any launch."""
+    from flowmap_b200._lib import FlowmapLibraryError, lib
+    from flowmap_b200.overfit import FusedOverfitter, OverfitCfg
+    from flowmap_b200.types import Batch
+    f, h, w = 4, 16, 24
+    dev = torch.device("cuda:0")
+    batch = Batch(torch.zeros(1, f, 3, h, w, device=dev), torch.arange(f, device=dev)[None], ["s"], ["d"])
+    o = FusedOverfitter(OverfitCfg(), batch, _flows(1, f, h, w, 0).to(dev), device=dev)
+    assert o._args.clock is not None
+    torch.cuda.synchronize()
+    for fields, match in (({"step": 1, "clock": None}, "needs the step clock"),
+                          ({"step": 2}, r"off \(0\) or on \(1\)")):
+        n0 = lib().fm_launch_count()
+        with pytest.raises(FlowmapLibraryError, match=match):
+            o._call_step(**fields)
+        assert lib().fm_launch_count() == n0, fields
